@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """bench.py -- PointFlow iterations / second on synthetic DTU-shaped input.
 
-    python bench.py --gpus N --steps K --warmup W            # this repo's sm_100a path
+    python bench.py --gpus N --steps K --warmup W            # this repo's sm_90a (H100) path
+    python bench.py ... --dump-outputs DIR                   # + the last timed step's outputs as DIR/<name>.npy
     python bench.py --impl reference --gpus N --steps K ...  # the reference algorithm on host cores
 
 A "step" is one pass of the hot path (the 3-iteration point_flow loop, reference
@@ -37,6 +38,10 @@ CONFIGS = {
 IMG_SCALES = (0.125, 0.25, 0.5)      # config.py:70
 INTER_SCALES = (1.0, 0.75, 0.15)     # config.py:71
 METRIC = "PointFlow iters/sec"
+# NVIDIA's data sheet for the H100 SXM (700 W): the denominators of the roofline fields
+H100_HBM_GBS = 3350.0
+H100_TF32_TFLOPS = 495.0
+DUMP_BUDGET_BYTES = 64 << 20
 
 
 def load_pretrained_hot_path_weights():
@@ -108,6 +113,33 @@ def algorithmic_bytes_per_pass(H, W, V, B=1):
     return out
 
 
+def dump_outputs(directory, arrays, budget=DUMP_BUDGET_BYTES):
+    """Writes each tensor of `arrays` as directory/<name>.npy (float32).  When all of them together exceed `budget`
+    bytes, every array is cut to the same share of its elements: a sorted sample of flat indices drawn with a fixed
+    seed, so that two runs with the same arguments store the same elements."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    host = {k: v.detach().to("cpu", torch.float32).numpy() for k, v in arrays.items()}
+    total = sum(a.nbytes for a in host.values())
+    for name, a in sorted(host.items()):
+        if total > budget:
+            keep = max(1, int(a.size * (budget / total)))
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=keep, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(directory, name + ".npy"), np.ascontiguousarray(a))
+
+
+def gpu_name_and_power_limit(local_gpu):
+    """The card the numbers belong to: name and power limit in watts (None when nvidia-smi is unavailable)."""
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(local_gpu), "--query-gpu=name,power.limit",
+                              "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=20).stdout
+        name, watts = [x.strip() for x in out.strip().splitlines()[0].split(",")]
+        return {"name": name, "power_limit_w": float(watts)}
+    except Exception:
+        return {"name": torch.cuda.get_device_name(local_gpu), "power_limit_w": None}
+
+
 def sample_clocks_start(local_gpu):
     try:
         f = tempfile.NamedTemporaryFile("w+", suffix=".csv", delete=False)
@@ -162,8 +194,7 @@ def sample_clocks_stop(p, f):
 # --------------------------------------------------------------------------------------
 def cpu_reference_pass(cfg_name, steps, warmup, budget_s=200.0):
     """Times the reference algorithm (oracle/pointflow_oracle.py, a restatement of the
-    reference's Python; /root/reference itself does not exist on the GPU box) on the host
-    cores.  A step is ALWAYS one whole 3-iteration pass of the same workload (same inputs, same
+    reference's Python) on the host cores.  A step is ALWAYS one whole 3-iteration pass of the same workload (same inputs, same
     pretrained weights); when `steps + warmup` passes do not fit the time budget, FEWER passes are
     timed (never a part of a pass) and the count actually timed is returned.
     Returns (iters_per_s, ms_per_step, info)."""
@@ -181,8 +212,8 @@ def cpu_reference_pass(cfg_name, steps, warmup, budget_s=200.0):
                               inp["mean"], inp["std"], inp["img_hw"], params, img_scales=sc, inter_scales=it)
 
     # Give the reference its best thread count: PyTorch's CPU kernels on these per-call tensors
-    # get slower with too many threads (all 128 host threads are ~10x slower than 16 on the B200 host), so
-    # iteration 1 is timed at a few pool sizes and the fastest is kept; `cores` reports it.
+    # get slower with too many threads, so iteration 1 is timed at a few pool sizes and the
+    # fastest is kept; `cores` reports it.
     t_begin = time.time()
     best = None
     for nt in sorted({t for t in (8, 16, 32, 64, cores) if t <= cores}):
@@ -279,8 +310,8 @@ def run_ours(args):
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
-        # NCCL_DEBUG=VERSION (this image's default) makes NCCL print a banner on stdout; stdout must
-        # carry ONE JSON line, so the banner is switched off (any other explicit level is kept)
+        # NCCL_DEBUG=VERSION makes NCCL print a banner on stdout; stdout must carry ONE JSON line,
+        # so the banner is switched off (any other explicit level is kept)
         if os.environ.get("NCCL_DEBUG", "").upper() == "VERSION":
             del os.environ["NCCL_DEBUG"]
         dist.init_process_group("nccl", device_id=dev)
@@ -318,7 +349,7 @@ def run_ours(args):
     h_f, w_f = set_a[0].outs[-1][0].shape[-2:]
     final_depths = torch.empty(G, 1, h_f, w_f, device=dev)   # the step's result: G final depth maps
     gathered = [torch.empty_like(final_depths) for _ in range(world)] if world > 1 else None
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # several times the 50 MB L2 of an H100
     stream = torch.cuda.current_stream(dev)
     side = [torch.cuda.Stream(device=dev) for _ in range(G)]
 
@@ -368,6 +399,15 @@ def run_ours(args):
     clocks = sample_clocks_stop(clk_p, clk_f) if rank == 0 else None
     ms_per_step = total_ms / args.steps
     value = world * G * n_iter / (ms_per_step / 1e3)
+    if args.dump_outputs and rank == 0:
+        # what the last timed step left in the captured passes' output buffers: per view in flight and iteration the
+        # refined depth map and the probability map (PointFlowPass.outs), and the step's result `final_depths`
+        arrays = {"final_depths": final_depths}
+        for g in range(G):
+            for i, (depth, prob) in enumerate(set_a[g].outs):
+                arrays["view%d_flow%d_depth" % (g, i + 1)] = depth
+                arrays["view%d_flow%d_prob" % (g, i + 1)] = prob
+        dump_outputs(args.dump_outputs, arrays)
 
     # ---- end-to-end: host buffers in, host result out, copies inside the timed region -----
     # Two sets of captured graphs with their own static input buffers alternate; the H2D copies of
@@ -459,18 +499,8 @@ def run_ours(args):
         except Exception:
             by_size = None
         alg = algorithmic_bytes_per_pass(H, W, V)
-        peaks = {}
-        try:
-            peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        except Exception:
-            pass
-        hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s"
-        traffic = {}
-        try:
-            traffic = json.load(open(os.path.join(ROOT, "profiles", "dram_traffic.json")))
-        except Exception:
-            pass
+        hbm_peak = H100_HBM_GBS
+        peak_src = "H100 SXM data sheet, 3350 GB/s HBM3 (a rate the card is specified for, not one measured here)"
         kernel_table = {}
         tot = sum(a[0] for a in agg.values())
         for name, (ms, cnt) in sorted(agg.items(), key=lambda kv: -kv[1][0]):
@@ -482,21 +512,20 @@ def run_ours(args):
                                   "alg_GBps": round(gbps, 1) if gbps is not None else None,
                                   "hbm_frac": round(gbps / hbm_peak, 4) if gbps is not None else None}
         # tensor-pipe view of the contraction kernels: executed TF32 FLOPs (3 products per element
-        # for 3xTF32) over their summed time, against half the measured dense bf16 GEMM rate
-        # (kind::tf32 runs at half the bf16 rate; MEASURED_PEAKS.json has no TF32 figure)
+        # for 3xTF32) over their summed time, against the data-sheet dense TF32 rate
         gemm_ms = sum(ms for name, (ms, cnt) in agg.items() if name.startswith("gemm_")) / reps
         mac_per_pt = 136 * 64 + 32 * 64 + 64 * 128 + 224 * 64 + 64 * 64 + 64 * 16
         pts = sum(5 * int(H * sc) * int(W * sc) for sc in IMG_SCALES)
         mode = _lib.lib.pmvs_get_gemm_mode()
         flops = 2.0 * mac_per_pt * pts * (3 if mode == 3 else 1)
-        tf32_peak = float(peaks.get("bf16_tflops", 1590.0)) / 2.0
+        tf32_peak = H100_TF32_TFLOPS
         roofline_gemm = None
         if gemm_ms > 0 and mode != 0:
             ach = flops / (gemm_ms * 1e-3) / 1e12
-            roofline_gemm = {"kernels": "gemm_* (tcgen05 kind::tf32, mode %d)" % mode, "bound": "tensor",
+            roofline_gemm = {"kernels": "gemm_* (wgmma tf32, mode %d)" % mode, "bound": "tensor",
                              "achieved": round(ach, 1), "peak": round(tf32_peak, 1), "unit": "TFLOP/s",
                              "frac": round(ach / tf32_peak, 4), "ms_per_pass": round(gemm_ms, 4),
-                             "peak_source": "MEASURED_PEAKS.json bf16_tflops / 2 (TF32 runs at half the bf16 rate)",
+                             "peak_source": "H100 SXM data sheet, 495 TFLOP/s dense TF32 at the 700 W limit",
                              "note": "the contractions are memory bound (25 FLOP/B): see kernels[*].alg_GBps"}
         # SURVEY.md 8(d) stage rooflines: the stage's single-pass algorithmic bytes over the summed event time of
         # the kernels that implement it (the pyramid `transpose` launches and the BN running-statistics update are
@@ -523,9 +552,7 @@ def run_ours(args):
         dom_bytes_per_launch = alg.get(dom, (0, 1))[0] / max(1, alg.get(dom, (0, 1))[1])
         achieved = dom_bytes_per_launch / (dom_ms_per_launch * 1e-3) / 1e9
         roofline = {"kernel": dom, "bound": "hbm", "achieved": round(achieved, 1), "peak": hbm_peak, "unit": "GB/s",
-                    "frac": round(achieved / hbm_peak, 4), "traffic": traffic.get(dom),
-                    "traffic_source": ("static: ncu capture of one pass, profiles/dram_traffic.json (%s)" %
-                                       traffic.get("_capture", "see its _comment")) if traffic.get(dom) else None,
+                    "frac": round(achieved / hbm_peak, 4),
                     "numerator": "bytes this kernel must read + write once given its boundaries (DESIGN.md 3); the "
                                  "SURVEY 8(d) stage figures are in roofline_stage",
                     "peak_source": peak_src,
@@ -562,7 +589,7 @@ def run_ours(args):
                            "inside every timed step"},
             "gpu_launches": int(launches_per_pass * G * args.steps),
             "launches_per_step": int(launches_per_pass * G),
-            "clocks": clocks, "roofline": roofline, "roofline_stage": roofline_stage, "roofline_gemm": roofline_gemm,
+            "gpu": gpu_name_and_power_limit(local), "clocks": clocks, "roofline": roofline, "roofline_stage": roofline_stage, "roofline_gemm": roofline_gemm,
             "cpu_baseline": cpu_baseline,
             "kernels": kernel_table,
             "per_iteration_size": by_size,
@@ -754,20 +781,28 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=20)
-    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--warmup", type=int, default=3, help="untimed steps before the timed ones; at least 3 are always run")
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--config", default="C2", choices=sorted(CONFIGS))
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--views-in-flight", type=int, default=4,
-                    help="independent reference views whose passes run concurrently on one GPU (default 4: measured "
-                         "1 -> 2 -> 4 views = 1.00 / 1.11 / 1.17x the single-view rate at C2)")
+                    help="independent reference views whose passes run concurrently on one GPU (default 4)")
     ap.add_argument("--mode", default="fused", choices=["fused", "oplevel"],
                     help="fused: the PointFlow module (default); oplevel: the reference closure over the stand-alone "
                          "operators (what an unchanged model.py runs)")
     ap.add_argument("--parallel", default="views", choices=["views", "subcloud"],
                     help="views: whole reference views per GPU (throughput, default); subcloud: all GPUs refine ONE "
                          "view, iterations 2/3 split by sub-cloud (BASELINE C5, latency)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (per view in flight and iteration "
+                         "the depth and probability maps, and the final depth maps) as DIR/<name>.npy, float32.  Only the "
+                         "default arm (--impl ours --mode fused --parallel views) has it; with several GPUs rank 0 "
+                         "writes its own views")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and (args.impl != "ours" or args.mode != "fused" or args.parallel != "views"):
+        ap.error("--dump-outputs belongs to the default arm (--impl ours --mode fused --parallel views)")
     if args.impl == "reference":
         run_reference_arm(args)
     else:

@@ -1,5 +1,5 @@
 /*
- * pmvs_b200.h -- C ABI of libpmvs_b200.so, the sm_100a implementation of the
+ * pmvs_b200.h -- C ABI of libpmvs_b200.so, the sm_90a implementation of the
  * PointMVSNet PointFlow hot path (reference: callmeray/PointMVSNet @ cacb2d7).
  *
  * Conventions (all entry points):
@@ -47,7 +47,7 @@ const char* pmvs_last_error(void);
 /* number of kernels this library has launched since load (all threads, all devices) */
 unsigned long long pmvs_launch_count(void);
 
-/* Arithmetic of the per-point contractions (1x1 convolutions): 3 = tcgen05 kind::tf32 with
+/* Arithmetic of the per-point contractions (1x1 convolutions): 3 = wgmma tf32 with
  * error-compensated 3xTF32 (default, fp32-level accuracy), 1 = plain TF32 tensor cores,
  * 0 = fp32 SIMT FMA kernel.  Process-wide; not thread-safe against concurrent launches. */
 int pmvs_set_gemm_mode(int mode);
@@ -59,10 +59,10 @@ int pmvs_get_gemm_mode(void);
  *                   0 = 16 L2 gathers per point (the kernels the stand-alone EdgeConv operator uses)
  *   PMVS_OPT_KNN    1 = batched sorting network + bitonic merge (kernel_size 5, knn 16),
  *                   0 = sorted insertion (the kernel every other (kernel_size, knn) uses)
- *   PMVS_OPT_FETCH  1 = consecutive hypotheses share the texel quad, packed fp32 math (3 CTAs / SM),
- *                   2 = the same with 2 CTAs / SM and no register spills, 0 = 4 taps per (hypothesis, view)
+ *   PMVS_OPT_FETCH  1 = consecutive hypotheses share the texel quad, fp32 pair math (3 CTAs / SM),
+ *                   2 = the same with 2 CTAs / SM and a larger register budget, 0 = 4 taps per (hypothesis, view)
  *                   (the kernel used for V > 6)
- *   PMVS_OPT_GEMM   2 = weights in tensor memory, points as N, persistent, cp.async staging ring (4 chunks in
+ *   PMVS_OPT_GEMM   2 = weights stationary in shared memory, persistent, cp.async staging ring (2-3 chunks in
  *                   flight), 1 = the same kernel with register prefetch,
  *                   0 = points-as-M with shared-memory operands (the kernel plain-TF32 mode uses)
  *   PMVS_OPT_DEBUG_IDX  1 = also materialise int32 neighbour indices in the workspace */

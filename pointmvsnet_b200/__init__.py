@@ -1,4 +1,4 @@
-"""pointmvsnet_b200 -- sm_100a implementation of PointMVSNet's PointFlow hot path.
+"""pointmvsnet_b200 -- sm_90a implementation of PointMVSNet's PointFlow hot path.
 
 Mirrors the reference's import surface (pointmvsnet/model.py:8-12):
     pointmvsnet_b200.networks            EdgeConv, EdgeConvNoC
@@ -21,7 +21,7 @@ def install_as_pointmvsnet(reference_root=None):
     With ``reference_root`` (a checkout of callmeray/PointMVSNet) the rest of the
     reference package (model.py, dataset, config ...) is imported from there and only
     the hot-path modules are replaced, so the unchanged ``pointmvsnet/model.py`` runs on
-    the sm_100a kernels.  Without it, stub parent packages are created and every module
+    the sm_90a kernels.  Without it, stub parent packages are created and every module
     this package mirrors is aliased (enough for ``from pointmvsnet.utils.torch_utils
     import get_knn_3d`` style imports).  See INTEGRATION.md."""
     import importlib

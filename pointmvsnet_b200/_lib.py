@@ -15,7 +15,7 @@ LIB_PATH = os.path.join(_HERE, "libpmvs_b200.so")
 if not os.path.exists(LIB_PATH):
     raise ImportError(
         "pointmvsnet_b200: %s is missing -- build it with pointmvsnet_b200/csrc/build.sh "
-        "(nvcc, sm_100a).  There is no CPU fallback." % LIB_PATH)
+        "(nvcc, sm_90a).  There is no CPU fallback." % LIB_PATH)
 
 lib = C.CDLL(LIB_PATH)
 
@@ -104,7 +104,7 @@ def ptr(t):
 def require_cuda(*tensors):
     for t in tensors:
         if t is not None and not t.is_cuda:
-            raise RuntimeError("pointmvsnet_b200 operators need CUDA tensors (sm_100a); there is no CPU fallback")
+            raise RuntimeError("pointmvsnet_b200 operators need CUDA tensors (sm_90a); there is no CPU fallback")
 
 
 def f32c(t):

@@ -1,6 +1,6 @@
 """Coarse-stage plane sweep (reference pointmvsnet/model.py:54-113): fetch the per-view coarse
 features at the D depth-hypothesis planes of the reference view and reduce them to the variance cost
-volume the 3-D U-Net consumes - one fused sm_100a kernel instead of FeatureFetcher + three passes
+volume the 3-D U-Net consumes - one fused sm_90a kernel instead of FeatureFetcher + three passes
 over the [B,V,C,D*h*w] tensor (503 MB at 640x512, V=4, D=96).  This is the row immediately before the
 PointFlow path (SURVEY.md section 8f-1); the reference model calls it once per forward."""
 import torch

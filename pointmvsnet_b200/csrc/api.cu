@@ -29,7 +29,7 @@ static struct OptDefaults {
     g_opt[OPT_EDGE].store(1);   // TMA halo-tile EdgeConv
     g_opt[OPT_KNN].store(1);    // batched sorting-network kNN
     g_opt[OPT_FETCH].store(1);  // texel-quad sharing fetch
-    g_opt[OPT_GEMM].store(2);   // TMEM-stationary GEMM, cp.async staging ring
+    g_opt[OPT_GEMM].store(2);   // weight-stationary persistent GEMM, cp.async staging ring
   }
 } g_opt_defaults;
 int opt(int key) { return (key >= 0 && key < OPT_COUNT) ? g_opt[key].load(std::memory_order_relaxed) : 0; }
@@ -259,7 +259,7 @@ extern "C" int pmvs_pyramid_to_channels_last(const float* nchw, float* nhwc, int
 extern "C" int pmvs_idx64_to_idx32(const int64_t* in, int32_t* out, long long n, pmvs_stream_t stream) {
   PMVS_REQUIRE(in && out && n >= 0, "idx64_to_idx32: bad arguments");
   if (n == 0) return PMVS_OK;
-  idx_convert_kernel<<<(int)std::min<long long>(cdiv(n, 256), 148 * 8), 256, 0, (cudaStream_t)stream>>>(in, out, n);
+  idx_convert_kernel<<<(int)std::min<long long>(cdiv(n, 256), sm_count() * 8), 256, 0, (cudaStream_t)stream>>>(in, out, n);
   return check_launch("idx_convert_kernel");
 }
 
@@ -269,7 +269,7 @@ extern "C" int pmvs_gather_knn_forward(const float* input, const int64_t* index,
   const long long total = (long long)B * C * N * K;
   if (total == 0) return PMVS_OK;  // empty input: nothing to do (pointers may be NULL)
   PMVS_REQUIRE(input && index && output, "gather_knn_forward: NULL pointer");
-  const int grid = (int)std::min<long long>(cdiv(total, 256), 148 * 16);
+  const int grid = (int)std::min<long long>(cdiv(total, 256), sm_count() * 16);
   gather_fwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(input, index, output, C, N, K, total);
   return check_launch("gather_fwd_kernel");
 }
@@ -287,7 +287,7 @@ extern "C" int pmvs_gather_knn_backward(const float* grad_output, const int64_t*
   }
   const long long total = (long long)B * C * N * K;
   if (total == 0) return PMVS_OK;
-  const int grid = (int)std::min<long long>(cdiv(total, 256), 148 * 16);
+  const int grid = (int)std::min<long long>(cdiv(total, 256), sm_count() * 16);
   gather_bwd_kernel<<<grid, 256, 0, st>>>(grad_output, index, grad_input, C, N, K, total);
   return check_launch("gather_bwd_kernel");
 }

@@ -1,10 +1,10 @@
 #!/usr/bin/env bash
-# Builds libpmvs_b200.so (sm_100a only) next to the Python package.
+# Builds libpmvs_b200.so (sm_90a only) next to the Python package.
 set -euo pipefail
 HERE="$(cd "$(dirname "${BASH_SOURCE[0]}")" && pwd)"
 OUT="${PMVS_OUT:-${HERE}/../libpmvs_b200.so}"   # PMVS_OUT=<path> builds a side copy (experimental flags)
 NVCC="${NVCC:-/usr/local/cuda/bin/nvcc}"
-FLAGS=(-gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -shared
+FLAGS=(-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -shared
        --expt-relaxed-constexpr -Xptxas -v)
 "${NVCC}" "${FLAGS[@]}" -o "${OUT}" "${HERE}"/api.cu "${HERE}"/knn3d.cu "${HERE}"/fetch.cu "${HERE}"/edgeconv.cu "${HERE}"/gemm_tc.cu "${HERE}"/edge_tile.cu "${HERE}"/gemm_ws.cu "${HERE}"/gather_det.cu "$@"
 echo "built ${OUT}"

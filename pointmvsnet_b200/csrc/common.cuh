@@ -1,4 +1,4 @@
-// Shared helpers for libpmvs_b200 (sm_100a only).
+// Shared helpers for libpmvs_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -46,38 +46,29 @@ inline int check_launch(const char* what, cudaStream_t st = nullptr) {
 
 static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 
+// SMs of the current device, for grid sizing (132 on an H100; the devices of one process are alike)
+inline int sm_count() {
+  static int n = 0;
+  if (n == 0) {
+    int dev = 0, v = 0;
+    cudaGetDevice(&dev);
+    n = (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && v > 0) ? v : 132;
+  }
+  return n;
+}
+
 __device__ __forceinline__ float4 ldg4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
 __device__ __forceinline__ void st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
 
-// Packed fp32 pairs (sm_100a FFMA2 / FADD2 / FMUL2: IEEE rn per lane, i.e. bit-identical to the scalar
-// operations, two lanes per issue slot).
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 pack2(float a, float b) {
-  f32x2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
-  return r;
-}
-__device__ __forceinline__ void unpack2(f32x2 v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-  f32x2 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
-}
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ f32x2 sub2(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
+// fp32 pairs: two IEEE round-to-nearest operations per call, written with the intrinsics that are never contracted
+// (a mul2 followed by an add2 stays two roundings), so a pair computes bit for bit what the scalar code computes.
+typedef float2 f32x2;
+__device__ __forceinline__ f32x2 pack2(float a, float b) { return make_float2(a, b); }
+__device__ __forceinline__ void unpack2(f32x2 v, float& a, float& b) { a = v.x; b = v.y; }
+__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ f32x2 sub2(f32x2 a, f32x2 b) { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
 
 // ---- run-time implementation switches (pmvs_set_option; api.cu) -------------------------------
 enum {
@@ -85,7 +76,7 @@ enum {
                   // 2 = TMA halo tile 16x4x5
   OPT_KNN = 2,    // 0 = sorted insertion (round 1), 1 = batched sort + bitonic merge
   OPT_FETCH = 3,  // 0 = 4 taps per (hypothesis, view), 1 = hypotheses of a pixel share the texel quad when they can
-  OPT_GEMM = 4,   // 0 = points-as-M shared-memory operands (round 1), 1 = weights in TMEM, points as N, persistent
+  OPT_GEMM = 4,   // 0 = points-as-M shared-memory operands (round 1), 1 / 2 = weights stationary in shared memory, persistent (gemm_ws.cu)
   OPT_DEBUG_IDX = 5,  // 1 = the fused path also materialises the int32 neighbour indices (tests)
   OPT_COUNT = 16
 };
@@ -151,9 +142,9 @@ struct GemmArgs {
   double* out_stats;
 };
 int launch_gemm(const GemmArgs& a, cudaStream_t st);
-// tcgen05 path; returns -1 when it does not apply (shape / alignment / mode) so the caller falls back
+// wgmma path; returns -1 when it does not apply (shape / alignment / mode) so the caller falls back
 int launch_gemm_tc(const GemmArgs& a, cudaStream_t st, const char* name);
-// second-generation tcgen05 path (gemm_ws.cu: weights in tensor memory, persistent, warp-specialised); 3xTF32 only
+// second-generation wgmma path (gemm_ws.cu: weights stationary in shared memory, persistent, warp-specialised); 3xTF32 only
 int launch_gemm_ws(const GemmArgs& a, cudaStream_t st, const char* name);
 
 struct EdgeArgs {

@@ -173,7 +173,7 @@ __global__ void __launch_bounds__(ET_THREADS, 3) edge_tile_kernel(const __grid_c
       const float4 lc = loc[s];
       const bool esc = ((ca.x | ca.y | ca.z | ca.w | cb.x | cb.y | cb.z | cb.w) & 0x80008000u) != 0u;
       const float* hbase = halo + pb0 + s * LAYER;
-      f32x2 A_lo = 0ull, A_hi = 0ull, c_lo = 0ull, c_hi = 0ull, o_lo = pack2(0.f, 0.f), o_hi = o_lo;
+      f32x2 o_lo = pack2(0.f, 0.f), o_hi = o_lo, A_lo = o_lo, A_hi = o_lo, c_lo = o_lo, c_hi = o_lo;
       const f32x2 l_lo = pack2(lc.x, lc.y), l_hi = pack2(lc.z, lc.w);
       if (APPLY) {
         const float4 A4 = *reinterpret_cast<const float4*>(&coef[ch0 + cl]);
@@ -340,14 +340,10 @@ int launch_variant(const EdgeTileArgs& a, cudaStream_t st) {
   // instead of once per tile.
   static int slots = 0;
   if (slots == 0) {
-    int dev = 0, sms = 0;
-    cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
-    slots = 3 * sms;  // __launch_bounds__(ET_THREADS, 3)
+    slots = 3 * sm_count();  // __launch_bounds__(ET_THREADS, 3)
   }
   const int tiles_per_group = cdiv(a.gw, TX) * cdiv(a.gh, TY) * a.clouds_per_group;
-  // Measured (C2, one view): statistics 0.187 -> 0.178 ms (32 ch) and 0.153 -> 0.150 ms (64 ch) per pass; the apply
-  // kernel has no per-CTA flush to amortise and lost 5 % to the static tile assignment, so it keeps one tile per CTA.
+  // The apply kernel has no per-CTA flush to amortise, so it keeps one tile per CTA.
   int ctas = APPLY ? tiles_per_group : std::min(tiles_per_group, std::max(1, slots / a.groups));
   ctas = cdiv(tiles_per_group, cdiv(tiles_per_group, ctas));  // same longest walk with fewer CTAs
   PMVS_REQUIRE(ctas <= 0x7fffffff / 2, "edge_tile: too many tiles");
@@ -364,9 +360,8 @@ int launch_edge_tile(const EdgeTileArgs& a, int tile_w, cudaStream_t st) {
                "edge_tile: NULL pointer");
   PMVS_REQUIRE(a.cout == 32 || a.cout == 64, "edge_tile: out_channels %d (supported: 32, 64)", a.cout);
   PMVS_REQUIRE(a.gh > 0 && a.gw > 0 && a.groups > 0 && a.clouds_per_group > 0, "edge_tile: bad cloud shape");
-  // Measured and dropped (git history): a 16 x 4 x 5 tile with 2 CTAs / SM (25 % slower), and a ring variant - one
-  // persistent 21-warp CTA per SM, 3-deep ring of TMA boxes loaded two items ahead - which removed the TMA waits
-  // (23 % of the warp samples here) but ran 4-16 % slower at every iteration size: 20 consumer warps instead of 24.
+  // Tried and dropped before the H100 port (git history; not re-measured on H100): a 16 x 4 x 5 tile with 2 CTAs / SM,
+  // and a ring variant - one persistent 21-warp CTA per SM, 3-deep ring of TMA boxes loaded two items ahead.
   (void)tile_w;
   return a.cout == 32 ? launch_variant<32, APPLY, 8, 4>(a, st) : launch_variant<64, APPLY, 8, 4>(a, st);
 }

@@ -224,8 +224,8 @@ struct WarpSourceParams {
 
 __global__ void __launch_bounds__(256) warp_source_kernel(const WarpSourceParams p) {
   // grid: x = chunks of 256 float4s along one output row (w * 28 float4s, memory order: a warp writes 512 contiguous
-  // bytes), y = output row, z = b*V + v.  (A variant with level-uniform blocks - no per-thread level selects - measured
-  // 40 % slower: its stores are 64..256-byte pieces at a 448-byte pitch.)
+  // bytes), y = output row, z = b*V + v.  (A variant with level-uniform blocks - no per-thread level selects - was
+  // dropped: its stores are 64..256-byte pieces at a 448-byte pitch.)
   const int xi = blockIdx.x * 256 + threadIdx.x;
   if (xi >= p.w * FETCH_C4) return;
   const int x = xi / FETCH_C4, c4 = xi - x * FETCH_C4;
@@ -455,7 +455,7 @@ __global__ void __launch_bounds__(FETCH_WARPS * 32, MINB) fused_fetch_kernel(con
       // Views outermost.  Consecutive hypotheses of a pixel project ~0.1 texel apart along the epipolar line, so a
       // hypothesis usually hits the texel quad of the previous one: the 4 taps are then NOT re-loaded (a warp-uniform
       // test on the ballot of phase 1), about 1.4 quads per view instead of 5.  The arithmetic is the scalar kernel's
-      // on fp32 pairs (FMUL2 / FFMA2 / FADD2: IEEE rn per lane, so the results are bit-identical); per hypothesis the
+      // on fp32 pairs (common.cuh f32x2: IEEE rn per lane, so the results are bit-identical); per hypothesis the
       // views are still accumulated in view order.
       if (lane < FETCH_C4) {
         f32x2 s1l[PMVS_NUM_HYP], s1h[PMVS_NUM_HYP], s2l[PMVS_NUM_HYP], s2h[PMVS_NUM_HYP];
@@ -471,8 +471,10 @@ __global__ void __launch_bounds__(FETCH_WARPS * 32, MINB) fused_fetch_kernel(con
               const uint4 o = *reinterpret_cast<const uint4*>(dm->o);
               t0 = __ldg(src + o.x); t1 = __ldg(src + o.y); t2 = __ldg(src + o.z); t3 = __ldg(src + o.w);
             }
-            const ulonglong2 wa = *reinterpret_cast<const ulonglong2*>(dm->w);   // (w0,w0) (w1,w1)
-            const ulonglong2 wb = *reinterpret_cast<const ulonglong2*>(dm->wd);  // (w2,w2) (w3,w3)
+            const float4 wa4 = *reinterpret_cast<const float4*>(dm->w);   // (w0,w0) (w1,w1)
+            const float4 wb4 = *reinterpret_cast<const float4*>(dm->wd);  // (w2,w2) (w3,w3)
+            const struct { f32x2 x, y; } wa = {pack2(wa4.x, wa4.y), pack2(wa4.z, wa4.w)},
+                                         wb = {pack2(wb4.x, wb4.y), pack2(wb4.z, wb4.w)};
             // ATen grid_sampler_2d accumulation order: NW, NE, SW, SE
             const f32x2 al = fma2(pack2(t3.x, t3.y), wb.y, fma2(pack2(t2.x, t2.y), wb.x,
                                   fma2(pack2(t1.x, t1.y), wa.y, mul2(pack2(t0.x, t0.y), wa.x))));
@@ -660,7 +662,7 @@ int launch_fused_fetch(const FusedFetchParams& p0, cudaStream_t st) {
   p.rlog2 = -1;
   for (int q = 0; q < 16; ++q) if ((1 << q) == p.ratio) p.rlog2 = q;
   // several consecutive pixels of a row per warp once there are enough pixels to fill the machine
-  const long long per = npix / (148ll * FETCH_WARPS * 8);
+  const long long per = npix / ((long long)sm_count() * FETCH_WARPS * 8);
   p.ppw = per >= 4 ? 4 : (per >= 2 ? 2 : 1);
   dim3 grid(cdiv(p.w, 4 * p.ppw), cdiv(p.h, 2), p.B);  // CTA = (4 * ppw) x 2 pixels
   const size_t smem = fetch_smem_total(p.V);

@@ -195,7 +195,7 @@ extern "C" int pmvs_gather_knn_backward_det(const float* grad_output, const int6
   }
   const long long NK = (long long)N * K, entries = (long long)B * NK, rows = (long long)B * N;
   const long long outs = rows * C;
-  auto blocks = [](long long n) { return (int)std::min<long long>(std::max<long long>(cdiv(n, GD_THREADS), 1), 148 * 16); };
+  auto blocks = [](long long n) { return (int)std::min<long long>(std::max<long long>(cdiv(n, GD_THREADS), 1), sm_count() * 16); };
   if (entries > 0) {
     gd_count_kernel<<<blocks(entries), GD_THREADS, 0, st>>>(index, cnt, entries, N, NK);
     PMVS_TRY(check_launch("gd_count_kernel"));

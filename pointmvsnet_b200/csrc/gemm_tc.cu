@@ -1,109 +1,38 @@
-// tcgen05 (5th-gen tensor core) GEMM for the per-point contractions of EdgeConv / flow_mlp:
+// Warpgroup-MMA (wgmma) GEMM for the per-point contractions of EdgeConv / flow_mlp:
 //   Y[r, 0:N] = f(X[r, 0:K]) * W[0:N, 0:K]^T        r = points (rows), fp32 in / fp32 out
 // (reference: nn.Conv1d 1x1 in networks.py:13-14,22-23,51-52 and nn/conv.py:21-30 followed by
 // train-mode BatchNorm + ReLU, which is fused here as the INPUT transform of the next layer).
 //
 // The contraction is memory/latency bound (25 FLOP/B), so the kernel is organised for bytes in
-// flight rather than for MMA throughput: one CTA (256 threads) owns one 128-row tile, uses
-// ~40-70 KB of shared memory and 32-128 TMEM columns, and 3-4 CTAs are resident per SM, each in
-// a different phase (load / MMA / epilogue).  Per 32-column K chunk:
+// flight rather than for MMA throughput: one CTA (256 threads = two warpgroups) owns one 128-row
+// tile, uses ~40-70 KB of shared memory, and 3-4 CTAs are resident per SM, each in a different
+// phase (load / MMA / epilogue).  Per 32-column K chunk:
 //   all threads : coalesced 128-bit loads of the X slab (128 x 32 fp32) and of the W slab
 //                 (N x 32) into registers - issued BEFORE waiting for the previous chunk's MMA
-//   all threads : fused BatchNorm+ReLU, TF32 hi/lo split, stores in the UMMA K-major
-//                 SWIZZLE_128B layout, fence.proxy.async, __syncthreads
-//   one thread  : tcgen05.mma.cta_group::1.kind::tf32 (M=128, N, K=8) x ksteps, tcgen05.commit
-// Epilogue: all 8 warps tcgen05.ld the fp32 accumulator from TMEM, stage it through shared
-// memory, coalesced stores, per-column sum / sum-of-squares (BN statistics of the next layer)
-// reduced in fp64.
+//   all threads : fused BatchNorm+ReLU, TF32 hi/lo split, stores in the K-major SWIZZLE_128B
+//                 layout, fence.proxy.async, __syncthreads
+//   warpgroup w : wgmma.mma_async m64nNk8 tf32 x ksteps on rows [64 w, 64 w + 64), commit, wait
+// Epilogue: the fp32 accumulator fragments go from registers through shared memory to
+// coalesced stores; per-column sum / sum-of-squares (BN statistics of the next layer) reduced in fp64.
 //
-// Precision: kind::tf32 has a 10-bit mantissa (and truncates).  NSPLIT = 3 runs the error-
+// Precision: tf32 operands have a 10-bit mantissa.  NSPLIT = 3 runs the error-
 // compensated product A*B ~= Alo*Bhi + Ahi*Blo + Ahi*Bhi ("3xTF32", residuals exact in fp32),
 // which keeps fp32-level accuracy (measured in tests/test_gpu_parity.py); NSPLIT = 1 is plain TF32.
 #include <algorithm>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace pmvs {
 
 namespace tc {
 
-constexpr int BM = 128;            // rows per tile == UMMA M
+using namespace wg;
+
+constexpr int BM = 128;            // rows per tile: two warpgroups x wgmma M = 64
 constexpr int KC = 32;             // fp32 columns per K chunk == one 128-byte swizzle row
 constexpr int NUM_THREADS = 256;
 constexpr int A_PLANE_BYTES = BM * KC * 4;  // 16 KB
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done = 0;
-  while (!done) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-  }
-}
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::tf32, issued by ONE thread
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start
-// address >> 4 in bits [0,14), LBO (unused for swizzled K-major) = 1 in [16,30), SBO = 1024 B
-// (one 8-row x 128 B swizzle atom) >> 4 in [32,46), version 1 in [46,48), layout 2 in [61,64).
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) |
-         ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-}
-// instruction descriptor (cute::UMMA::InstrDescriptor): D = F32 (1 @ bit 4), A = B = TF32 (2 @ bits
-// 7 and 10), both K-major (bits 15, 16 = 0), N >> 3 at bit 17, M >> 4 at bit 24
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-template <int NC>
-__device__ __forceinline__ void tmem_ld(uint32_t taddr, float (&v)[NC]);
-template <>
-__device__ __forceinline__ void tmem_ld<32>(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-template <>
-__device__ __forceinline__ void tmem_ld<8>(uint32_t taddr, float (&v)[8]) {
-  uint32_t r[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
 
 // TF32 split: hi keeps the 10 explicit mantissa bits the tensor core reads, lo = x - hi (exact)
 __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
@@ -130,7 +59,7 @@ struct Smem {
   static constexpr int AB_BYTES = NPL * (A_PLANE_BYTES + B_PLANE_BYTES);
   static constexpr int D_BYTES = BM * D_PITCH * 4;
   static constexpr int MAIN_BYTES = AB_BYTES > D_BYTES ? AB_BYTES : D_BYTES;  // D staging aliases A/B
-  static constexpr int TOTAL = 1024 /*align slack*/ + MAIN_BYTES + 4 * 224 * 4 /*BN coeffs*/ + 64;
+  static constexpr int TOTAL = 1024 /*align slack*/ + MAIN_BYTES + 4 * 224 * 4 /*BN coeffs*/;
 };
 
 template <int N_OUT, int NSPLIT>
@@ -140,11 +69,12 @@ __global__ void __launch_bounds__(NUM_THREADS) gemm_tc_kernel(const GemmArgs a) 
   constexpr bool SPLIT = NSPLIT == 3;
   // 3xTF32 with N <= 64 stacks [Bhi ; Blo] into one N' = 2N operand: A_hi * [Bhi;Blo] is ONE MMA that
   // reads A_hi once (accumulator columns [0,N) = Ahi*Bhi, [N,2N) = Ahi*Blo), and A_lo * B_hi
-  // accumulates into [N,2N); the epilogue adds the two halves.  14 KB instead of 18 KB of
-  // shared-memory operand reads per k-step - the resource that bounds this kernel.
+  // accumulates into [N,2N); the epilogue adds the two halves, so the small terms are summed apart
+  // from the large one.  N = 128 keeps one accumulator (64 registers a thread).
   constexpr bool STACKED = SPLIT && N_OUT <= 64;
   constexpr int ACC_COLS = STACKED ? 2 * N_OUT : N_OUT;
-  constexpr int TMEM_COLS = ACC_COLS < 32 ? 32 : ACC_COLS;  // power of two >= 32
+  constexpr int ACC_REGS = ACC_COLS / 2;              // accumulator registers per thread (64 rows x ACC_COLS / 128 threads)
+  constexpr int BLK = N_OUT < 64 ? N_OUT : 64;        // one wgmma shape for every product into this accumulator (wgmma.cuh)
   constexpr int A_LD = BM * 8 / NUM_THREADS;          // float4 loads per thread per chunk (4)
   constexpr int B_LD = (N_OUT * 8 + NUM_THREADS - 1) / NUM_THREADS;
   extern __shared__ unsigned char smem_raw[];
@@ -153,30 +83,17 @@ __global__ void __launch_bounds__(NUM_THREADS) gemm_tc_kernel(const GemmArgs a) 
   unsigned char* sB = sA + NPL * A_PLANE_BYTES;              // [plane][N_OUT x 128 B swizzled]
   float* sD = (float*)smem;                                  // epilogue staging (aliases sA/sB)
   float* sBN = (float*)(smem + S::MAIN_BYTES);               // mean, istd, gamma, beta  x 224
-  uint64_t* bar = (uint64_t*)(sBN + 4 * 224);
-  uint32_t* tmem_slot = (uint32_t*)(bar + 1);
-  const uint32_t bar_mma = smem_u32(bar);
 
   const int K = a.cin;
   const int nch = (K + KC - 1) / KC;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wgi = warp >> 2;  // warpgroup: rows [64 * wgi, 64 * wgi + 64) of the tile
   const int g = blockIdx.y;
   const int row0 = blockIdx.x * BM;
   const int rows_valid = min(BM, a.rows_per_group - row0);
   const size_t grow0 = (size_t)g * a.rows_per_group + row0;
   const bool in_bn = a.in_stats != nullptr;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      mbar_init(bar_mma, 1);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "n"(TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   if (in_bn) {
     const double* s = a.in_stats + (size_t)g * 2 * K;
     for (int c = tid; c < K; c += NUM_THREADS) {
@@ -218,14 +135,14 @@ __global__ void __launch_bounds__(NUM_THREADS) gemm_tc_kernel(const GemmArgs a) 
         v.z = fmaxf(bn_apply(v.z, sBN[k0 + 2], sBN[224 + k0 + 2], sBN[448 + k0 + 2], sBN[672 + k0 + 2]), 0.f);
         v.w = fmaxf(bn_apply(v.w, sBN[k0 + 3], sBN[224 + k0 + 3], sBN[448 + k0 + 3], sBN[672 + k0 + 3]), 0.f);
       }
-      const int off = (r >> 3) * 1024 + (r & 7) * 128 + ((pc ^ (r & 7)) << 4);
+      const int off = swz128(r, pc);
       store_planes(sA, A_PLANE_BYTES, off, v, SPLIT);
     }
 #pragma unroll
     for (int i = 0; i < B_LD; ++i) {
       const int n = arow + 32 * i;
       if (n < N_OUT) {
-        const int off = (n >> 3) * 1024 + (n & 7) * 128 + ((pc ^ (n & 7)) << 4);
+        const int off = swz128(n, pc);
         store_planes(sB, S::B_PLANE_BYTES, off, xb[i], SPLIT);
       }
     }
@@ -233,72 +150,52 @@ __global__ void __launch_bounds__(NUM_THREADS) gemm_tc_kernel(const GemmArgs a) 
 
   float4 xa[A_LD], xb[B_LD];
   load_chunk(0, xa, xb);
-  tc_fence_before();
-  __syncthreads();   // TMEM address + BN coefficients + barrier init visible
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  constexpr uint32_t idesc = make_idesc(BM, N_OUT);
+  __syncthreads();   // BN coefficients visible
+  float acc[ACC_REGS];
+  const uint32_t a_hi = smem_u32(sA) + wgi * 64 * 128, a_lo = a_hi + A_PLANE_BYTES;
+  const uint32_t b_hi = smem_u32(sB), b_lo = b_hi + S::B_PLANE_BYTES;
 
   for (int c = 0; c < nch; ++c) {
     store_chunk(c, xa, xb);
     fence_proxy_async();   // generic-proxy stores -> visible to the tensor core's async proxy
     __syncthreads();
     if (c + 1 < nch) load_chunk(c + 1, xa, xb);   // in flight while the tensor core works
-    if (tid == 0) {
-      tc_fence_after();
-      const int ksteps = min(KC, K - c * KC) / 8;
-      const uint32_t a_hi = smem_u32(sA), a_lo = a_hi + A_PLANE_BYTES;
-      const uint32_t b_hi = smem_u32(sB), b_lo = b_hi + S::B_PLANE_BYTES;
-      for (int j = 0; j < ksteps; ++j) {
-        const uint32_t acc = (c == 0 && j == 0) ? 0u : 1u;
-        if (STACKED) {
-          // B planes are contiguous in shared memory: rows [0,N) = Bhi, [N,2N) = Blo
-          umma_tf32(tmem_base, make_desc(a_hi + j * 32), make_desc(b_hi + j * 32), make_idesc(BM, 2 * N_OUT), acc);
-          umma_tf32(tmem_base + N_OUT, make_desc(a_lo + j * 32), make_desc(b_hi + j * 32), idesc, 1u);
-        } else if (SPLIT) {
-          umma_tf32(tmem_base, make_desc(a_lo + j * 32), make_desc(b_hi + j * 32), idesc, acc);
-          umma_tf32(tmem_base, make_desc(a_hi + j * 32), make_desc(b_lo + j * 32), idesc, 1u);
-          umma_tf32(tmem_base, make_desc(a_hi + j * 32), make_desc(b_hi + j * 32), idesc, 1u);
-        } else {
-          umma_tf32(tmem_base, make_desc(a_hi + j * 32), make_desc(b_hi + j * 32), idesc, acc);
-        }
+    const int ksteps = min(KC, K - c * KC) / 8;
+    fence();
+    for (int j = 0; j < ksteps; ++j) {
+      const uint32_t first = (c == 0 && j == 0) ? 0u : 1u;
+      if (STACKED) {
+        // B planes are contiguous in shared memory: rows [0,N) = Bhi, [N,2N) = Blo
+        mma_tile<2 * N_OUT, BLK>(acc, a_hi + j * 32, b_hi + j * 32, first);
+        mma_tile<N_OUT, BLK>(acc + N_OUT / 2, a_lo + j * 32, b_hi + j * 32, 1u);
+      } else if (SPLIT) {
+        mma_tile<N_OUT, BLK>(acc, a_lo + j * 32, b_hi + j * 32, first);
+        mma_tile<N_OUT, BLK>(acc, a_hi + j * 32, b_lo + j * 32, 1u);
+        mma_tile<N_OUT, BLK>(acc, a_hi + j * 32, b_hi + j * 32, 1u);
+      } else {
+        mma_tile<N_OUT, BLK>(acc, a_hi + j * 32, b_hi + j * 32, first);
       }
-      umma_commit(bar_mma);
     }
-    mbar_wait(bar_mma, c & 1);   // the MMAs have consumed this chunk's shared memory
+    commit();
+    wait_all();
+    fence_regs(acc);
+    __syncthreads();   // both warpgroups have consumed this chunk's shared memory
   }
-  tc_fence_after();
 
-  // ---- epilogue: TMEM -> registers -> shared (aliases the operand buffers) -> global --------
+  // ---- epilogue: accumulator fragments -> shared (aliases the operand buffers) -> global --------
   {
-    const int q = warp & 3;                       // TMEM lane quarter
-    const int half = warp >> 2;                   // column half handled by this warp
-    const int row = q * 32 + lane;
-    constexpr int CPW = N_OUT / 2;                // columns per warp (half of the tile)
-    constexpr int CB = CPW >= 32 ? 32 : 8;
-    const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + half * CPW;
+    const int row = wgi * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int col = 2 * (lane & 3);
 #pragma unroll
-    for (int cb = 0; cb < CPW / CB; ++cb) {
-      float v[CB];
-      tmem_ld<CB>(taddr + cb * CB, v);
-      if (STACKED) {  // add the small-terms half of the accumulator
-        float v2[CB];
-        tmem_ld<CB>(taddr + N_OUT + cb * CB, v2);
+    for (int i = 0; i < N_OUT / 8; ++i) {
+      float v[4];
 #pragma unroll
-        for (int j = 0; j < CB; ++j) v[j] += v2[j];
-      }
-#pragma unroll
-      for (int j = 0; j < CB; j += 4)
-        *reinterpret_cast<float4*>(sD + row * S::D_PITCH + half * CPW + cb * CB + j) =
-            make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
+      for (int e = 0; e < 4; ++e) v[e] = STACKED ? acc[4 * i + e] + acc[N_OUT / 2 + 4 * i + e] : acc[4 * i + e];
+      *reinterpret_cast<float2*>(sD + row * S::D_PITCH + 8 * i + col) = make_float2(v[0], v[1]);
+      *reinterpret_cast<float2*>(sD + (row + 8) * S::D_PITCH + 8 * i + col) = make_float2(v[2], v[3]);
     }
   }
-  tc_fence_before();
   __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
-  }
   constexpr int C4 = N_OUT / 4;
   for (int e = tid; e < BM * C4; e += NUM_THREADS) {
     const int r = e / C4, c4 = e - r * C4;

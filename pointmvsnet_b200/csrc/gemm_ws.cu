@@ -1,169 +1,67 @@
-// tcgen05 GEMM, second generation: WEIGHTS STATIONARY IN TENSOR MEMORY, points as the N dimension.
+// Warpgroup-MMA GEMM, second generation: persistent, warp-specialised, WEIGHTS STATIONARY IN SHARED MEMORY.
 //
 //   Y[r, 0:cout] = f(X[r, 0:K]) * W[0:cout, 0:K]^T       r = points, fp32 in / fp32 out (3xTF32)
 // (reference: the 1x1 nn.Conv1d of networks.py:13-14,22-23,51-52 and nn/conv.py:21-30, followed by
 // train-mode BatchNorm + ReLU, which is fused here as the INPUT transform of the next layer).
 //
-// Why this shape.  The round-1 kernel (gemm_tc.cu) put the points on the M side and both operands in
-// shared memory; every M=128 x N=64 x K=8 MMA then re-read 6 KB of operands at the ~64 B/clk the
-// tensor core's shared-memory port delivers, i.e. the MMAs were operand-fetch bound at 3x their math
-// time, and one CTA per tile serialised load -> convert -> MMA -> epilogue.  Here
-//   * D^T[cout, points] = W[cout, K] * X^T[K, points]: the weight matrix is the A operand and lives in
-//     TENSOR MEMORY for the whole (persistent) kernel - written once per CTA with tcgen05.st, split into
-//     the TF32 planes  [W_hi ; W_lo]  stacked on the M side (cout <= 64) - so a k-step of 128 points
-//     reads only the two 4 KB point planes X_hi, X_lo from shared memory (64 B per point and k-step
-//     instead of 112) and issues 2 MMAs (M=128, N=128, K=8):  [W_hi;W_lo] * X_hi  and  [W_hi;W_lo] * X_lo.
-//     Accumulator lanes [0,64) hold W_hi*X, lanes [64,128) hold W_lo*X; the epilogue adds them.
-//     cout = 128 uses two A operands (W_hi, W_lo) and two accumulators (3 MMAs per k-step).
-//   * warp-specialised, persistent: 16 (K > 64) or 8 producer warps (coalesced 128-bit global loads four chunks ahead
-//     in registers -> fused input BatchNorm+ReLU -> TF32 hi/lo split -> K-major SWIZZLE_128B stores
-//     into a 4-stage mbarrier ring), 1 MMA warp (one elected thread: tcgen05.mma, tcgen05.commit frees
-//     the stage), 4 epilogue warps per accumulator buffer (tcgen05.ld of one accumulator while the MMAs fill the
-//     other; K <= 64 runs one epilogue group per buffer, see Roles).
-//   * the accumulator is TRANSPOSED (lane = output channel, column = point): a warp stores 32
-//     consecutive channels of one point = one full 128-byte line per instruction with no shared-memory
-//     staging, and the BatchNorm statistics of the outputs (per-channel sum / sum of squares) are
-//     per-thread running sums - no cross-lane reduction at all; fp64 atomics once per group and CTA.
-// Precision: as gemm_tc.cu - hi = the 10 explicit mantissa bits the tensor core reads, lo = x - hi
-// (exact); the extra W_lo*X_lo term this formulation adds is below fp32 resolution.
+// Why this shape.  The round-1 kernel (gemm_tc.cu) re-loads and re-splits the weight slab for every 128-row tile
+// and one CTA per tile serialises load -> convert -> MMA -> epilogue.  Here
+//   * the CTA is persistent: the TF32 planes [W_hi ; W_lo] of the whole weight matrix are written to shared memory
+//     once per CTA (K-major SWIZZLE_128B, one 32-column chunk after the other) and stay there as the B operand of
+//     every tile; cout <= 64 stacks the two planes into one N' = 2 cout operand, so X_hi is read once per k-step
+//     (accumulator columns [0,cout) = X_hi*W_hi, [cout,2cout) = X_hi*W_lo + X_lo*W_hi; the epilogue adds the halves).
+//   * warp-specialised: 8 producer warps (coalesced 128-bit global loads several chunks ahead -> fused input
+//     BatchNorm+ReLU -> TF32 hi/lo split -> K-major SWIZZLE_128B stores into an mbarrier ring of 128-point operand
+//     stages) and two consumer warpgroups (wgmma.mma_async m64nNk8 on rows [64 w, 64 w + 64) of the stage, accumulator
+//     in registers, epilogue straight from the fragments).  The producers run ahead of the consumers' epilogue by
+//     the depth of the ring, so the global loads never stop.
+//   * the BatchNorm statistics of the outputs (per-channel sum / sum of squares) are reduced per warp and tile in
+//     fp32 (shuffles), combined over the warps in fp64 (shared-memory atomics), carried by one thread per statistic,
+//     and leave the CTA as one fp64 atomic per statistic and group.
+// Precision: as gemm_tc.cu - hi = the 10 explicit mantissa bits the tensor core reads, lo = x - hi (exact).
 #include <algorithm>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace pmvs {
 
 namespace ws {
 
-constexpr int NT = 128;                       // points per tile == UMMA N
+using namespace wg;
+
+constexpr int NT = 128;                       // points per tile: two consumer warpgroups x wgmma M = 64
 constexpr int KC = 32;                        // fp32 K columns per chunk == one 128-byte swizzle row
 constexpr int PLANE_BYTES = NT * KC * 4;      // 16 KB
 constexpr int STAGE_BYTES = 2 * PLANE_BYTES;  // X_hi, X_lo
-// Warp roles.  EG = 1: 4 epilogue warps, 16 producer warps (672 threads) - the shapes with K > 64, whose main loop is
-// longer than the epilogue.  EG = 2: TWO epilogue groups (one per accumulator buffer: group e drains the tiles with
-// it % 2 == e, so consecutive tiles' epilogues overlap) and 8 producer warps (544 threads) - K = 32 / 64, where a
-// tile's epilogue is longer than its one or two chunks of main loop.  Measured at it.3 (us, EG = 1 / EG = 2):
-// 32->64 39.2 / 33.4, 64->64 59.7 / 53.6, 64->16 57.7 / 49.5, 64->128 65.9 / 63.9, but 136->64 68.0 / 72.1 and
-// 224->64 92.5 / 96.6.
-constexpr int EPI_GROUP = 4;                  // warps of one epilogue group = the 4 TMEM lane quarters
-template <int EG>
-struct Roles {
-  static constexpr int EPI_WARPS = EG * EPI_GROUP;
-  static constexpr int PROD_WARPS = EG == 2 ? 8 : 16;
-  static constexpr int MMA_WARP = EPI_WARPS;
-  static constexpr int PROD_WARP0 = EPI_WARPS + 1;
-  static constexpr int PROD_THREADS = PROD_WARPS * 32;
-  static constexpr int THREADS = 32 * (EPI_WARPS + 1 + PROD_WARPS);  // 672 / 544
-  static constexpr int A_LD = NT * 8 / PROD_THREADS;  // 16-byte pieces per producer thread and chunk (2 / 4)
-  static_assert(A_LD * PROD_THREADS == NT * 8, "the producers share a chunk evenly");
-};
+// Warp roles: warps [0, 8) = two consumer warpgroups, warps [8, 16) = producers.  512 threads leave 128 registers a
+// thread, which the 64 accumulator registers of a consumer need.
+constexpr int CONS_WARPS = 8, CONS_THREADS = CONS_WARPS * 32;
+constexpr int PROD_WARPS = 8, PROD_WARP0 = CONS_WARPS, PROD_THREADS = PROD_WARPS * 32;
+constexpr int THREADS = CONS_THREADS + PROD_THREADS;
+constexpr int A_LD = NT * 8 / PROD_THREADS;   // 16-byte pieces per producer thread and chunk (4)
+static_assert(A_LD * PROD_THREADS == NT * 8, "the producers share a chunk evenly");
 constexpr int MAXK = 224;
+constexpr int SMEM_MAX = 227 * 1024;          // shared memory a block may use on sm_90
 
-// Shared-memory layout.  ASYNC = 0: the producers prefetch through registers (4 chunks ahead) into a 4-stage operand
-// ring.  ASYNC = N > 0: the raw fp32 chunks travel global -> shared memory with cp.async (LDGSTS, no registers
-// held) into an N-stage staging ring, N - 1 chunks ahead; the producer converts its own pieces from there into a
-// 2-stage operand ring.  16 KB per staging stage, 32 KB per operand stage (X_hi | X_lo).
+// Shared-memory layout.  ASYNC = 0: the producers prefetch through registers (4 chunks ahead) into an NSTAGES-stage
+// operand ring.  ASYNC = N > 0: the raw fp32 chunks travel global -> shared memory with cp.async (LDGSTS, no registers
+// held) into an N-stage staging ring, N - 1 chunks ahead; the producer converts its own pieces from there into the
+// operand ring.  16 KB per staging stage, 32 KB per operand stage (X_hi | X_lo).  The weight planes follow
+// (2 * cout * 128 bytes per K chunk, sized at launch), then the small tables at TAIL.
 template <int ASYNC, int NSTAGES>
 struct Layout {
   static constexpr int NST = NSTAGES;  // operand stages
   static constexpr int RING = 0;
   static constexpr int STAGING = RING + NST * STAGE_BYTES;
-  static constexpr int BN = STAGING + ASYNC * PLANE_BYTES;
-  static constexpr int BAR = BN + 4 * MAXK * 4;
-  static constexpr int TOTAL = BAR + 128;
-  static_assert(TOTAL <= 227 * 1024, "shared memory budget");
+  static constexpr int W = STAGING + ASYNC * PLANE_BYTES;
 };
+__host__ __device__ constexpr int weight_bytes(int cout, int nch) { return nch * 2 * cout * 128; }
+// after the weights: input BatchNorm tables (2 x MAXK floats), the output-statistics scratch (2 x cout doubles), the mbarriers
+constexpr int TAIL_BN = 0, TAIL_RED = TAIL_BN + 2 * MAXK * 4;
+__host__ __device__ constexpr int tail_bar(int cout) { return TAIL_RED + 2 * cout * 8; }
+__host__ __device__ constexpr int tail_bytes(int cout) { return tail_bar(cout) + 128; }
 
-constexpr int TM_A = 0;      // A operand(s): columns [0, 256)
-constexpr int TM_A2 = 128;   // second A operand (W_lo) when cout = 128
-constexpr int TM_D = 256;    // accumulators: two 128-column buffers
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done = 0;
-  while (!done) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-  }
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc {lo, hi}], kind::tf32, issued by ONE thread
-__device__ __forceinline__ void umma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint32_t bdesc_lo, uint32_t bdesc_hi,
-                                             uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 bd;\n\t"
-      "mov.b64 bd, {%2, %3};\n\t"
-      "setp.ne.b32 p, %5, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], bd, %4, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "r"(bdesc_lo), "r"(bdesc_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// one lane of a CONVERGED warp (elect.sync): the issuer of the warp's tcgen05.mma / tcgen05.commit
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-// 16 columns, no wait: the caller issues tcgen05.wait::ld after the last load of a batch.  The outputs are written
-// asynchronously, so they must not be read before that wait (volatile asm keeps the order).
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, float (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7]), "=f"(v[8]),
-        "=f"(v[9]), "=f"(v[10]), "=f"(v[11]), "=f"(v[12]), "=f"(v[13]), "=f"(v[14]), "=f"(v[15])
-      : "r"(taddr));
-}
-// tcgen05.wait::ld with the loaded registers as in/out operands: their uses cannot be scheduled above the wait
-__device__ __forceinline__ void tmem_wait_ld16(float (&v)[16]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+f"(v[0]), "+f"(v[1]), "+f"(v[2]), "+f"(v[3]), "+f"(v[4]), "+f"(v[5]), "+f"(v[6]), "+f"(v[7]), "+f"(v[8]),
-                 "+f"(v[9]), "+f"(v[10]), "+f"(v[11]), "+f"(v[12]), "+f"(v[13]), "+f"(v[14]), "+f"(v[15])
-               :
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const float (&v)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr),
-               "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])),
-               "r"(__float_as_uint(v[3])), "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])),
-               "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7]))
-               : "memory");
-}
-// explicit shared-space accesses on 32-bit shared addresses (STS.128 / LDS.128, never generic ST.E / LD.E)
 __device__ __forceinline__ void sts128(uint32_t addr, float4 v) {
   asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
 }
@@ -184,110 +82,54 @@ __device__ __forceinline__ TileRange my_tiles(int total) {
   return TileRange{lo, hi - lo};
 }
 
-template <int COUT, bool IN_BN, int ASYNC, int NSTAGES, int EG>
-__global__ void __launch_bounds__(Roles<EG>::THREADS, 1) gemm_ws_kernel(const GemmArgs a) {
-  using R = Roles<EG>;
-  constexpr int PROD_WARPS = R::PROD_WARPS, MMA_WARP = R::MMA_WARP, PROD_WARP0 = R::PROD_WARP0;
-  constexpr int PROD_THREADS = R::PROD_THREADS, A_LD = R::A_LD;
+template <int COUT, bool IN_BN, int ASYNC, int NSTAGES>
+__global__ void __launch_bounds__(THREADS, 1) gemm_ws_kernel(const GemmArgs a) {
   using LY = Layout<ASYNC, NSTAGES>;
   constexpr int STAGES = LY::NST;
-  constexpr int SM_RING = LY::RING, SM_STAGING = LY::STAGING, SM_BN = LY::BN, SM_BAR = LY::BAR;
+  constexpr int SM_RING = LY::RING, SM_STAGING = LY::STAGING, SM_W = LY::W;
   constexpr int PF = ASYNC > 0 ? ASYNC - 1 : 4;  // chunks of global loads in flight per producer thread
   constexpr bool STACKED = COUT <= 64;
+  constexpr int W_CHUNK = 2 * COUT * 128;        // [W_hi ; W_lo] of one K chunk
   extern __shared__ __align__(1024) unsigned char smem[];  // SWIZZLE_128B operands need 1024-byte alignment
   const uint32_t smem_base = smem_u32(smem);
-  float* sBN = (float*)(smem + SM_BN);  // input BatchNorm as one FMA per element: A = istd * gamma | B = beta - mean * A, x MAXK
-  uint64_t* bars = (uint64_t*)(smem + SM_BAR);
-  // bars: full[STAGES], empty[STAGES], acc_full[2], acc_empty[2]; then the TMEM base slot
-  const uint32_t bar0 = smem_u32(bars);
-  auto bar_full = [&](int s) { return bar0 + 8u * (uint32_t)s; };
-  auto bar_empty = [&](int s) { return bar0 + 8u * (uint32_t)(STAGES + s); };
-  auto bar_accf = [&](int b) { return bar0 + 8u * (uint32_t)(2 * STAGES + b); };
-  auto bar_acce = [&](int b) { return bar0 + 8u * (uint32_t)(2 * STAGES + 2 + b); };
-  const uint32_t bar_w = bar0 + 8u * (uint32_t)(2 * STAGES + 4);  // weights are in tensor memory
-  uint32_t* tmem_slot = (uint32_t*)(bars + 2 * STAGES + 5);
 
   const int K = a.cin;
   const int nch = (K + KC - 1) / KC;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  // the warp index through a shuffle: the compiler then knows the role branches below are warp-uniform
+  const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
   const int tpg = (a.rows_per_group + NT - 1) / NT;  // tiles per group
   const TileRange tr = my_tiles(a.groups * tpg);
 
-  if (warp == MMA_WARP) {
-    if (lane == 0) {
-      for (int s = 0; s < STAGES; ++s) {
-        mbar_init(bar_full(s), PROD_WARPS);
-        mbar_init(bar_empty(s), 1);
-      }
-      for (int b = 0; b < 2; ++b) {
-        mbar_init(bar_accf(b), 1);
-        mbar_init(bar_acce(b), EPI_GROUP);
-      }
-      mbar_init(bar_w, EPI_GROUP);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(512)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  unsigned char* tail = smem + SM_W + weight_bytes(COUT, nch);
+  float* sBN = (float*)(tail + TAIL_BN);      // input BatchNorm as one FMA per element: A = istd * gamma | B = beta - mean * A, x MAXK
+  double* sRed = (double*)(tail + TAIL_RED);  // per-tile sums of the outputs: [sum(COUT) | sumsq(COUT)]
+  // bars: full[STAGES] (one arrival per producer warp), empty[STAGES] (one per consumer warp)
+  const uint32_t bar0 = smem_u32(tail + tail_bar(COUT));
+  auto bar_full = [&](int s) { return bar0 + 8u * (uint32_t)s; };
+  auto bar_empty = [&](int s) { return bar0 + 8u * (uint32_t)(STAGES + s); };
 
-  if (warp < EPI_GROUP) {
-    // ---- weights -> tensor memory (A operand): lane L of TMEM = row L of [W_hi ; W_lo] ----------------
-    const int L = warp * 32 + lane;
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(warp * 32) << 16);
-    // One row of K floats per thread, in batches of 32 columns: the 8 loads of a batch are in flight together (a
-    // serial 8-column loop cost K/8 dependent L2 round trips = ~10 us of prologue for K = 224).
-    const float* wrow;
-    bool is_hi = true, live = true;
-    if (STACKED) {
-      // lane quarter q = 16 channels: lanes [0,16) of the quarter hold W_hi[16q + i], lanes [16,32) W_lo[16q + i],
-      // so the hi and lo products of a channel meet inside ONE epilogue warp (lane ^ 16), no shared-memory exchange
-      const int ch = warp * 16 + (lane & 15);
-      is_hi = lane < 16;
-      live = ch < COUT;
-      wrow = a.w + (size_t)(live ? ch : 0) * K;
-    } else {
-      wrow = a.w + (size_t)L * K;
+  if (tid == 0) {
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(bar_full(s), PROD_WARPS);
+      mbar_init(bar_empty(s), CONS_WARPS);
     }
-    for (int kb = 0; kb < K; kb += 32) {
-      float4 wv[8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-        wv[i] = kb + 4 * i < K ? ldg4(wrow + kb + 4 * i) : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        if (kb + 8 * j < K) {  // K is a multiple of 8
-          const float x[8] = {wv[2 * j].x, wv[2 * j].y, wv[2 * j].z, wv[2 * j].w,
-                              wv[2 * j + 1].x, wv[2 * j + 1].y, wv[2 * j + 1].z, wv[2 * j + 1].w};
-          float vh[8], vl[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            vh[i] = tf32_hi(x[i]);
-            vl[i] = __fsub_rn(x[i], vh[i]);
-          }
-          if (STACKED) {
-            float v[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) v[i] = !live ? 0.f : (is_hi ? vh[i] : vl[i]);
-            tmem_st8(lane_addr + TM_A + kb + 8 * j, v);
-          } else {
-            tmem_st8(lane_addr + TM_A + kb + 8 * j, vh);
-            tmem_st8(lane_addr + TM_A2 + kb + 8 * j, vl);
-          }
-        }
-      }
-    }
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-    // only the MMA warp needs the weights: it waits on bar_w; the producers start loading X right away
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(bar_w);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
+  for (int i = tid; i < 2 * COUT; i += THREADS) sRed[i] = 0.0;
+  // ---- weights -> shared memory (B operand), once per CTA: chunk c = rows [0,COUT) W_hi | rows [COUT,2 COUT) W_lo ----
+  for (int e = tid; e < COUT * nch * 8; e += THREADS) {
+    const int n = e / (nch * 8), rem = e - n * (nch * 8), c = rem >> 3, pc = rem & 7;
+    const int k0 = c * KC + pc * 4;  // K is a multiple of 8: a 16-byte piece is all inside or all padding
+    const float4 v = k0 < K ? ldg4(a.w + (size_t)n * K + k0) : make_float4(0.f, 0.f, 0.f, 0.f);
+    float4 hi, lo;
+    hi.x = tf32_hi(v.x); hi.y = tf32_hi(v.y); hi.z = tf32_hi(v.z); hi.w = tf32_hi(v.w);
+    lo.x = __fsub_rn(v.x, hi.x); lo.y = __fsub_rn(v.y, hi.y); lo.z = __fsub_rn(v.z, hi.z); lo.w = __fsub_rn(v.w, hi.w);
+    const uint32_t dst = smem_base + SM_W + c * W_CHUNK + swz128(n, pc);
+    sts128(dst, hi);
+    sts128(dst + COUT * 128, lo);
+  }
+  fence_proxy_async();  // the weight planes are read by the tensor core's async proxy
+  __syncthreads();
 
   if (warp >= PROD_WARP0) {
     // =============================== producers ==========================================================
@@ -303,7 +145,7 @@ __global__ void __launch_bounds__(Roles<EG>::THREADS, 1) gemm_ws_kernel(const Ge
 #pragma unroll
     for (int i = 0; i < A_LD; ++i) {
       const int r = prow + ROWS_STEP * i;
-      soff[i] = (r >> 3) * 1024 + (r & 7) * 128 + ((pc ^ (r & 7)) << 4);
+      soff[i] = swz128(r, pc);
     }
 
     // (tile, chunk) cursors of the load stream and of the store stream: both walk items 0, 1, 2, .. in order, so
@@ -411,9 +253,7 @@ __global__ void __launch_bounds__(Roles<EG>::THREADS, 1) gemm_ws_kernel(const Ge
         sts128(hi_plane + soff[i], hi);
         sts128(hi_plane + PLANE_BYTES + soff[i], lo);
       }
-      // No fence.proxy.async here: it lowers to MEMBAR.ALL.CTA, which would wait for this thread's PF chunks of
-      // global loads in flight and serialise the prefetch.  The stores are published by the release-arrive below;
-      // the MMA thread executes the proxy fence after its acquire-wait, before it issues the MMAs that read them.
+      fence_proxy_async();  // these generic-proxy stores are read by the consumers' wgmma (async proxy)
       __syncwarp();
       if (lane == 0) mbar_arrive(bar_full(stage));
       advance(cp);
@@ -446,90 +286,24 @@ __global__ void __launch_bounds__(Roles<EG>::THREADS, 1) gemm_ws_kernel(const Ge
         }
       }
     }
-  } else if (warp == MMA_WARP) {
-    // =============================== MMA issuer ==========================================================
-    // The whole warp walks the pipeline CONVERGED and one elected lane issues (elect.sync): in warp-uniform code ptxas
-    // keeps descriptors in uniform registers and emits the UTCHMMAs back to back.  Issued from an `if (lane == 0)`
-    // region every MMA was wrapped in an ELECT / BRA.U.ANY loop with ~10 dependent uniform-datapath instructions -
-    // ~2000 clk of issue latency per 32-channel chunk against 555 clk of tensor-pipe time, which capped every GEMM
-    // of the pass at ~2.7 TB/s (profiles/README_r02.md).
-    {
-      constexpr uint32_t idesc = make_idesc(128, NT);
-      // K-major SWIZZLE_128B descriptor = {lo: (addr >> 4) | LBO 1, hi: SBO 1024 B | version 1 | swizzle 2};
-      // stage / plane / k-step offsets are plain adds on the low word (the ring lies below 256 KB: no carry)
-      constexpr uint32_t desc_hi = (uint32_t)(1024 >> 4) | (1u << 14) | (2u << 29);
-      const uint32_t desc_lo0 = (((smem_base + SM_RING) >> 4) & 0x3FFFu) | (1u << 16);
-      constexpr uint32_t D_STAGE = STAGE_BYTES >> 4, D_PLANE = PLANE_BYTES >> 4, D_KSTEP = 32 >> 4;
-      mbar_wait(bar_w, 0u);  // [W_hi ; W_lo] written by the four epilogue warps
-      tc_fence_after();
-      int n = 0;
-      for (int it = 0; it < tr.count; ++it) {
-        const int b = it & 1, use = it >> 1;
-        mbar_wait(bar_acce(b), (uint32_t)((use & 1) ^ 1));  // the epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t d0 = tmem_base + TM_D + b * NT;
-        for (int c = 0; c < nch; ++c, ++n) {
-          const int stage = n % STAGES;
-          mbar_wait(bar_full(stage), (uint32_t)((n / STAGES) & 1));
-          if (elect_one()) {
-            fence_proxy_async();  // the producers' generic-proxy stores (acquired above) -> the tensor core's async proxy
-            tc_fence_after();
-            const uint32_t x_hi = desc_lo0 + (uint32_t)stage * D_STAGE, x_lo = x_hi + D_PLANE;
-            const uint32_t a0 = tmem_base + TM_A + (uint32_t)(c * KC);
-            const int ksteps = min(KC, K - c * KC) / 8;
-            auto kstep = [&](int j, uint32_t acc) {
-              if (STACKED) {
-                umma_tf32_ts(d0, a0 + j * 8, x_hi + j * D_KSTEP, desc_hi, idesc, acc);
-                umma_tf32_ts(d0, a0 + j * 8, x_lo + j * D_KSTEP, desc_hi, idesc, 1u);
-              } else {
-                umma_tf32_ts(d0, a0 + j * 8, x_hi + j * D_KSTEP, desc_hi, idesc, acc);
-                umma_tf32_ts(d0, a0 + j * 8, x_lo + j * D_KSTEP, desc_hi, idesc, 1u);
-                umma_tf32_ts(d0, a0 + (TM_A2 - TM_A) + j * 8, x_hi + j * D_KSTEP, desc_hi, idesc, 1u);  // W_lo * X_hi
-              }
-            };
-            if (ksteps == KC / 8) {
-#pragma unroll
-              for (int j = 0; j < KC / 8; ++j) kstep(j, (c | j) != 0 ? 1u : 0u);
-            } else {
-              for (int j = 0; j < ksteps; ++j) kstep(j, (c | j) != 0 ? 1u : 0u);
-            }
-            umma_commit(bar_empty(stage));  // the MMAs have consumed this stage's shared memory
-            if (c == nch - 1) umma_commit(bar_accf(b));  // accumulator complete
-          }
-          __syncwarp();
-        }
-      }
-    }
   } else {
-    // =============================== epilogue ===========================================================
-    const int q = warp & (EPI_GROUP - 1);  // TMEM lane quarter
-    const int eg = warp / EPI_GROUP;       // epilogue group = accumulator buffer
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16);
-    // stacked: lane 32q + i of the accumulator = W_hi * X (i < 16) or W_lo * X (i >= 16) of channel 16q + (i & 15),
-    // column = point.  hi + lo is one shuffle with lane ^ 16; the lower half-warp then owns the even points of the
-    // slab and the upper half the odd ones: a store instruction writes 16 consecutive channels of two points.
-    constexpr int NCH_T = 1;   // channels per thread
-    const int half = lane >> 4;
-    const int chs[1] = {STACKED ? q * 16 + (lane & 15) : q * 32 + lane};
-    double acc1[NCH_T], acc2[NCH_T];
-#pragma unroll
-    for (int h = 0; h < NCH_T; ++h) acc1[h] = acc2[h] = 0.0;
+    // =============================== consumers: MMA + epilogue ==========================================
+    const int wgi = warp >> 2;                                   // warpgroup: rows [64 wgi, 64 wgi + 64) of a tile
+    const int frow = wgi * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's fragment rows: frow, frow + 8
+    const int fcol = 2 * (lane & 3);                             // fragment columns 8 i + fcol + {0, 1}
+    constexpr int ACC_REGS = (STACKED ? 2 * COUT : COUT) / 2;
+    constexpr int BLK = COUT < 64 ? COUT : 64;  // one wgmma shape for every product into this accumulator (wgmma.cuh)
+    float acc[ACC_REGS];
+    const uint32_t w_base = smem_base + SM_W;
+    // output statistics: thread t < 2 COUT carries statistic t ([sum | sumsq] x COUT) of the current group in fp64
+    double racc = 0.0;
     int acc_g = -1;
     auto flush = [&]() {
-      if (a.out_stats != nullptr && acc_g >= 0) {
-        double* o = a.out_stats + (size_t)acc_g * 2 * a.cout;
-#pragma unroll
-        for (int h = 0; h < NCH_T; ++h) {
-          if (chs[h] < COUT) {
-            atomicAdd(o + chs[h], acc1[h]);
-            atomicAdd(o + a.cout + chs[h], acc2[h]);
-          }
-        }
-      }
-#pragma unroll
-      for (int h = 0; h < NCH_T; ++h) acc1[h] = acc2[h] = 0.0;
+      if (a.out_stats != nullptr && acc_g >= 0 && tid < 2 * COUT) atomicAdd(a.out_stats + (size_t)acc_g * 2 * a.cout + tid, racc);
+      racc = 0.0;
     };
-    for (int it = eg; it < tr.count; it += EG) {
+    int n = 0;
+    for (int it = 0; it < tr.count; ++it) {
       const int t = tr.first + it;
       const int g = t / tpg, row0 = (t - g * tpg) * NT;
       const int rows_valid = min(NT, a.rows_per_group - row0);
@@ -538,129 +312,125 @@ __global__ void __launch_bounds__(Roles<EG>::THREADS, 1) gemm_ws_kernel(const Ge
         flush();
         acc_g = g;
       }
-      const int b = it & 1, use = it >> 1;
-      mbar_wait(bar_accf(b), (uint32_t)(use & 1));
-      tc_fence_after();
-      const uint32_t d0 = lane_addr + TM_D + b * NT;
-      float s1[NCH_T], s2[NCH_T];
-#pragma unroll
-      for (int h = 0; h < NCH_T; ++h) s1[h] = s2[h] = 0.f;
-      if (STACKED) {
-        // 32 points per step.  (Measured: 16-column steps with the next tcgen05.ld in flight during the stores were
-        // 6-12 % SLOWER for the stacked shapes - twice the TMEM loads and waits for the same data.)
-#pragma unroll 1
-        for (int slab = 0; slab < NT / 32; ++slab) {
-          float v[32];
-          tmem_ld32(d0 + slab * 32, v);
-          const int ch = chs[0];
-          float* yp = a.y + (grow0 + slab * 32 + half) * a.ldy + ch;
-          const int pmax = rows_valid - slab * 32 - half;  // this half-warp's point 2*jj + half is valid iff 2*jj < pmax
-#pragma unroll
-          for (int jj = 0; jj < 16; ++jj) {
-            // lower half keeps its even point and hands over its odd one; the upper half the other way round
-            const float mine = half ? v[2 * jj + 1] : v[2 * jj];
-            const float send = half ? v[2 * jj] : v[2 * jj + 1];
-            const float o = mine + __shfl_xor_sync(0xffffffffu, send, 16);
-            if (ch < COUT && 2 * jj < pmax) {
-              *yp = o;
-              s1[0] += o;
-              s2[0] = fmaf(o, o, s2[0]);
-            }
-            yp += 2 * a.ldy;
+      for (int c = 0; c < nch; ++c, ++n) {
+        const int stage = n % STAGES;
+        mbar_wait(bar_full(stage), (uint32_t)((n / STAGES) & 1));
+        const uint32_t x_hi = smem_base + SM_RING + stage * STAGE_BYTES + wgi * 64 * 128, x_lo = x_hi + PLANE_BYTES;
+        const uint32_t w_hi = w_base + c * W_CHUNK, w_lo = w_hi + COUT * 128;
+        const int ksteps = min(KC, K - c * KC) / 8;
+        fence();
+        for (int j = 0; j < ksteps; ++j) {
+          const uint32_t first = (c | j) != 0 ? 1u : 0u;
+          if (STACKED) {
+            mma_tile<2 * COUT, BLK>(acc, x_hi + j * 32, w_hi + j * 32, first);
+            mma_tile<COUT, BLK>(acc + COUT / 2, x_lo + j * 32, w_hi + j * 32, 1u);
+          } else {
+            mma_tile<COUT, BLK>(acc, x_lo + j * 32, w_hi + j * 32, first);
+            mma_tile<COUT, BLK>(acc, x_hi + j * 32, w_lo + j * 32, 1u);
+            mma_tile<COUT, BLK>(acc, x_hi + j * 32, w_hi + j * 32, 1u);
           }
         }
-      } else {
-        // lane = channel; W_hi * (X_hi + X_lo) + W_lo * X_hi were accumulated in place.  16 points at a time, the
-        // tcgen05.ld of the next 16 columns in flight while the current ones are stored
-        auto consume = [&](const float (&v)[16], int p0) {
-          float* yp = a.y + (grow0 + p0) * a.ldy + chs[0];
-          const int pmax = rows_valid - p0;
+        commit();
+        wait_all();
+        fence_regs(acc);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar_empty(stage));  // this warp's MMAs have consumed the stage
+      }
+      // ---- epilogue from the fragments: a warp's store instruction writes 32-byte runs of 8 rows ----
+      const bool ok0 = frow < rows_valid, ok1 = frow + 8 < rows_valid;
+      float* y0 = a.y + (grow0 + frow) * a.ldy + fcol;
+      float* y1 = y0 + (size_t)8 * a.ldy;
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            if (j < pmax) {
-              *yp = v[j];
-              s1[0] += v[j];
-              s2[0] = fmaf(v[j], v[j], s2[0]);
-            }
-            yp += a.ldy;
+      for (int i = 0; i < COUT / 8; ++i) {
+        float v[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) v[e] = STACKED ? acc[4 * i + e] + acc[COUT / 2 + 4 * i + e] : acc[4 * i + e];
+        if (ok0) *reinterpret_cast<float2*>(y0 + 8 * i) = make_float2(v[0], v[1]);
+        if (ok1) *reinterpret_cast<float2*>(y1 + 8 * i) = make_float2(v[2], v[3]);
+        if (a.out_stats != nullptr) {
+          if (!ok0) v[0] = v[1] = 0.f;
+          if (!ok1) v[2] = v[3] = 0.f;
+          float s[4] = {v[0] + v[2], v[1] + v[3], fmaf(v[0], v[0], v[2] * v[2]), fmaf(v[1], v[1], v[3] * v[3])};
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {  // the 8 lanes with the same lane % 4 hold the same columns
+            s[e] += __shfl_xor_sync(0xffffffffu, s[e], 4);
+            s[e] += __shfl_xor_sync(0xffffffffu, s[e], 8);
+            s[e] += __shfl_xor_sync(0xffffffffu, s[e], 16);
           }
-        };
-        float va[16], vb[16];
-        tmem_ld16_nowait(d0, va);
-        tmem_wait_ld16(va);
-#pragma unroll 1
-        for (int hs = 0; hs < NT / 16; hs += 2) {
-          tmem_ld16_nowait(d0 + (hs + 1) * 16, vb);
-          consume(va, hs * 16);
-          tmem_wait_ld16(vb);
-          if (hs + 2 < NT / 16) tmem_ld16_nowait(d0 + (hs + 2) * 16, va);
-          consume(vb, (hs + 1) * 16);
-          if (hs + 2 < NT / 16) tmem_wait_ld16(va);
+          if (lane < 4) {  // fp64 from here on: the order in which the 8 warps arrive does not show in the fp32 results
+            atomicAdd(&sRed[8 * i + fcol], (double)s[0]);
+            atomicAdd(&sRed[8 * i + fcol + 1], (double)s[1]);
+            atomicAdd(&sRed[COUT + 8 * i + fcol], (double)s[2]);
+            atomicAdd(&sRed[COUT + 8 * i + fcol + 1], (double)s[3]);
+          }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_acce(b));
-#pragma unroll
-      for (int h = 0; h < NCH_T; ++h) {
-        acc1[h] += (double)s1[h];
-        acc2[h] += (double)s2[h];
+      if (a.out_stats != nullptr) {
+        named_bar_sync(2, CONS_THREADS);  // every consumer warp has added this tile's sums
+        if (tid < 2 * COUT) {
+          racc += sRed[tid];
+          sRed[tid] = 0.0;
+        }
+        named_bar_sync(2, CONS_THREADS);  // cleared before the next tile's sums arrive
       }
     }
     flush();
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == MMA_WARP) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512) : "memory");
-  }
 }
 
-template <int COUT, bool IN_BN, int ASYNC, int NSTAGES, int EG>
+// Ring depths by K: <ASYNC staging stages, operand stages> of the cp.async form and of the register-prefetch form
+constexpr int DEEP_K = 160;
+template <int ASYNC, int NSTAGES>
+constexpr int smem_bytes(int cout, int cin) {
+  return Layout<ASYNC, NSTAGES>::W + weight_bytes(cout, (cin + KC - 1) / KC) + tail_bytes(cout);
+}
+constexpr bool fits(int cin, int cout) {
+  return cin <= DEEP_K ? (smem_bytes<4, 2>(cout, cin) <= SMEM_MAX && smem_bytes<0, 4>(cout, cin) <= SMEM_MAX)
+                       : (smem_bytes<3, 2>(cout, cin) <= SMEM_MAX && smem_bytes<0, 3>(cout, cin) <= SMEM_MAX);
+}
+// The six contractions of a PointFlow iteration must stay on this kernel: growing the tail tables or the rings, or a
+// static __shared__ variable in the kernel (which would also break the 1024-byte alignment the swizzled planes need:
+// the dynamic window is 1024-aligned only while it starts the block's shared memory), shows up here, not as a
+// silently slower pass.  224 -> 64 leaves 128 bytes.
+static_assert(fits(136, 64) && fits(32, 64) && fits(64, 128) && fits(224, 64) && fits(64, 64) && fits(64, 16),
+              "a hot-path GEMM shape no longer fits the shared memory of gemm_ws_kernel");
+
+template <int COUT, bool IN_BN, int ASYNC, int NSTAGES>
 static int launch_pf(const GemmArgs& a, cudaStream_t st, const char* name) {
-  constexpr int SM_TOTAL = Layout<ASYNC, NSTAGES>::TOTAL;
+  const int smem_total = smem_bytes<ASYNC, NSTAGES>(COUT, a.cin);
+  if (smem_total > SMEM_MAX) return -1;  // the weight planes of this shape do not fit beside the rings
   static unsigned long long smem_done = 0;
-  PMVS_TRY((ensure_dyn_smem(gemm_ws_kernel<COUT, IN_BN, ASYNC, NSTAGES, EG>, SM_TOTAL, smem_done, "gemm_ws")));
-  static int num_sms = 0;
-  if (num_sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || num_sms <= 0) num_sms = 148;
-  }
+  PMVS_TRY((ensure_dyn_smem(gemm_ws_kernel<COUT, IN_BN, ASYNC, NSTAGES>, SMEM_MAX, smem_done, "gemm_ws")));
   const long long tiles = (long long)a.groups * cdiv(a.rows_per_group, NT);
-  const int grid = (int)std::min<long long>(tiles, num_sms);
+  const int grid = (int)std::min<long long>(tiles, sm_count());
   prof_begin(name, st);
-  gemm_ws_kernel<COUT, IN_BN, ASYNC, NSTAGES, EG><<<grid, Roles<EG>::THREADS, SM_TOTAL, st>>>(a);
+  gemm_ws_kernel<COUT, IN_BN, ASYNC, NSTAGES><<<grid, THREADS, smem_total, st>>>(a);
   return check_launch("gemm_ws_kernel", st);
 }
 template <int COUT, bool IN_BN>
 static int launch_one(const GemmArgs& a, cudaStream_t st, const char* name) {
-  // Depth variants measured within 1 % of each other at BASELINE C2 (staging 3..7 stages x operand 2..4 stages, round 2):
-  // the kernels sit at ~70 % of what a read-dominated stream reaches on this part (profiles/r02/hbm_read_probe.txt),
-  // not at a pipeline-depth limit.  Two are kept: the default and the register-prefetch form.
-  if (opt(OPT_GEMM) == 1) return launch_pf<COUT, IN_BN, 0, 4, 1>(a, st, name);  // register prefetch, 4 chunks in flight, 4 operand stages
-  // cp.async staging: 4 chunks (64 KB) in flight, 3 operand stages; two epilogue groups when the main loop is short
-  if (a.cin <= 64) return launch_pf<COUT, IN_BN, 5, 3, 2>(a, st, name);
-  return launch_pf<COUT, IN_BN, 5, 3, 1>(a, st, name);
+  // The weight planes take 2 * cout * 128 bytes per 32-column chunk of K (112 KB for 224 -> 64), the rings get the
+  // rest of the 227 KB: deeper rings for the shapes with K <= 160.
+  const bool deep = a.cin <= DEEP_K;
+  if (opt(OPT_GEMM) == 1)  // register prefetch, 4 chunks in flight
+    return deep ? launch_pf<COUT, IN_BN, 0, 4>(a, st, name) : launch_pf<COUT, IN_BN, 0, 3>(a, st, name);
+  // cp.async staging, 3 or 2 chunks (48 / 32 KB) in flight, 2 operand stages
+  return deep ? launch_pf<COUT, IN_BN, 4, 2>(a, st, name) : launch_pf<COUT, IN_BN, 3, 2>(a, st, name);
 }
 
 }  // namespace ws
 
 // returns -1 when this path does not apply (caller falls back to gemm_tc / SIMT)
 int launch_gemm_ws(const GemmArgs& a, cudaStream_t st, const char* name) {
-  if (a.cin % 8 != 0 || a.cin > ws::MAXK || a.ldx % 4 != 0 || a.groups <= 0 || a.rows_per_group <= 0) return -1;
-  if (((uintptr_t)a.x & 15) || ((uintptr_t)a.w & 15)) return -1;
+  if (a.cin % 8 != 0 || a.cin > ws::MAXK || a.ldx % 4 != 0 || a.ldy % 2 != 0 || a.groups <= 0 || a.rows_per_group <= 0) return -1;
+  if (((uintptr_t)a.x & 15) || ((uintptr_t)a.w & 15) || ((uintptr_t)a.y & 7)) return -1;
   if ((long long)a.groups * cdiv(a.rows_per_group, ws::NT) >= (1ll << 31) / ws::MAXK) return -1;
   const bool bn = a.in_stats != nullptr;
   switch (a.cout) {
     case 16: return bn ? ws::launch_one<16, true>(a, st, name) : ws::launch_one<16, false>(a, st, name);
     case 32: return bn ? ws::launch_one<32, true>(a, st, name) : ws::launch_one<32, false>(a, st, name);
     case 64: return bn ? ws::launch_one<64, true>(a, st, name) : ws::launch_one<64, false>(a, st, name);
-    case 128:
-      if (a.cin > 128) return -1;
-      return bn ? ws::launch_one<128, true>(a, st, name) : ws::launch_one<128, false>(a, st, name);
+    case 128: return bn ? ws::launch_one<128, true>(a, st, name) : ws::launch_one<128, false>(a, st, name);
   }
   return -1;
 }

@@ -1,7 +1,7 @@
 """EdgeConv / EdgeConvNoC (reference networks.py:9-81), CUDA-branch semantics.
 
 Same constructor, parameter names (``conv1``, ``conv2``, ``bn``) and forward signature as
-the reference, so its checkpoints load unchanged.  The forward runs three sm_100a kernels
+the reference, so its checkpoints load unchanged.  The forward runs three sm_90a kernels
 (GEMM, gathered-difference statistics, normalise + ReLU + mean over K) on points-major
 data; the [B,C,N,K] tensors of the reference are never materialised.  Forward only: the
 backward of the fused layer is a later row of the scope table (SURVEY.md section 8f)."""

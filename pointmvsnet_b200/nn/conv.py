@@ -1,6 +1,6 @@
 """Conv1d / Conv2d + BN + ReLU containers (reference nn/conv.py:7-41, 43-81).  Parameter names
 (``conv.weight``, ``bn.*``) match the reference so its checkpoints load unchanged; inside
-PointFlow the arithmetic is done by the fused sm_100a kernels, this forward is the
+PointFlow the arithmetic is done by the fused sm_90a kernels, this forward is the
 stock-library path for stand-alone use."""
 import torch.nn.functional as F
 from torch import nn

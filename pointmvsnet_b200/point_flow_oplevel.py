@@ -7,7 +7,7 @@ This is what an UNCHANGED reference ``model.py`` does once ``install_as_pointmvs
 hot operator served by this package's stand-alone kernels (``pmvs_feature_fetch``, ``pmvs_knn3d``,
 ``pmvs_edgeconv_pm``) and the glue (interpolate, cat, softmax, the ``flow_mlp`` 1x1 convolutions + BatchNorm1d) by
 stock PyTorch exactly as in the reference.  It exists so that the operator-level drop-in has a GPU test
-(tests/test_gpu_parity.py::test_oplevel_closure_equals_fused_point_flow) and a measured rate
+(tests/test_gpu_parity.py::test_oplevel_closure_equals_fused_point_flow) and a benchmark arm
 (``bench.py --mode oplevel``); the product path is the fused ``PointFlow`` (~17 launches per iteration instead of
 ~100 per sub-cloud).
 """

@@ -1,5 +1,5 @@
 """FeatureFetcher: differentiable homography warp + bilinear multi-view fetch
-(reference utils/feature_fetcher.py:8-60), one sm_100a kernel per direction."""
+(reference utils/feature_fetcher.py:8-60), one sm_90a kernel per direction."""
 import torch
 import torch.nn as nn
 

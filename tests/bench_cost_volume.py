@@ -1,5 +1,5 @@
-import sys, torch
-sys.path.insert(0, "/root/repo")
+import os, sys, torch
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from pointmvsnet_b200 import _lib
 from pointmvsnet_b200.cost_volume import build_cost_volume
 from pointmvsnet_b200.synthetic import make_cameras

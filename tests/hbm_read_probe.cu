@@ -67,6 +67,8 @@ int main() {
     }
     printf("%-44s %8.1f us  %7.1f GB/s\n", name, best * 1e3, nbytes / (best * 1e-3) / 1e9);
   };
+  int sms = 0;  // one CTA per SM (132 on an H100)
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
   cudaFuncSetAttribute(rd<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * 16384);
   cudaFuncSetAttribute(rd<7>, cudaFuncAttributeMaxDynamicSharedMemorySize, 7 * 16384);
   cudaFuncSetAttribute(rd<12>, cudaFuncAttributeMaxDynamicSharedMemorySize, 12 * 16384);
@@ -77,16 +79,16 @@ int main() {
     const size_t nb = (size_t)rows * K * 4;
     char nm[128];
     for (int mode = 0; mode < 2; ++mode) {
-      snprintf(nm, 128, "K=%d ld=%d mode=%s D=4", K, ldx, mode ? "seq" : "chunked"); time_it([&] { rd<4><<<148, 512, 4 * 16384>>>(x, out, rows, K, ldx, mode); }, nb, nm);
-      snprintf(nm, 128, "K=%d ld=%d mode=%s D=7", K, ldx, mode ? "seq" : "chunked"); time_it([&] { rd<7><<<148, 512, 7 * 16384>>>(x, out, rows, K, ldx, mode); }, nb, nm);
-      snprintf(nm, 128, "K=%d ld=%d mode=%s D=12", K, ldx, mode ? "seq" : "chunked"); time_it([&] { rd<12><<<148, 512, 12 * 16384>>>(x, out, rows, K, ldx, mode); }, nb, nm);
+      snprintf(nm, 128, "K=%d ld=%d mode=%s D=4", K, ldx, mode ? "seq" : "chunked"); time_it([&] { rd<4><<<sms, 512, 4 * 16384>>>(x, out, rows, K, ldx, mode); }, nb, nm);
+      snprintf(nm, 128, "K=%d ld=%d mode=%s D=7", K, ldx, mode ? "seq" : "chunked"); time_it([&] { rd<7><<<sms, 512, 7 * 16384>>>(x, out, rows, K, ldx, mode); }, nb, nm);
+      snprintf(nm, 128, "K=%d ld=%d mode=%s D=12", K, ldx, mode ? "seq" : "chunked"); time_it([&] { rd<12><<<sms, 512, 12 * 16384>>>(x, out, rows, K, ldx, mode); }, nb, nm);
     }
   }
   // strided slices of a 224-wide matrix (EdgeConv layer inputs): K=64 of ld=224, K=32 of ld=224
-  { const size_t nb = (size_t)rows * 64 * 4; time_it([&] { rd<7><<<148, 512, 7 * 16384>>>(x, out, rows, 64, 224, 0); }, nb, "K=64 of ld=224 chunked D=7"); }
-  { const size_t nb = (size_t)rows * 32 * 4; time_it([&] { rd<7><<<148, 512, 7 * 16384>>>(x, out, rows, 32, 224, 0); }, nb, "K=32 of ld=224 chunked D=7"); }
-  time_it([&] { rd_plain<<<148 * 2, 1024>>>((const float4*)x, out, bytes / 16); }, bytes, "plain LDG.128 grid-stride, 2048 thr/SM");
-  time_it([&] { rd_plain<<<148, 512>>>((const float4*)x, out, bytes / 16); }, bytes, "plain LDG.128 grid-stride, 512 thr/SM");
+  { const size_t nb = (size_t)rows * 64 * 4; time_it([&] { rd<7><<<sms, 512, 7 * 16384>>>(x, out, rows, 64, 224, 0); }, nb, "K=64 of ld=224 chunked D=7"); }
+  { const size_t nb = (size_t)rows * 32 * 4; time_it([&] { rd<7><<<sms, 512, 7 * 16384>>>(x, out, rows, 32, 224, 0); }, nb, "K=32 of ld=224 chunked D=7"); }
+  time_it([&] { rd_plain<<<sms * 2, 1024>>>((const float4*)x, out, bytes / 16); }, bytes, "plain LDG.128 grid-stride, 2048 thr/SM");
+  time_it([&] { rd_plain<<<sms, 512>>>((const float4*)x, out, bytes / 16); }, bytes, "plain LDG.128 grid-stride, 512 thr/SM");
   printf("done\n");
   return 0;
 }

@@ -1,6 +1,5 @@
 """GPU parity tests: the CUDA path (through the C ABI / Python mirror) against the CPU oracle
-and the committed golden vectors.  Tolerances (fp32, stated per stage; measured errors on
-B200 are ~10x smaller, see profiles/parity_r01.md):
+and the committed golden vectors.  Tolerances (fp32, stated per stage):
 
   gather_knn fwd/bwd ............ bit exact
   FeatureFetcher vs oracle ...... atol 1e-5 (same op sequence; measured 0)
@@ -401,7 +400,7 @@ def test_chained_pass_vs_oracle_pass(golden_weights, golden_params):
 @pytest.mark.parametrize("cin,cout,rows", [(136, 64, 1000), (224, 64, 25600), (64, 128, 300), (64, 16, 4097), (32, 64, 128)])
 def test_linear_pm_modes_vs_fp64(mode, rtol, cin, cout, rows):
     """The per-point contraction in its three arithmetic modes (fp32 SIMT, 3xTF32 and TF32 on
-    tcgen05) against an fp64 matmul, with fused input BatchNorm+ReLU and output statistics.
+    the tensor cores) against an fp64 matmul, with fused input BatchNorm+ReLU and output statistics.
     Error is normalised by |x|.|w| per output element (rtol)."""
     from pointmvsnet_b200 import _lib
     gen = torch.Generator().manual_seed(cin * 1000 + cout)
@@ -648,7 +647,7 @@ def test_coarse_cost_volume_golden_and_oracle():
 
 def test_edgeconv_generic_paths_runtime_k_and_simt_fallback():
     """K != 16 (runtime-K gather loop), out_channels 16 (contraction falls back to the fp32 SIMT
-    kernel: the tcgen05 path covers N in {16, 64, 128}) and a ragged point count."""
+    kernel: the tensor-core path covers N in {16, 64, 128}) and a ragged point count."""
     from pointmvsnet_b200.networks import EdgeConv, EdgeConvNoC
     gen = torch.Generator().manual_seed(41)
     for cls, cin, cout, K, concat in ((EdgeConv, 16, 16, 8, True), (EdgeConvNoC, 24, 32, 5, False),

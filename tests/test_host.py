@@ -262,33 +262,55 @@ def test_bench_per_iteration_grouping():
     assert bench.per_iteration_kernel_ms([("knn3d", 1.0)], 3) is None
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/pointmvsnet"), reason="reference checkout not present")
-def test_unchanged_reference_model_imports_our_operators():
-    """Drop-in check (build container only): with install_as_pointmvsnet(reference_root) the
-    reference's UNCHANGED pointmvsnet/model.py resolves its hot-path imports (model.py:8-12) to
-    this package, and its PointMVSNet owns our EdgeConv modules with checkpoint-compatible names."""
+def test_install_as_pointmvsnet_into_a_package_tree(tmp_path):
+    """install_as_pointmvsnet(root) with a real `pointmvsnet` package under root (here a throw-away one with a model.py
+    of a few import lines, standing in for a checkout of the reference): the package's own modules are imported from
+    root, only the hot-path modules are replaced, its networks module gets our EdgeConv classes, and a PointFlow
+    built on the model's modules shares them."""
+    pkg = tmp_path / "pointmvsnet"
+    for sub in ("", "functions", "utils"):
+        (pkg / sub).mkdir(exist_ok=True)
+        (pkg / sub / "__init__.py").write_text("")
+    (pkg / "functions" / "functions.py").write_text("MARK = 'from the package tree'\n")
+    (pkg / "networks.py").write_text(
+        "import torch.nn as nn\n"
+        "from pointmvsnet.functions.gather_knn import gather_knn\n"
+        "class EdgeConv(nn.Module):\n    pass\n"
+        "class EdgeConvNoC(nn.Module):\n    pass\n")
+    (pkg / "model.py").write_text(
+        "import torch.nn as nn\n"
+        "from pointmvsnet.networks import *\n"
+        "from pointmvsnet.functions.functions import MARK\n"
+        "from pointmvsnet.utils.feature_fetcher import FeatureFetcher\n"
+        "from pointmvsnet.utils.torch_utils import get_knn_3d\n"
+        "class Net(nn.Module):\n"
+        "    def __init__(self):\n"
+        "        super().__init__()\n"
+        "        self.feature_fetcher = FeatureFetcher()\n"
+        "        self.flow_edge_conv = nn.ModuleList([EdgeConvNoC(136, 32), EdgeConv(32, 32), EdgeConv(64, 64)])\n"
+        "        self.flow_mlp = nn.Sequential(nn.Conv1d(224, 64, 1), nn.Conv1d(64, 1, 1))\n")
     code = r"""
 import sys
 sys.path.insert(0, %r)
 import pointmvsnet_b200
-pointmvsnet_b200.install_as_pointmvsnet("/root/reference")
+pointmvsnet_b200.install_as_pointmvsnet(%r)
 import pointmvsnet.model as m
 import pointmvsnet_b200.networks as ours
 from pointmvsnet_b200.utils.feature_fetcher import FeatureFetcher
 from pointmvsnet_b200.utils.torch_utils import get_knn_3d
-assert m.get_knn_3d is get_knn_3d
-assert m.FeatureFetcher is FeatureFetcher
-net = m.PointMVSNet()
+from pointmvsnet_b200.functions.gather_knn import gather_knn
+assert m.__file__.startswith(%r) and m.MARK == 'from the package tree'
+assert m.get_knn_3d is get_knn_3d and m.FeatureFetcher is FeatureFetcher
+import pointmvsnet.networks as ref_networks, pointmvsnet.functions as pf
+assert ref_networks.gather_knn is gather_knn and hasattr(pf.dgcnn_ext, "gather_knn_forward")
+net = m.Net()
 assert isinstance(net.flow_edge_conv[0], ours.EdgeConvNoC) and isinstance(net.flow_edge_conv[2], ours.EdgeConv)
 assert isinstance(net.feature_fetcher, FeatureFetcher)
-import torch
-sd = torch.load("/root/reference/outputs/dtu_wde3/model_pretrained.pth", map_location="cpu", weights_only=False)["model"]
-net.load_state_dict({k[7:]: v for k, v in sd.items()})
 from pointmvsnet_b200.point_flow import PointFlow
-pf = PointFlow(flow_edge_conv=net.flow_edge_conv, flow_mlp=net.flow_mlp)  # shares the modules
-assert pf.flow_mlp[1].weight is net.flow_mlp[1].weight
+shared = PointFlow(flow_edge_conv=net.flow_edge_conv, flow_mlp=net.flow_mlp)
+assert shared.flow_edge_conv is net.flow_edge_conv and shared.flow_mlp[1].weight is net.flow_mlp[1].weight
 print("DROPIN-OK")
-""" % ROOT
+""" % (ROOT, str(tmp_path), str(tmp_path))
     out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=300)
     assert "DROPIN-OK" in out.stdout, out.stdout + out.stderr
 
