@@ -62,15 +62,20 @@ int pmvs_get_gemm_mode(void);
  *   PMVS_OPT_FETCH  1 = consecutive hypotheses share the texel quad, fp32 pair math (3 CTAs / SM),
  *                   2 = the same with 2 CTAs / SM and a larger register budget, 0 = 4 taps per (hypothesis, view)
  *                   (the kernel used for V > 6)
- *   PMVS_OPT_GEMM   2 = weights stationary in shared memory, persistent, cp.async staging ring (2-3 chunks in
- *                   flight), 1 = the same kernel with register prefetch,
+ *   PMVS_OPT_GEMM   3 = weights stationary in shared memory, persistent, X through TMA rings (one per
+ *                   consumer warpgroup, 4-16 stages of 8 KB), A fragments in registers, two ping-pong consumer
+ *                   warpgroups (option 2 when the tensor map cannot be encoded), 2 = the same weights with a cp.async staging ring (2-3
+ *                   chunks in flight), 1 = option 2 with register prefetch,
  *                   0 = points-as-M with shared-memory operands (the kernel plain-TF32 mode uses)
- *   PMVS_OPT_DEBUG_IDX  1 = also materialise int32 neighbour indices in the workspace */
+ *   PMVS_OPT_DEBUG_IDX  1 = also materialise int32 neighbour indices in the workspace
+ *   PMVS_OPT_GEMM_STRICT  0 = off; 1 = under PMVS_OPT_GEMM 3, a contraction the TMA kernel does not take
+ *                   returns PMVS_ERR_ARG instead of running on option 2 (tests) */
 #define PMVS_OPT_EDGE 1
 #define PMVS_OPT_KNN 2
 #define PMVS_OPT_FETCH 3
 #define PMVS_OPT_GEMM 4
 #define PMVS_OPT_DEBUG_IDX 5
+#define PMVS_OPT_GEMM_STRICT 6
 int pmvs_set_option(int key, int value);
 int pmvs_get_option(int key);
 

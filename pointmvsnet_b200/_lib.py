@@ -137,7 +137,7 @@ def set_gemm_mode(mode):
 
 
 # implementation switches (include/pmvs_b200.h PMVS_OPT_*): which kernel family serves a stage of the fused path
-OPTIONS = {"edge": 1, "knn": 2, "fetch": 3, "gemm": 4, "debug_idx": 5}
+OPTIONS = {"edge": 1, "knn": 2, "fetch": 3, "gemm": 4, "debug_idx": 5, "gemm_strict": 6}
 
 
 def set_option(name, value):

@@ -29,7 +29,7 @@ static struct OptDefaults {
     g_opt[OPT_EDGE].store(1);   // TMA halo-tile EdgeConv
     g_opt[OPT_KNN].store(1);    // batched sorting-network kNN
     g_opt[OPT_FETCH].store(1);  // texel-quad sharing fetch
-    g_opt[OPT_GEMM].store(2);   // weight-stationary persistent GEMM, cp.async staging ring
+    g_opt[OPT_GEMM].store(3);   // weight-stationary persistent GEMM, TMA ring, register-A wgmma, ping-pong
   }
 } g_opt_defaults;
 int opt(int key) { return (key >= 0 && key < OPT_COUNT) ? g_opt[key].load(std::memory_order_relaxed) : 0; }

@@ -76,8 +76,10 @@ enum {
                   // 2 = TMA halo tile 16x4x5
   OPT_KNN = 2,    // 0 = sorted insertion (round 1), 1 = batched sort + bitonic merge
   OPT_FETCH = 3,  // 0 = 4 taps per (hypothesis, view), 1 = hypotheses of a pixel share the texel quad when they can
-  OPT_GEMM = 4,   // 0 = points-as-M shared-memory operands (round 1), 1 / 2 = weights stationary in shared memory, persistent (gemm_ws.cu)
+  OPT_GEMM = 4,   // 0 = points-as-M shared-memory operands (round 1), 1 / 2 = weights stationary in shared memory, persistent
+                  // (gemm_ws.cu), 3 = the same weights with a TMA-fed X ring, register-A wgmma and ping-pong warpgroups
   OPT_DEBUG_IDX = 5,  // 1 = the fused path also materialises the int32 neighbour indices (tests)
+  OPT_GEMM_STRICT = 6,  // 1 = under OPT_GEMM 3, a contraction gemm_tma_kernel does not take is an error (tests)
   OPT_COUNT = 16
 };
 int opt(int key);

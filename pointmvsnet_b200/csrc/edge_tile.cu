@@ -19,9 +19,9 @@
 // s1 += d, s2 = fma(d, d, s2); apply fma(e, A, c0) with A = istd * gamma, c0 = beta - (mean + l) * A.
 // The statistics of the central half come from the GEMM epilogue (per-column sums of LE).
 #include <algorithm>
-#include <cuda.h>  // CUtensorMap and its enums only; cuTensorMapEncodeTiled is resolved at run time
 
 #include "common.cuh"
+#include "tensor_map.cuh"
 
 namespace pmvs {
 
@@ -32,23 +32,6 @@ constexpr int ET_WARPS = ET_THREADS / 32;
 constexpr int ET_CP = 32;            // channels per slab = one 128-byte row of the halo tile
 constexpr int ET_LPP = ET_CP / 4;    // 8 lanes per point
 constexpr int ET_PPW = 32 / ET_LPP;  // 4 points per warp step
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn encode_fn() {
-  static EncodeTiledFn fn = [] {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess ||
-        q != cudaDriverEntryPointSuccess)
-      p = nullptr;
-    cudaGetLastError();
-    return (EncodeTiledFn)p;
-  }();
-  return fn;
-}
 
 __device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
 
@@ -309,7 +292,7 @@ __global__ void __launch_bounds__(ET_THREADS, 3) edge_tile_kernel(const __grid_c
 template <int COUT, bool APPLY, int TX, int TY>
 int launch_variant(const EdgeTileArgs& a, cudaStream_t st) {
   using G = TileGeom<TX, TY>;
-  EncodeTiledFn enc = encode_fn();
+  EncodeTiledFn enc = encode_tiled_fn();
   if (enc == nullptr) {
     set_error("edge_tile: cuTensorMapEncodeTiled is not available from this driver");
     return PMVS_ERR_CUDA;

@@ -20,8 +20,10 @@
 //     and leave the CTA as one fp64 atomic per statistic and group.
 // Precision: as gemm_tc.cu - hi = the 10 explicit mantissa bits the tensor core reads, lo = x - hi (exact).
 #include <algorithm>
+#include <type_traits>
 
 #include "common.cuh"
+#include "tensor_map.cuh"
 #include "wgmma.cuh"
 
 namespace pmvs {
@@ -407,8 +409,356 @@ static int launch_pf(const GemmArgs& a, cudaStream_t st, const char* name) {
   gemm_ws_kernel<COUT, IN_BN, ASYNC, NSTAGES><<<grid, THREADS, smem_total, st>>>(a);
   return check_launch("gemm_ws_kernel", st);
 }
+// =============================== PMVS_OPT_GEMM = 3: TMA producer, register-A wgmma, ping-pong consumers ===========
+// The same weight planes and the same products as above, with a different path for X:
+//   * each consumer warpgroup owns every other 64-point tile of the CTA's range (ping-pong: one warpgroup's epilogue
+//     overlaps the other's MMAs) and has its own producer warp, ring and full / empty barriers.  One thread of the
+//     producer warp loads 64-row x 32-column boxes of X with the TMA (3-D tensor map (cin, rows, groups),
+//     SWIZZLE_128B; the ragged rows of a group and the K padding arrive as zeros) into the warpgroup's ring of 8 KB
+//     stages, completing on expect_tx barriers.  The two rings share the shared memory the weight planes leave (6 + 6
+//     stages for 224 -> 64).  A stage is only ever filled for and read by one warpgroup, in order, so a parity wait
+//     can never see the phase of another warpgroup's item, whatever order the TMA boxes complete in;
+//   * per chunk a consumer reads its wgmma A fragments straight from the swizzled stage (4 LDS.32 per k-step,
+//     conflict-free), applies the input BatchNorm+ReLU, splits hi / lo in registers and issues the chunk's MMAs as
+//     one wgmma group (the k-step count is a template parameter, so no branch separates them).  It waits for the
+//     group, then hands the stage back and the next chunk rewrites the fragments; the other warpgroup's MMAs and the
+//     producers' loads continue meanwhile.
+// No shared-memory copy of the converted operands exists any more: per 224 -> 64 chunk of 64 points, shared memory
+// carries the 8 KB the TMA writes, the 8 KB read into the fragments and the weight reads of the MMAs.
+// Every output element goes through the same instruction sequence as under option 2, so Y is identical; the output
+// statistics are summed in another order (fp64 per warpgroup and group instead of per CTA and tile).
+namespace tma {
+constexpr int NT = 64;                              // points per tile = one warpgroup's wgmma M
+constexpr int STAGE_BYTES = NT * KC * 4;            // one TMA box, 8 KB
+constexpr int CONS_THREADS = 256;                   // two consumer warpgroups
+constexpr int THREADS = CONS_THREADS + 64;          // + one producer warp per warpgroup (168 registers a thread)
+constexpr int MAX_STAGES = 32, MIN_STAGES = 8;      // both rings together; each warpgroup gets half
+constexpr int BN_FLOATS = (MAXK / KC) * 4 * 16;     // per warpgroup: [chunk][lane % 4][A x 8 | B x 8]
+// after the ring: BatchNorm tables and output sums of each warpgroup, then the full / empty barriers
+constexpr int TAIL_BN = 0, TAIL_RED = TAIL_BN + 2 * BN_FLOATS * 4;
+__host__ __device__ constexpr int tail_bar(int cout) { return TAIL_RED + 2 * 2 * cout * 8; }
+__host__ __device__ constexpr int tail_bytes(int cout) { return tail_bar(cout) + 2 * MAX_STAGES * 8; }
+__host__ __device__ constexpr int stages_for(int cin, int cout) {
+  return (SMEM_MAX - weight_bytes(cout, (cin + KC - 1) / KC) - tail_bytes(cout)) / STAGE_BYTES < MAX_STAGES
+             ? (SMEM_MAX - weight_bytes(cout, (cin + KC - 1) / KC) - tail_bytes(cout)) / STAGE_BYTES
+             : MAX_STAGES;
+}
+}  // namespace tma
+
+// one round of a reduce-scatter over lanes l, l ^ m: the lane keeps the half of its N values selected by lane bit m and
+// adds the partner's copy of that half (the sum of the pair is the one a butterfly step computes)
+template <int N>
+__device__ __forceinline__ void reduce_scatter_round(float* sv, int lane, int m) {
+  const bool up = (lane & m) != 0;
+#pragma unroll
+  for (int k = 0; k < N / 2; ++k) {
+    const float keep = up ? sv[k + N / 2] : sv[k], send = up ? sv[k] : sv[k + N / 2];
+    sv[k] = keep + __shfl_xor_sync(0xffffffffu, send, m);
+  }
+}
+
+template <int COUT, bool IN_BN>
+__global__ void __launch_bounds__(tma::THREADS, 1) gemm_tma_kernel(const __grid_constant__ CUtensorMap tmx,
+                                                                   const GemmArgs a, const int wstages) {
+  constexpr int NT = tma::NT, STAGE_BYTES = tma::STAGE_BYTES, CONS_THREADS = tma::CONS_THREADS;
+  constexpr int MAX_STAGES = tma::MAX_STAGES, BN_FLOATS = tma::BN_FLOATS, TAIL_BN = tma::TAIL_BN, TAIL_RED = tma::TAIL_RED;
+  constexpr bool STACKED = COUT <= 64;
+  constexpr int W_CHUNK = 2 * COUT * 128;
+  constexpr int ACC_REGS = (STACKED ? 2 * COUT : COUT) / 2;
+  constexpr int BLK = COUT < 64 ? COUT : 64;
+  extern __shared__ __align__(1024) unsigned char smem[];
+  const uint32_t smem_base = smem_u32(smem);
+
+  const int K = a.cin;
+  const int nch = (K + KC - 1) / KC;
+  const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
+  const int tpg = (a.rows_per_group + NT - 1) / NT;
+  const TileRange tr = my_tiles(a.groups * tpg);
+  // [weights | ring of warpgroup 0 | ring of warpgroup 1 | tail], each 1024-byte aligned
+  unsigned char* tail = smem + weight_bytes(COUT, nch) + 2 * wstages * STAGE_BYTES;
+  const uint32_t bar0 = smem_u32(tail + tma::tail_bar(COUT));
+  // barriers of stage s of warpgroup w's ring: full (one arrival + the TMA bytes), empty (one arrival per consumer warp)
+  auto bar_full = [&](int w, int s) { return bar0 + 8u * (uint32_t)(w * (MAX_STAGES / 2) + s); };
+  auto bar_empty = [&](int w, int s) { return bar0 + 8u * (uint32_t)(MAX_STAGES + w * (MAX_STAGES / 2) + s); };
+
+  if (tid == 0) {
+    for (int w = 0; w < 2; ++w)
+      for (int s = 0; s < wstages; ++s) {
+        mbar_init(bar_full(w, s), 1);
+        mbar_init(bar_empty(w, s), 4);
+      }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (warp >= CONS_THREADS / 32) {
+    // =============================== producers: one thread per warpgroup, TMA ==================================
+    // They start while the consumers are still writing the weight planes.
+    const int w = warp - CONS_THREADS / 32;
+    if (lane == 0) {
+      const uint32_t ring = smem_base + weight_bytes(COUT, nch) + w * wstages * STAGE_BYTES;
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int i = w; i < tr.count; i += 2) {
+        const int t = tr.first + i, g = t / tpg, row0 = (t - g * tpg) * NT;
+        for (int c = 0; c < nch; ++c) {
+          mbar_wait(bar_empty(w, stage), phase ^ 1u);
+          mbar_arrive_expect_tx(bar_full(w, stage), STAGE_BYTES);
+          tma_load_3d(ring + stage * STAGE_BYTES, &tmx, c * KC, row0, g, bar_full(w, stage));
+          if (++stage == wstages) {
+            stage = 0;
+            phase ^= 1u;
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // =============================== consumers ==========================================================
+  const int wgi = warp >> 2, wtid = tid & 127;
+  const uint32_t ring = smem_base + weight_bytes(COUT, nch) + wgi * wstages * STAGE_BYTES;
+  float* sBN = (float*)(tail + TAIL_BN) + wgi * BN_FLOATS;
+  double* sRed = (double*)(tail + TAIL_RED) + wgi * 2 * COUT;  // this warpgroup's [sum(COUT) | sumsq(COUT)] of a group
+  for (int i = wtid; i < 2 * COUT; i += 128) sRed[i] = 0.0;
+  // weights -> shared memory (B operand), as in gemm_ws_kernel
+  for (int e = tid; e < COUT * nch * 8; e += CONS_THREADS) {
+    const int n = e / (nch * 8), rem = e - n * (nch * 8), c = rem >> 3, pc = rem & 7;
+    const int k0 = c * KC + pc * 4;
+    const float4 v = k0 < K ? ldg4(a.w + (size_t)n * K + k0) : make_float4(0.f, 0.f, 0.f, 0.f);
+    float4 hi, lo;
+    hi.x = tf32_hi(v.x); hi.y = tf32_hi(v.y); hi.z = tf32_hi(v.z); hi.w = tf32_hi(v.w);
+    lo.x = __fsub_rn(v.x, hi.x); lo.y = __fsub_rn(v.y, hi.y); lo.z = __fsub_rn(v.z, hi.z); lo.w = __fsub_rn(v.w, hi.w);
+    const uint32_t dst = smem_base + c * W_CHUNK + swz128(n, pc);
+    sts128(dst, hi);
+    sts128(dst + COUT * 128, lo);
+  }
+  fence_proxy_async();
+  named_bar_sync(1, CONS_THREADS);
+
+  // this thread's A elements: rows r, r + 8 of the warpgroup's tile, columns 8 j + q (+ 4) of k-step j; in the
+  // swizzled box the 16-byte piece p of row r sits at piece p ^ (r & 7), and row r + 8 is 1024 bytes further
+  const int r = (warp & 3) * 16 + (lane >> 2), q = lane & 3;
+  const uint32_t fbase = r * 128 + q * 4, fx = (r & 7) << 4;
+  const int frow = r, fcol = 2 * q;  // accumulator fragment: rows frow, frow + 8, columns 8 i + fcol + {0, 1}
+  const uint32_t w_base = smem_base;
+  float acc[ACC_REGS];
+  uint32_t fh[16], fl[16];  // [4 j + e]: the hi / lo A fragments of the k-steps of a chunk
+  const uint32_t wg_bar = 2 + wgi;
+
+  // Output statistics.  Per tile, a warp's fp32 sums over its 16 rows are reduce-scattered over the 8 lanes that
+  // hold the same columns (the same pairings, lane ^ 4, then ^ 8, then ^ 16, as the butterfly of gemm_ws_kernel, so
+  // the same fp32 values), after which lane l owns NV statistics and adds them to fp64 registers.  The 4 warps meet
+  // in shared memory once per group.  Statistic of value k = 4 i + e (e: sum col, sum col + 1, sumsq col, sumsq col + 1
+  // of col = 8 i + fcol): lane l owns k = kofs + j, j < NV.
+  // cout = 128 runs this in two passes of 64 columns (i += 8 h), which keeps it within 168 registers.
+  constexpr int HC = COUT < 64 ? COUT : 64, NH = COUT / HC;
+  constexpr int NV = HC / 16;  // (HC / 8) x 4 values per lane, / 8 lanes
+  const int kofs = ((lane >> 2) & 1) * (8 * NV / 2) + ((lane >> 3) & 1) * (8 * NV / 4) + ((lane >> 4) & 1) * (8 * NV / 8);
+  double racc[NH][NV];
+#pragma unroll
+  for (int h = 0; h < NH; ++h)
+#pragma unroll
+    for (int j = 0; j < NV; ++j) racc[h][j] = 0.0;
+  auto flush = [&](int g) {  // the warpgroup's sums of group g -> global memory, once per statistic
+    if (a.out_stats == nullptr) return;
+#pragma unroll
+    for (int h = 0; h < NH; ++h)
+#pragma unroll
+      for (int j = 0; j < NV; ++j) {
+        const int k = kofs + j, i = (k >> 2) + h * (HC / 8), e = k & 3;
+        atomicAdd(&sRed[(e >> 1) * COUT + 8 * i + fcol + (e & 1)], racc[h][j]);
+        racc[h][j] = 0.0;
+      }
+    named_bar_sync(wg_bar, 128);
+    for (int s = wtid; s < 2 * COUT; s += 128) {
+      atomicAdd(a.out_stats + (size_t)g * 2 * a.cout + s, sRed[s]);
+      sRed[s] = 0.0;
+    }
+  };
+
+  // chunk c of the current tile (item m of this warpgroup's ring) with KSTEPS k-steps
+  auto chunk = [&](auto KSTEPS, int c, int m) {
+    constexpr int ksteps = decltype(KSTEPS)::value;
+    const int stage = m % wstages;
+    mbar_wait(bar_full(wgi, stage), (uint32_t)((m / wstages) & 1));
+    const uint32_t st = ring + stage * STAGE_BYTES + fbase;
+    float bA[8], bB[8];
+    if (IN_BN) {
+      const float4* t4 = reinterpret_cast<const float4*>(sBN + (c * 4 + q) * 16);
+      const float4 a0 = t4[0], a1 = t4[1], b0 = t4[2], b1 = t4[3];
+      bA[0] = a0.x; bA[1] = a0.y; bA[2] = a0.z; bA[3] = a0.w; bA[4] = a1.x; bA[5] = a1.y; bA[6] = a1.z; bA[7] = a1.w;
+      bB[0] = b0.x; bB[1] = b0.y; bB[2] = b0.z; bB[3] = b0.w; bB[4] = b1.x; bB[5] = b1.y; bB[6] = b1.z; bB[7] = b1.w;
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      if (j < ksteps) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint32_t addr = st + ((uint32_t)((2 * j + h) << 4) ^ fx);
+          float v[2];
+          asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v[0]) : "r"(addr) : "memory");
+          asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v[1]) : "r"(addr + 1024) : "memory");
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            float x = v[e];
+            if (IN_BN) x = fmaxf(fmaf(x, bA[2 * j + h], bB[2 * j + h]), 0.f);
+            const float hi = tf32_hi(x);
+            fh[4 * j + 2 * h + e] = __float_as_uint(hi);
+            fl[4 * j + 2 * h + e] = __float_as_uint(__fsub_rn(x, hi));
+          }
+        }
+      }
+    }
+    fence();
+    const uint32_t w_hi = w_base + c * W_CHUNK, w_lo = w_hi + COUT * 128;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      if (j < ksteps) {
+        const uint32_t first = (c | j) != 0 ? 1u : 0u;
+        if (STACKED) {
+          mma_tile_ra<2 * COUT, BLK>(acc, &fh[4 * j], w_hi + j * 32, first);
+          mma_tile_ra<COUT, BLK>(acc + COUT / 2, &fl[4 * j], w_hi + j * 32, 1u);
+        } else {
+          mma_tile_ra<COUT, BLK>(acc, &fl[4 * j], w_hi + j * 32, first);
+          mma_tile_ra<COUT, BLK>(acc, &fh[4 * j], w_lo + j * 32, 1u);
+          mma_tile_ra<COUT, BLK>(acc, &fh[4 * j], w_hi + j * 32, 1u);
+        }
+      }
+    }
+    commit();
+    // The next chunk rewrites the fragments.  A second fragment buffer (wait_group 1) does not fit: ptxas then
+    // serialises every wgmma for lack of registers.  The other warpgroup's MMAs fill the tensor pipe meanwhile.
+    wait<0>();
+    fence_regs(fh);
+    fence_regs(fl);
+    // The stage goes back to the producer only now.  Released straight after the loads, the arrive was scheduled
+    // ahead of the loads' results and the TMA could overwrite data that had not been read yet.  The fragments went
+    // through the MMAs just waited for, so every value read from the stage has arrived.
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bar_empty(wgi, stage));
+  };
+  // only the last chunk of a K that is not a multiple of 32 (136: one k-step) has fewer than 4 k-steps
+  auto chunk_ks = [&](int c, int m) {
+    switch (min(KC, K - c * KC) / 8) {
+      case 4: chunk(std::integral_constant<int, 4>(), c, m); break;
+      case 3: chunk(std::integral_constant<int, 3>(), c, m); break;
+      case 2: chunk(std::integral_constant<int, 2>(), c, m); break;
+      default: chunk(std::integral_constant<int, 1>(), c, m); break;
+    }
+  };
+
+  int cur_g = -1;
+  for (int i = wgi; i < tr.count; i += 2) {
+    const int t = tr.first + i;
+    const int g = t / tpg, row0 = (t - g * tpg) * NT;
+    const int rows_valid = min(NT, a.rows_per_group - row0);
+    const size_t grow0 = (size_t)g * a.rows_per_group + row0;
+    if (g != cur_g) {
+      named_bar_sync(wg_bar, 128);  // the warpgroup is done with the previous group's tables and sums
+      if (cur_g >= 0) flush(cur_g);
+      if (IN_BN) {
+        // relu(fma(x, A, B)) coefficients as in gemm_ws_kernel, laid out per (chunk, lane % 4); zero beyond K
+        const double* s = a.in_stats + (size_t)g * 2 * K;
+        for (int e = wtid; e < nch * 64; e += 128) {
+          const int c = e >> 6, qq = (e >> 4) & 3, k = e & 15, jh = k & 7;
+          const int col = c * KC + 8 * (jh >> 1) + qq + 4 * (jh & 1);
+          float val = 0.f;
+          if (col < K) {
+            const BnCoef bc = bn_coef(s[col], s[K + col], a.in_count, a.eps);
+            const float A = __fmul_rn(bc.invstd, a.in_gamma[col]);
+            val = k < 8 ? A : fmaf(-bc.mean, A, a.in_beta[col]);
+          }
+          sBN[e] = val;
+        }
+      }
+      named_bar_sync(wg_bar, 128);
+      cur_g = g;
+    }
+    const int m0 = (i >> 1) * nch;  // this warpgroup's ring items of the tile
+    for (int c = 0; c < nch; ++c) chunk_ks(c, m0 + c);
+    fence_regs(acc);
+    // ---- epilogue from the fragments, as in gemm_ws_kernel ----
+    const bool ok0 = frow < rows_valid, ok1 = frow + 8 < rows_valid;
+    float* y0 = a.y + (grow0 + frow) * a.ldy + fcol;
+    float* y1 = y0 + (size_t)8 * a.ldy;
+#pragma unroll
+    for (int h = 0; h < NH; ++h) {
+      float sv[HC / 2];  // this thread's per-tile sums of columns [64 h, 64 h + HC): k = 4 (i - 8 h) + e
+#pragma unroll
+      for (int il = 0; il < HC / 8; ++il) {
+        const int ii = h * (HC / 8) + il;
+        float v[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) v[e] = STACKED ? acc[4 * ii + e] + acc[COUT / 2 + 4 * ii + e] : acc[4 * ii + e];
+        if (ok0) *reinterpret_cast<float2*>(y0 + 8 * ii) = make_float2(v[0], v[1]);
+        if (ok1) *reinterpret_cast<float2*>(y1 + 8 * ii) = make_float2(v[2], v[3]);
+        if (!ok0) v[0] = v[1] = 0.f;
+        if (!ok1) v[2] = v[3] = 0.f;
+        sv[4 * il + 0] = v[0] + v[2];
+        sv[4 * il + 1] = v[1] + v[3];
+        sv[4 * il + 2] = fmaf(v[0], v[0], v[2] * v[2]);
+        sv[4 * il + 3] = fmaf(v[1], v[1], v[3] * v[3]);
+      }
+      if (a.out_stats != nullptr) {
+        // reduce-scatter: in each round a lane keeps the half of its values selected by one lane bit and adds the
+        // partner's copy of that half
+        reduce_scatter_round<HC / 2>(sv, lane, 4);
+        reduce_scatter_round<HC / 4>(sv, lane, 8);
+        reduce_scatter_round<HC / 8>(sv, lane, 16);
+#pragma unroll
+        for (int j = 0; j < NV; ++j) racc[h][j] += (double)sv[j];
+      }
+    }
+  }
+  if (cur_g >= 0) flush(cur_g);
+}
+
+// Ring depth of the six contractions of a PointFlow iteration: growing the tail tables or the weight planes, or a
+// static __shared__ variable (which would also break the 1024-byte alignment of the swizzled planes), shows up here,
+// not as a silently shallower ring.  224 -> 64 gets 6 + 6 stages.
+static_assert(tma::stages_for(136, 64) >= tma::MIN_STAGES && tma::stages_for(32, 64) >= tma::MIN_STAGES &&
+                  tma::stages_for(64, 128) >= tma::MIN_STAGES && tma::stages_for(224, 64) >= tma::MIN_STAGES &&
+                  tma::stages_for(64, 64) >= tma::MIN_STAGES && tma::stages_for(64, 16) >= tma::MIN_STAGES,
+              "a hot-path GEMM shape no longer gets the minimum ring depth of gemm_tma_kernel");
+
+// -1: this shape or argument set does not suit the kernel (the caller uses option 2, or reports an error under
+// PMVS_OPT_GEMM_STRICT)
+template <int COUT, bool IN_BN>
+static int launch_tma(const GemmArgs& a, cudaStream_t st, const char* name) {
+  const int stages = tma::stages_for(a.cin, COUT);
+  if (stages < tma::MIN_STAGES) return -1;
+  const int wstages = stages / 2;
+  const unsigned long long row_bytes = (unsigned long long)a.ldx * 4, group_bytes = row_bytes * a.rows_per_group;
+  if (group_bytes >= (1ull << 40) || (unsigned long long)a.groups > 0xffffffffull) return -1;
+  EncodeTiledFn enc = encode_tiled_fn();
+  if (enc == nullptr) return -1;
+  // X as (cin, rows_per_group, groups): columns >= cin and rows >= rows_per_group of a box read as zeros
+  CUtensorMap tm;
+  const cuuint64_t gdim[3] = {(cuuint64_t)a.cin, (cuuint64_t)a.rows_per_group, (cuuint64_t)a.groups};
+  const cuuint64_t gstr[2] = {row_bytes, group_bytes};
+  const cuuint32_t box[3] = {KC, tma::NT, 1};
+  const cuuint32_t estr[3] = {1, 1, 1};
+  if (enc(&tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(a.x), gdim, gstr, box, estr,
+          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+    return -1;
+  const int smem_total = weight_bytes(COUT, cdiv(a.cin, KC)) + 2 * wstages * tma::STAGE_BYTES + tma::tail_bytes(COUT);
+  static unsigned long long smem_done = 0;
+  PMVS_TRY((ensure_dyn_smem(gemm_tma_kernel<COUT, IN_BN>, SMEM_MAX, smem_done, "gemm_tma")));
+  const long long tiles = (long long)a.groups * cdiv(a.rows_per_group, tma::NT);
+  const int grid = (int)std::min<long long>(tiles, sm_count());
+  prof_begin(name, st);
+  gemm_tma_kernel<COUT, IN_BN><<<grid, tma::THREADS, smem_total, st>>>(tm, a, wstages);
+  return check_launch("gemm_tma_kernel", st);
+}
+
 template <int COUT, bool IN_BN>
 static int launch_one(const GemmArgs& a, cudaStream_t st, const char* name) {
+  if (opt(OPT_GEMM) == 3) {
+    const int rc = launch_tma<COUT, IN_BN>(a, st, name);
+    if (rc >= 0 || opt(OPT_GEMM_STRICT)) return rc;
+  }
   // The weight planes take 2 * cout * 128 bytes per 32-column chunk of K (112 KB for 224 -> 64), the rings get the
   // rest of the 227 KB: deeper rings for the shapes with K <= 160.
   const bool deep = a.cin <= DEEP_K;
@@ -420,8 +770,7 @@ static int launch_one(const GemmArgs& a, cudaStream_t st, const char* name) {
 
 }  // namespace ws
 
-// returns -1 when this path does not apply (caller falls back to gemm_tc / SIMT)
-int launch_gemm_ws(const GemmArgs& a, cudaStream_t st, const char* name) {
+static int launch_gemm_ws_any(const GemmArgs& a, cudaStream_t st, const char* name) {
   if (a.cin % 8 != 0 || a.cin > ws::MAXK || a.ldx % 4 != 0 || a.ldy % 2 != 0 || a.groups <= 0 || a.rows_per_group <= 0) return -1;
   if (((uintptr_t)a.x & 15) || ((uintptr_t)a.w & 15) || ((uintptr_t)a.y & 7)) return -1;
   if ((long long)a.groups * cdiv(a.rows_per_group, ws::NT) >= (1ll << 31) / ws::MAXK) return -1;
@@ -433,6 +782,18 @@ int launch_gemm_ws(const GemmArgs& a, cudaStream_t st, const char* name) {
     case 128: return bn ? ws::launch_one<128, true>(a, st, name) : ws::launch_one<128, false>(a, st, name);
   }
   return -1;
+}
+
+// returns -1 when this path does not apply (caller falls back to gemm_tc / SIMT); under PMVS_OPT_GEMM = 3 with
+// PMVS_OPT_GEMM_STRICT = 1 a launch that gemm_tma_kernel does not take is an error instead
+int launch_gemm_ws(const GemmArgs& a, cudaStream_t st, const char* name) {
+  const int rc = launch_gemm_ws_any(a, st, name);
+  if (rc < 0 && opt(OPT_GEMM) == 3 && opt(OPT_GEMM_STRICT)) {
+    set_error("gemm: gemm_tma_kernel does not take cin %d, cout %d, ldx %d, %d groups of %d rows (strict mode)", a.cin,
+              a.cout, a.ldx, a.groups, a.rows_per_group);
+    return PMVS_ERR_ARG;
+  }
+  return rc;
 }
 
 }  // namespace pmvs

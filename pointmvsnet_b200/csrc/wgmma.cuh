@@ -31,6 +31,16 @@ __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+// TMA: the box of a 3-D tensor map at (c0, c1, c2) -> shared memory, completion counted in bytes on `bar`
+__device__ __forceinline__ void tma_load_3d(uint32_t dst, const void* tmap, int c0, int c1, int c2, uint32_t bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
+      ::"r"(dst), "l"(tmap), "r"(c0), "r"(c1), "r"(c2), "r"(bar)
+      : "memory");
+}
 
 // byte offset of 16-byte piece `pc` of row `r` inside a K-major SWIZZLE_128B plane
 __device__ __forceinline__ int swz128(int r, int pc) { return (r >> 3) * 1024 + (r & 7) * 128 + ((pc ^ (r & 7)) << 4); }
@@ -106,6 +116,67 @@ __device__ __forceinline__ void mma_tile(float* d, uint32_t a_addr, uint32_t b_a
 #pragma unroll
   for (int nb = 0; nb < N / BLK; ++nb)
     mma_tf32<BLK>(d + (BLK / 2) * nb, make_desc(a_addr), make_desc(b_addr + nb * BLK * 128), accumulate);
+}
+
+// ---- A operand in registers -------------------------------------------------------------------------------------
+// Thread t = 32 * w + l of the warpgroup holds a[0..3] = A[16 w + l / 4][l % 4], A[16 w + l / 4 + 8][l % 4],
+// A[16 w + l / 4][l % 4 + 4], A[16 w + l / 4 + 8][l % 4 + 4] (tf32 bit patterns).  The registers are read
+// asynchronously: they must not change before the instruction's group has been waited for.
+template <int N>
+__device__ __forceinline__ void wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+template <int R>
+__device__ __forceinline__ void fence_regs(uint32_t (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+r"(d[i])::"memory");
+}
+
+template <int N>
+__device__ __forceinline__ void mma_tf32_ra(float* d, const uint32_t* a, uint64_t bdesc, uint32_t accumulate);
+template <>
+__device__ __forceinline__ void mma_tf32_ra<16>(float* d, const uint32_t* a, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7}, "
+      "{%8, %9, %10, %11}, %12, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]),
+        "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
+template <>
+__device__ __forceinline__ void mma_tf32_ra<32>(float* d, const uint32_t* a, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+      "{%16, %17, %18, %19}, %20, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]),
+        "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+        "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
+template <>
+__device__ __forceinline__ void mma_tf32_ra<64>(float* d, const uint32_t* a, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "{%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]),
+        "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+        "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]),
+        "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]),
+        "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
+// mma_tile with the A fragment in registers
+template <int N, int BLK>
+__device__ __forceinline__ void mma_tile_ra(float* d, const uint32_t* a, uint32_t b_addr, uint32_t accumulate) {
+  static_assert(N % BLK == 0 && (BLK == 16 || BLK == 32 || BLK == 64), "block shape");
+#pragma unroll
+  for (int nb = 0; nb < N / BLK; ++nb) mma_tf32_ra<BLK>(d + (BLK / 2) * nb, a, make_desc(b_addr + nb * BLK * 128), accumulate);
 }
 
 }  // namespace wg
