@@ -9,6 +9,13 @@ and the committed golden vectors.  Tolerances (fp32, stated per stage):
   EdgeConv / EdgeConvNoC ........ atol 2e-5 + rtol 1e-4   (fp32 FMA order)
   depth after one iteration ..... atol 5e-4 mm (< 5e-5 * interval; depths ~650 mm, ulp 6e-5)
   flow probabilities ............ atol 5e-5
+
+The fused path after the kNN is checked stage by stage against float64 in tests/test_gpu_fused_stages.py:
+  fused EdgeConv columns ........ atol 2e-5 + rtol 1e-4, plus the fp32 rounding of the pre-BN values and of the
+                                  raw-moment BN sums, amplified by gamma * invstd (matters only for N = 5)
+  h2 ............................ |err| / (per-group column std) <= 1e-4
+  head .......................... probabilities 5e-5, depth 5e-5 * interval
+  running statistics (all six) .. atol 1e-5 + rtol 1e-4, num_batches_tracked exact
 """
 import numpy as np
 import pytest
