@@ -161,6 +161,29 @@ int pmvs_edgeconv_pm(const float* x, int ldx, const int32_t* idx32, const float*
                      int groups, int rows_per_group, int N, int K, int cin, int cout,
                      pmvs_stream_t stream);
 
+/* Backward of pmvs_edgeconv_pm for ONE BatchNorm group of B*N rows (B clouds of N points; the
+ * neighbour indices are local to a cloud).  Inputs are what the forward used or produced: x [B*N, ldx]
+ * points-major, idx32 [B*N, K] and the same indices as int64 idx64 (for the inverse neighbour lists),
+ * w12 [2*cout, cin], gamma/beta, le [B*N, 2*cout] (le_scratch after the forward) and stats [4*cout]
+ * fp64 (stats_scratch after the forward: the batch sums when bn_train != 0, the caller's running-
+ * statistic sums when bn_train == 0).  dy [B*N, lddy] is the points-major gradient of `out`.
+ * Outputs: dx [B*N, lddx] points-major (NULL: not computed), dw12 [2*cout, cin], dgamma/dbeta (same
+ * length as gamma).  The ReLU mask is recomputed from le and stats with the forward's arithmetic.
+ * bn_train == 0 (frozen statistics): the batch-statistic terms of the BatchNorm backward are zero.
+ * Deterministic: every sum has a fixed order (per-CTA partials over a fixed row partition combined
+ * in order, inverse neighbour lists sorted by source position, weight gradients over fixed 1024-row
+ * slabs), so the result is the same bits on every run and any H100.  Shape limits as the forward:
+ * cout in {16, 32, 64, 128}, cin % 8 == 0, cin <= 224, B*N*K < 2^31; ldx, lddy, lddx multiples of 4.
+ * workspace: pmvs_edgeconv_pm_backward_workspace_bytes(B, N, K, cin, cout) bytes (0 = unsupported
+ * shape), 256-byte aligned, device memory. */
+size_t pmvs_edgeconv_pm_backward_workspace_bytes(int B, int N, int K, int cin, int cout);
+int pmvs_edgeconv_pm_backward(const float* x, int ldx, const int32_t* idx32, const int64_t* idx64,
+                              const float* w12, const float* gamma, const float* beta, float eps,
+                              int concat_central, int bn_train, const float* le, const double* stats,
+                              const float* dy, int lddy, float* dx, int lddx, float* dw12,
+                              float* dgamma, float* dbeta, void* workspace, size_t workspace_bytes,
+                              int B, int N, int K, int cin, int cout, pmvs_stream_t stream);
+
 /* ---- a14 building block: 1x1 convolution on points-major rows (nn/conv.py:21-30) ---------- */
 /* y[r, 0:cout] = f(x[r, 0:cin]) * w[cout, cin]^T over groups * rows_per_group rows.
  * Optional fused input BatchNorm(batch statistics)+ReLU: in_stats [groups, 2*cin] fp64 sums and

@@ -116,6 +116,14 @@ __device__ __forceinline__ BnCoef bn_coef(double s1, double s2, double count, fl
 __device__ __forceinline__ float bn_apply(float x, float mean, float invstd, float g, float b) {
   return __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(x, mean), invstd), g), b);
 }
+// EdgeConv neighbour half: ((e - local - mean) * invstd) * gamma + beta evaluated as one FMA per gathered value,
+// pre = e * A + c0 with A = invstd * gamma and c0 = beta - (mean + local) * A.  The forward (edge_kernel) and the
+// backward (edge_bwd.cu, which recomputes the ReLU mask) both use these, so the two masks agree bit for bit.
+__device__ __forceinline__ float edge_nb_scale(float invstd, float gamma) { return __fmul_rn(invstd, gamma); }
+__device__ __forceinline__ float edge_nb_offset(float mean, float local, float A, float beta) {
+  return __fmaf_rn(-__fadd_rn(mean, local), A, beta);
+}
+__device__ __forceinline__ float edge_nb_pre(float e, float A, float c0) { return __fmaf_rn(e, A, c0); }
 
 // ---- internal launchers shared between translation units ---------------------------
 // knn3d of the fused path (ksize 5, knn 16): 16-bit neighbour codes [clouds*D*H*W, 16] (knn3d.cu knn_code16: halo-tile
@@ -163,6 +171,14 @@ struct EdgeArgs {
 };
 int launch_edge_stats(const EdgeArgs& a, cudaStream_t st);
 int launch_edge_apply(const EdgeArgs& a, cudaStream_t st);
+
+// Inverse neighbour lists of B clouds of N points with K neighbours each (gather_det.cu): for every point j of cloud b,
+// list[b*N*K + off[b*(N+1)+j] .. off[b*(N+1)+j+1]) holds the source positions p = n*K + k with idx[b,n,k] == j in
+// ascending order.  Out-of-range entries are skipped.  ws: inv_lists_bytes(B, N, K) bytes, 256-byte aligned.
+// prof_name != NULL brackets every launch for pmvs_profile_enable.
+size_t inv_lists_bytes(long long B, long long N, long long K);
+int build_inv_lists(const int64_t* idx, int B, int N, int K, void* ws, const int** off, const int** list,
+                    const char* prof_name, cudaStream_t st);
 
 // EdgeConv statistics / apply on a structured cloud, neighbour rows gathered from a TMA-loaded
 // shared-memory halo tile (edge_tile.cu)

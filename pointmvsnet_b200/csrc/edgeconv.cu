@@ -182,7 +182,9 @@ int launch_gemm(const GemmArgs& a, cudaStream_t st) {
   PMVS_REQUIRE(a.groups <= 65535, "gemm: too many groups");
   const int tiles = cdiv(a.rows_per_group, G_BM);
   static const char* const names[] = {"gemm_136x64", "gemm_32x64", "gemm_64x128", "gemm_224x64",
-                                      "gemm_64x64", "gemm_64x16", "gemm_other"};
+                                      "gemm_64x64", "gemm_64x16", "gemm_other",
+                                      // also the dX = dLE * W12 shapes of the model's EdgeConv backward (edge_bwd.cu)
+                                      "gemm_64x136", "gemm_64x32", "gemm_128x64"};
   int ni = 6;
   if (a.cin == 136 && a.cout == 64) ni = 0;
   else if (a.cin == 32 && a.cout == 64) ni = 1;
@@ -190,6 +192,9 @@ int launch_gemm(const GemmArgs& a, cudaStream_t st) {
   else if (a.cin == 224 && a.cout == 64) ni = 3;
   else if (a.cin == 64 && a.cout == 64) ni = 4;
   else if (a.cin == 64 && a.cout == 16) ni = 5;
+  else if (a.cin == 64 && a.cout == 136) ni = 7;
+  else if (a.cin == 64 && a.cout == 32) ni = 8;
+  else if (a.cin == 128 && a.cout == 64) ni = 9;
   if (opt(OPT_GEMM) != 0 && pmvs_get_gemm_mode() == 3) {
     const int rc = launch_gemm_ws(a, st, names[ni]);
     if (rc >= 0) return rc;
@@ -260,24 +265,25 @@ __global__ void __launch_bounds__(E_THREADS) edge_kernel(const EdgeArgs a) {
     const int32_t* ip = a.idx + row * K;
     float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
     // apply: ((d - mean) * istd) * gamma + beta with d = e - loc is evaluated as fma(e, A, c0),
-    // A = istd * gamma, c0 = beta - (mean + loc) * A  (one FFMA per gathered value)
+    // A = istd * gamma, c0 = beta - (mean + loc) * A  (one FFMA per gathered value; common.cuh edge_nb_*)
     float4 A4, c0;
     if (APPLY) {
       const float4 m = *reinterpret_cast<const float4*>(&c_mean[1][cl]);
       const float4 is = *reinterpret_cast<const float4*>(&c_istd[1][cl]);
       const float4 gm = *reinterpret_cast<const float4*>(&c_g[1][cl]);
       const float4 bt = *reinterpret_cast<const float4*>(&c_b[1][cl]);
-      A4 = make_float4(is.x * gm.x, is.y * gm.y, is.z * gm.z, is.w * gm.w);
-      c0 = make_float4(fmaf(-(m.x + loc.x), A4.x, bt.x), fmaf(-(m.y + loc.y), A4.y, bt.y),
-                       fmaf(-(m.z + loc.z), A4.z, bt.z), fmaf(-(m.w + loc.w), A4.w, bt.w));
+      A4 = make_float4(edge_nb_scale(is.x, gm.x), edge_nb_scale(is.y, gm.y), edge_nb_scale(is.z, gm.z),
+                       edge_nb_scale(is.w, gm.w));
+      c0 = make_float4(edge_nb_offset(m.x, loc.x, A4.x, bt.x), edge_nb_offset(m.y, loc.y, A4.y, bt.y),
+                       edge_nb_offset(m.z, loc.z, A4.z, bt.z), edge_nb_offset(m.w, loc.w, A4.w, bt.w));
     }
     auto body = [&](int nb) {
       const float4 e = ldg4(a.le + (cloud_base + nb) * LD + COUT + cl);
       if (APPLY) {
-        o.x += fmaxf(fmaf(e.x, A4.x, c0.x), 0.f);
-        o.y += fmaxf(fmaf(e.y, A4.y, c0.y), 0.f);
-        o.z += fmaxf(fmaf(e.z, A4.z, c0.z), 0.f);
-        o.w += fmaxf(fmaf(e.w, A4.w, c0.w), 0.f);
+        o.x += fmaxf(edge_nb_pre(e.x, A4.x, c0.x), 0.f);
+        o.y += fmaxf(edge_nb_pre(e.y, A4.y, c0.y), 0.f);
+        o.z += fmaxf(edge_nb_pre(e.z, A4.z, c0.z), 0.f);
+        o.w += fmaxf(edge_nb_pre(e.w, A4.w, c0.w), 0.f);
       } else {
         const float dx = __fsub_rn(e.x, loc.x), dy = __fsub_rn(e.y, loc.y);
         const float dz = __fsub_rn(e.z, loc.z), dw = __fsub_rn(e.w, loc.w);

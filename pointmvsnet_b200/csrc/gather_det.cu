@@ -159,13 +159,52 @@ DetPlan det_plan(long long B, long long N, long long K) {
 
 }  // namespace
 
+size_t inv_lists_bytes(long long B, long long N, long long K) { return det_plan(B, N, K).total; }
+
+// count -> exclusive scan -> fill -> sort; shared by pmvs_gather_knn_backward_det and pmvs_edgeconv_pm_backward
+int build_inv_lists(const int64_t* idx, int B, int N, int K, void* workspace, const int** off_out,
+                    const int** list_out, const char* prof_name, cudaStream_t st) {
+  const DetPlan p = det_plan(B, N, K);
+  char* ws = (char*)workspace;
+  int* cnt = (int*)(ws + p.cnt);
+  int* cur = (int*)(ws + p.cur);
+  int* off = (int*)(ws + p.off);
+  int* list = (int*)(ws + p.list);
+  *off_out = off;
+  *list_out = list;
+  if (cudaMemsetAsync(cnt, 0, p.off - p.cnt, st) != cudaSuccess) {  // cnt and cur are adjacent
+    set_error("gather_knn_backward_det: memset failed");
+    return PMVS_ERR_CUDA;
+  }
+  cudaStream_t pst = prof_name ? st : nullptr;  // check_launch closes the profiling record on this stream
+  const long long NK = (long long)N * K, entries = (long long)B * NK, rows = (long long)B * N;
+  auto blocks = [](long long n) { return (int)std::min<long long>(std::max<long long>(cdiv(n, GD_THREADS), 1), sm_count() * 16); };
+  if (entries > 0) {
+    if (prof_name) prof_begin(prof_name, st);
+    gd_count_kernel<<<blocks(entries), GD_THREADS, 0, st>>>(idx, cnt, entries, N, NK);
+    PMVS_TRY(check_launch("gd_count_kernel", pst));
+  }
+  if (prof_name) prof_begin(prof_name, st);
+  gd_scan_kernel<<<B, 1024, 0, st>>>(cnt, off, N);
+  PMVS_TRY(check_launch("gd_scan_kernel", pst));
+  if (entries > 0) {
+    if (prof_name) prof_begin(prof_name, st);
+    gd_fill_kernel<<<blocks(entries), GD_THREADS, 0, st>>>(idx, off, cur, list, entries, N, NK);
+    PMVS_TRY(check_launch("gd_fill_kernel", pst));
+    if (prof_name) prof_begin(prof_name, st);
+    gd_sort_kernel<<<(int)cdiv(rows, GD_THREADS), GD_THREADS, 0, st>>>(off, list, rows, N, NK);
+    PMVS_TRY(check_launch("gd_sort_kernel", pst));
+  }
+  return PMVS_OK;
+}
+
 }  // namespace pmvs
 
 using namespace pmvs;
 
 extern "C" size_t pmvs_gather_knn_backward_det_workspace_bytes(int B, int N, int K) {
   if (B < 0 || N < 0 || K < 0) return 0;
-  return det_plan(B, N, K).total + 256;
+  return inv_lists_bytes(B, N, K) + 256;
 }
 
 extern "C" int pmvs_gather_knn_backward_det(const float* grad_output, const int64_t* index, float* grad_input, int B,
@@ -177,37 +216,19 @@ extern "C" int pmvs_gather_knn_backward_det(const float* grad_output, const int6
   PMVS_REQUIRE(grad_input && (index || (long long)N * K == 0), "gather_knn_backward_det: NULL pointer");
   PMVS_REQUIRE((long long)B * N * K < (1ll << 31) && (long long)B * (N + 1) < (1ll << 31),
                "gather_knn_backward_det: B*N*K must be below 2^31");
-  const DetPlan p = det_plan(B, N, K);
+  const size_t need = inv_lists_bytes(B, N, K);
   PMVS_REQUIRE(workspace != nullptr && ((uintptr_t)workspace & 255) == 0, "gather_knn_backward_det: workspace must be 256-byte aligned");
-  if (workspace_bytes < p.total) {
-    set_error("gather_knn_backward_det: workspace %zu bytes < required %zu", workspace_bytes, p.total);
+  if (workspace_bytes < need) {
+    set_error("gather_knn_backward_det: workspace %zu bytes < required %zu", workspace_bytes, need);
     return PMVS_ERR_WORKSPACE;
   }
   cudaStream_t st = (cudaStream_t)stream;
-  char* ws = (char*)workspace;
-  int* cnt = (int*)(ws + p.cnt);
-  int* cur = (int*)(ws + p.cur);
-  int* off = (int*)(ws + p.off);
-  int* list = (int*)(ws + p.list);
-  if (cudaMemsetAsync(cnt, 0, p.off - p.cnt, st) != cudaSuccess) {  // cnt and cur are adjacent
-    set_error("gather_knn_backward_det: memset failed");
-    return PMVS_ERR_CUDA;
-  }
-  const long long NK = (long long)N * K, entries = (long long)B * NK, rows = (long long)B * N;
+  const int* off = nullptr;
+  const int* list = nullptr;
+  PMVS_TRY(build_inv_lists(index, B, N, K, workspace, &off, &list, nullptr, st));
+  const long long NK = (long long)N * K, rows = (long long)B * N;
   const long long outs = rows * C;
   auto blocks = [](long long n) { return (int)std::min<long long>(std::max<long long>(cdiv(n, GD_THREADS), 1), sm_count() * 16); };
-  if (entries > 0) {
-    gd_count_kernel<<<blocks(entries), GD_THREADS, 0, st>>>(index, cnt, entries, N, NK);
-    PMVS_TRY(check_launch("gd_count_kernel"));
-  }
-  gd_scan_kernel<<<B, 1024, 0, st>>>(cnt, off, N);
-  PMVS_TRY(check_launch("gd_scan_kernel"));
-  if (entries > 0) {
-    gd_fill_kernel<<<blocks(entries), GD_THREADS, 0, st>>>(index, off, cur, list, entries, N, NK);
-    PMVS_TRY(check_launch("gd_fill_kernel"));
-    gd_sort_kernel<<<(int)cdiv(rows, GD_THREADS), GD_THREADS, 0, st>>>(off, list, rows, N, NK);
-    PMVS_TRY(check_launch("gd_sort_kernel"));
-  }
   gd_reduce_kernel<<<blocks(outs), GD_THREADS, 0, st>>>(grad_output, off, list, grad_input, outs, C, N, NK);
   return check_launch("gd_reduce_kernel");
 }

@@ -3,15 +3,33 @@
 Same constructor, parameter names (``conv1``, ``conv2``, ``bn``) and forward signature as
 the reference, so its checkpoints load unchanged.  The forward runs three sm_90a kernels
 (GEMM, gathered-difference statistics, normalise + ReLU + mean over K) on points-major
-data; the [B,C,N,K] tensors of the reference are never materialised.  Forward only: the
-backward of the fused layer is a later row of the scope table (SURVEY.md section 8f)."""
+data; the [B,C,N,K] tensors of the reference are never materialised.
+
+By default the layers are forward-only and raise under autograd.  ``enable_backward()`` turns on a fused, deterministic
+backward (``pmvs_edgeconv_pm_backward``) so that a model built from these layers trains."""
 import torch
 import torch.nn as nn
+from torch.autograd.function import once_differentiable
 
 from ._lib import lib, check, stream_ptr, ptr, require_cuda, f32c
 from .nn.conv import Conv2d
 
 _SUPPORTED_COUT = (16, 32, 64, 128)
+_backward_enabled = False
+
+
+def enable_backward(enabled=True):
+    """Process-wide switch: while on, ``EdgeConv`` / ``EdgeConvNoC`` called with grad enabled (and a feature or
+    parameter that requires grad) run through an autograd Function whose backward is the fused CUDA backward;
+    while off (the default) such calls raise ``NotImplementedError``.  Returns the previous setting.
+
+    It is opt-in because a grad-enabled forward keeps the layer's [B*N, 2*out] ``LE`` activations, the neighbour
+    indices (int32 and int64), the points-major input and the fp64 batch sums alive until backward runs.  Under
+    ``torch.no_grad()`` the switch has no effect.  The fused ``PointFlow`` stays forward-only either way."""
+    global _backward_enabled
+    prev = _backward_enabled
+    _backward_enabled = bool(enabled)
+    return prev
 
 
 def _edge_layer(mod, feature, knn_inds, concat_central):
@@ -19,8 +37,17 @@ def _edge_layer(mod, feature, knn_inds, concat_central):
     if feature.dim() != 3 or knn_inds.dim() != 3:
         raise RuntimeError("EdgeConv: feature must be [B,C,N] and knn_inds [B,N,K]")
     if torch.is_grad_enabled() and (feature.requires_grad or any(p.requires_grad for p in mod.parameters())):
-        # inference under torch.no_grad() is the supported mode (test.py:62)
-        raise NotImplementedError("pointmvsnet_b200 EdgeConv is forward-only; wrap the call in torch.no_grad()")
+        if not _backward_enabled:
+            # inference under torch.no_grad() is the supported mode (test.py:62); training needs enable_backward()
+            raise NotImplementedError("pointmvsnet_b200 EdgeConv is forward-only; wrap the call in torch.no_grad() "
+                                      "or call pointmvsnet_b200.networks.enable_backward()")
+        return _EdgeConvFn.apply(feature, mod.conv1.weight, mod.conv2.weight, mod.bn.weight, mod.bn.bias, mod,
+                                 knn_inds, concat_central)
+    return _edge_forward(mod, feature, knn_inds, concat_central, None)
+
+
+def _edge_forward(mod, feature, knn_inds, concat_central, ctx):
+    """The forward kernels; with `ctx` (an autograd context) the tensors the backward needs are saved on it."""
     B, cin, N = feature.shape
     K = knn_inds.shape[2]
     cout = mod.conv1.out_channels
@@ -62,7 +89,58 @@ def _edge_layer(mod, feature, knn_inds, concat_central):
             _update_running(mod.bn, stats, cout, rows, K, concat_central)
         out = torch.empty(B, ctot, N, device=dev, dtype=torch.float32)
         check(lib.pmvs_transpose(ptr(out_pm), ptr(out), B, N, ctot, st))
+    if ctx is not None:
+        # stats: the sums the forward normalised with (batch sums in train mode, the running statistics otherwise)
+        ctx.save_for_backward(x_pm, idx32, ind, le, stats, w12, gamma, beta)
+        ctx.shape = (B, N, K, cin, cout)
+        ctx.bn = (float(mod.bn.eps), bool(concat_central), bool(train))
     return out
+
+
+class _EdgeConvFn(torch.autograd.Function):
+    """EdgeConv / EdgeConvNoC with a fused backward.  Inputs are the module's own parameters, so their .grad fills;
+    the stacked copy `_layer_params` caches is only what the kernels read."""
+
+    @staticmethod
+    def forward(ctx, feature, w1, w2, gamma, beta, mod, knn_inds, concat_central):
+        ctx.dtypes = (feature.dtype, w1.dtype, w2.dtype, gamma.dtype, beta.dtype)
+        return _edge_forward(mod, feature, knn_inds, concat_central, ctx)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_out):
+        x_pm, idx32, ind, le, stats, w12, gamma, beta = ctx.saved_tensors
+        B, N, K, cin, cout = ctx.shape
+        eps, concat_central, train = ctx.bn
+        ctot = 2 * cout if concat_central else cout
+        dev = x_pm.device
+        need_dx = ctx.needs_input_grad[0]
+        with torch.cuda.device(dev):
+            st = stream_ptr()
+            dy = f32c(grad_out)
+            dy_pm = torch.empty(B, N, ctot, device=dev, dtype=torch.float32)
+            check(lib.pmvs_transpose(ptr(dy), ptr(dy_pm), B, ctot, N, st))
+            dx_pm = torch.empty(B, N, cin, device=dev, dtype=torch.float32) if need_dx else None
+            dw12 = torch.empty(2 * cout, cin, device=dev, dtype=torch.float32)
+            dgamma = torch.empty_like(gamma)
+            dbeta = torch.empty_like(beta)
+            nbytes = lib.pmvs_edgeconv_pm_backward_workspace_bytes(B, N, K, cin, cout)
+            ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+            check(lib.pmvs_edgeconv_pm_backward(ptr(x_pm), cin, ptr(idx32), ptr(ind), ptr(w12), ptr(gamma), ptr(beta),
+                                                eps, 1 if concat_central else 0, 1 if train else 0, ptr(le), ptr(stats),
+                                                ptr(dy_pm), ctot, ptr(dx_pm), cin, ptr(dw12), ptr(dgamma), ptr(dbeta),
+                                                ptr(ws), nbytes, B, N, K, cin, cout, st))
+            dx = None
+            if need_dx:
+                dx = torch.empty(B, cin, N, device=dev, dtype=torch.float32)
+                check(lib.pmvs_transpose(ptr(dx_pm), ptr(dx), B, N, cin, st))
+        fdt, w1dt, w2dt, gdt, bdt = ctx.dtypes
+        grads = (dx.to(fdt) if dx is not None else None,
+                 dw12[:cout].unsqueeze(-1).to(w1dt) if ctx.needs_input_grad[1] else None,
+                 dw12[cout:].unsqueeze(-1).to(w2dt) if ctx.needs_input_grad[2] else None,
+                 dgamma.to(gdt) if ctx.needs_input_grad[3] else None,
+                 dbeta.to(bdt) if ctx.needs_input_grad[4] else None)
+        return grads + (None, None, None)
 
 
 def _layer_params(mod, dev):
