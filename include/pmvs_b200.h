@@ -59,7 +59,11 @@ int pmvs_get_gemm_mode(void);
  *                   0 = 16 L2 gathers per point (the kernels the stand-alone EdgeConv operator uses)
  *   PMVS_OPT_KNN    1 = batched sorting network + bitonic merge (kernel_size 5, knn 16),
  *                   0 = sorted insertion (the kernel every other (kernel_size, knn) uses)
- *   PMVS_OPT_FETCH  1 = consecutive hypotheses share the texel quad, fp32 pair math (3 CTAs / SM),
+ *   PMVS_OPT_FETCH  3 = option 1 fused with EdgeConvNoC(136, 32)'s contraction (one persistent launch, the
+ *                   136-channel point features are not written); taken under PMVS_OPT_GEMM 3, gemm mode 3,
+ *                   PMVS_OPT_EDGE != 0 and V <= 6, option 1 + the contraction otherwise (PMVS_OPT_GEMM_STRICT:
+ *                   an error instead),
+ *                   1 = consecutive hypotheses share the texel quad, fp32 pair math (3 CTAs / SM),
  *                   2 = the same with 2 CTAs / SM and a larger register budget, 0 = 4 taps per (hypothesis, view)
  *                   (the kernel used for V > 6)
  *   PMVS_OPT_GEMM   3 = weights stationary in shared memory, persistent, X through TMA rings (one per
@@ -69,7 +73,8 @@ int pmvs_get_gemm_mode(void);
  *                   0 = points-as-M with shared-memory operands (the kernel plain-TF32 mode uses)
  *   PMVS_OPT_DEBUG_IDX  1 = also materialise int32 neighbour indices in the workspace
  *   PMVS_OPT_GEMM_STRICT  0 = off; 1 = under PMVS_OPT_GEMM 3, a contraction the TMA kernel does not take
- *                   returns PMVS_ERR_ARG instead of running on option 2 (tests) */
+ *                   returns PMVS_ERR_ARG instead of running on option 2, and so does a PMVS_OPT_FETCH 3 call
+ *                   that the fused fetch kernel does not take (tests) */
 #define PMVS_OPT_EDGE 1
 #define PMVS_OPT_KNN 2
 #define PMVS_OPT_FETCH 3
@@ -268,6 +273,13 @@ int pmvs_pyramid_to_channels_last(const float* nchw, float* nhwc, int BV, int C,
  * d*25+h*5+w of the 5x5x5 window), off[9]=1 if idx32 was materialised;
  * S = ratio^2, N = 5*h'*w'. */
 int pmvs_point_flow_debug_offsets(const pmvs_flow_shape* shape, size_t off[10]);
+
+/* Rewrites the feature region (off[0]) of a workspace after pmvs_point_flow_iter with the unfused fetch kernel:
+ * under PMVS_OPT_FETCH 3 the iteration does not write it.  Needs the camera blocks and the resized pyramid map the
+ * iteration left in the workspace and the same depth_prev [B,1,prev_h,prev_w]; the values are bit-identical to
+ * the rows the iteration contracted.  Also rewrites xyz with the same values. */
+int pmvs_point_flow_debug_feature(const pmvs_flow_shape* shape, const float* depth_prev, void* workspace,
+                                  pmvs_stream_t stream);
 
 #ifdef __cplusplus
 }

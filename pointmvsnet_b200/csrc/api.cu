@@ -28,7 +28,7 @@ static struct OptDefaults {
   OptDefaults() {
     g_opt[OPT_EDGE].store(1);   // TMA halo-tile EdgeConv
     g_opt[OPT_KNN].store(1);    // batched sorting-network kNN
-    g_opt[OPT_FETCH].store(1);  // texel-quad sharing fetch
+    g_opt[OPT_FETCH].store(3);  // texel-quad sharing fetch fused with EdgeConvNoC's contraction
     g_opt[OPT_GEMM].store(3);   // weight-stationary persistent GEMM, TMA ring, register-A wgmma, ping-pong
   }
 } g_opt_defaults;
@@ -200,6 +200,17 @@ static int make_plan(const pmvs_flow_shape* s, FlowPlan& p) {
   return PMVS_OK;
 }
 
+// the fetch of an iteration (rows a2-a9) over the workspace of plan p
+static FusedFetchParams fetch_params(const pmvs_flow_shape* s, const FlowPlan& p, char* ws, const float* depth_prev) {
+  FusedFetchParams f{};
+  f.src = (const float*)(ws + p.warp_src);
+  f.depth_prev = depth_prev; f.cam_blocks = (const float*)(ws + p.cam); f.feature = (float*)(ws + p.feature);
+  f.xyz = (float*)(ws + p.xyz);
+  f.B = s->B; f.V = s->V; f.h = s->flow_h; f.w = s->flow_w; f.hp = s->prev_h; f.wp = s->prev_w;
+  f.ratio = s->ratio; f.sub_begin = p.sub_begin; f.sub_count = p.S;
+  return f;
+}
+
 }  // namespace pmvs
 
 using namespace pmvs;
@@ -346,6 +357,14 @@ extern "C" int pmvs_point_flow_debug_offsets(const pmvs_flow_shape* shape, size_
   return PMVS_OK;
 }
 
+extern "C" int pmvs_point_flow_debug_feature(const pmvs_flow_shape* shape, const float* depth_prev, void* workspace,
+                                             pmvs_stream_t stream) {
+  FlowPlan p;
+  PMVS_TRY(make_plan(shape, p));
+  PMVS_REQUIRE(depth_prev && workspace, "point_flow_debug_feature: NULL pointer");
+  return launch_fused_fetch(fetch_params(shape, p, (char*)workspace, depth_prev), (cudaStream_t)stream);
+}
+
 extern "C" int pmvs_point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flow_weights* wts,
                                     const float* const pyramids_cl[3], const float* depth_prev,
                                     const float* cam_params, const float* interval, const float* mean,
@@ -363,8 +382,8 @@ extern "C" int pmvs_point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flo
   cudaStream_t st = (cudaStream_t)stream;
   char* ws = (char*)workspace;
   float* cam = (float*)(ws + p.cam);
-  float* feature = (float*)(ws + p.feature);
-  float* xyz = (float*)(ws + p.xyz);
+  const float* feature = (const float*)(ws + p.feature);
+  const float* xyz = (const float*)(ws + p.xyz);
   int32_t* idx = (int32_t*)(ws + p.idx);
   float* le = (float*)(ws + p.le);
   float* ecat = (float*)(ws + p.ecat);
@@ -387,16 +406,24 @@ extern "C" int pmvs_point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flo
   float* warp_src = (float*)(ws + p.warp_src);
   PMVS_TRY(launch_warp_source(pyramids_cl, shape->pyr_h, shape->pyr_w, warp_src, B, shape->V, shape->flow_h,
                               shape->flow_w, st));
-  FusedFetchParams f{};
-  f.src = warp_src;
-  f.depth_prev = depth_prev; f.cam_blocks = cam; f.feature = feature; f.xyz = xyz;
-  f.B = B; f.V = shape->V; f.h = shape->flow_h; f.w = shape->flow_w; f.hp = shape->prev_h; f.wp = shape->prev_w;
-  f.ratio = shape->ratio; f.sub_begin = p.sub_begin; f.sub_count = S;
-  PMVS_TRY(launch_fused_fetch(f, st));
+  const int edge_impl = opt(OPT_EDGE);
+  const FusedFetchParams f = fetch_params(shape, p, ws, depth_prev);
+  // a2-a9 and EdgeConvNoC's contraction LE = F0 * W12^T in one launch, so that F0 never reaches memory.  Layer 0 has
+  // no input BatchNorm, and the column statistics of its LE are never read (below), so nothing else needs F0.
+  bool fused_le0 = false;
+  if (opt(OPT_FETCH) == 3 && opt(OPT_GEMM) == 3 && pmvs_get_gemm_mode() == 3 && edge_impl != 0) {
+    const int rc = launch_fetch_gemm(f, wts->ec_w12[0], le, st);
+    if (rc > 0) return rc;
+    fused_le0 = rc == 0;
+    if (!fused_le0 && opt(OPT_GEMM_STRICT)) {
+      set_error("point_flow: fetch_gemm_kernel does not take V=%d (strict mode)", shape->V);
+      return PMVS_ERR_ARG;
+    }
+  }
+  if (!fused_le0) PMVS_TRY(launch_fused_fetch(f, st));
 
   // a10: neighbour lists.  The tile EdgeConv path consumes 16-bit neighbour codes; the int32 row indices are only
   // materialised for the gather path (or on request, for the tests)
-  const int edge_impl = opt(OPT_EDGE);
   unsigned short* cand = (unsigned short*)(ws + p.cand);
   if (edge_impl != 0)
     PMVS_TRY(launch_knn3d_cand(xyz, opt(OPT_DEBUG_IDX) ? idx : nullptr, cand, S * B, PMVS_NUM_HYP, p.hs, p.ws, st));
@@ -411,8 +438,9 @@ extern "C" int pmvs_point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flo
     g.ldx = l == 0 ? PMVS_FEAT_CH : 224;
     g.w = wts->ec_w12[l]; g.y = le; g.ldy = 2 * cout[l];
     g.groups = S; g.rows_per_group = rows_per_group; g.cin = cin[l]; g.cout = 2 * cout[l]; g.eps = wts->eps;
-    if (edge_impl != 0) g.out_stats = stats + p.st_ec[l];  // column sums of LE: the central half's BN statistics
-    PMVS_TRY(launch_gemm(g, st));
+    // column sums of LE: the central half's BN statistics, which EdgeConvNoC (layer 0) does not have
+    if (edge_impl != 0 && l > 0) g.out_stats = stats + p.st_ec[l];
+    if (l > 0 || !fused_le0) PMVS_TRY(launch_gemm(g, st));
     if (edge_impl != 0) {
       EdgeTileArgs e{};
       e.le = le; e.cand = cand; e.cstats = stats + p.st_ec[l]; e.nstats = stats + p.st_ecn[l];

@@ -75,7 +75,8 @@ enum {
   OPT_EDGE = 1,   // EdgeConv statistics/apply of the fused path: 0 = L2 gathers (edge_kernel), 1 = TMA halo tile 8x4x5,
                   // 2 = TMA halo tile 16x4x5
   OPT_KNN = 2,    // 0 = sorted insertion (round 1), 1 = batched sort + bitonic merge
-  OPT_FETCH = 3,  // 0 = 4 taps per (hypothesis, view), 1 = hypotheses of a pixel share the texel quad when they can
+  OPT_FETCH = 3,  // 0 = 4 taps per (hypothesis, view), 1 = hypotheses of a pixel share the texel quad when they can,
+                  // 2 = the same at 2 CTAs / SM, 3 = 1 fused with EdgeConvNoC's contraction (fetch_gemm_kernel)
   OPT_GEMM = 4,   // 0 = points-as-M shared-memory operands (round 1), 1 / 2 = weights stationary in shared memory, persistent
                   // (gemm_ws.cu), 3 = the same weights with a TMA-fed X ring, register-A wgmma and ping-pong warpgroups
   OPT_DEBUG_IDX = 5,  // 1 = the fused path also materialises the int32 neighbour indices (tests)
@@ -217,6 +218,9 @@ size_t warp_source_bytes(int B, int V, int h, int w);
 int launch_cam_setup(const float* cam_params, const float* interval, const float* mean, const float* stdv,
                      float* blocks, int B, int V, float kscale, float iscale, cudaStream_t st);
 int launch_fused_fetch(const FusedFetchParams& p, cudaStream_t st);
+// fused_fetch and EdgeConvNoC's contraction LE [R, 64] = F0 * w12^T in one launch (3xTF32; p.feature is not written).
+// Returns -1 when it does not take the call (5 V > 30, or the shared memory cannot be had)
+int launch_fetch_gemm(const FusedFetchParams& p, const float* w12, float* le, cudaStream_t st);
 size_t cam_block_bytes(int B, int V);
 
 struct HeadArgs {

@@ -11,7 +11,10 @@
 //      112 pyramid channels as float4s, so a tap is one contiguous 448-byte read.
 //      Camera matrices for the CTA's batch element are staged into shared memory with one
 //      cp.async.bulk (TMA bulk copy) completing on an mbarrier.
+#include <algorithm>
+
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace pmvs {
 
@@ -291,12 +294,154 @@ __host__ __device__ constexpr size_t fetch_smem_total(int V) {  // + 16 floats o
   return fetch_smem_bytes(V) + FETCH_WARPS * 16 * sizeof(float);
 }
 
-// rows a2-a9; a CTA covers (4 * p.ppw) x 2 pixels, one pixel per warp at a time.  Phase 1: lane t =
-// (hypothesis m, view v) un-projects the hypothesis, projects it into the view and writes the
-// 4-tap descriptor.  Phase 2: lanes 0..27 each own one float4 of the 112 channels; for every
-// hypothesis the views are walked in order and the lane keeps the sum / sum of squares of its
-// channels (model.py:188-189), so there is no cross-lane reduction; one tap = one 128-bit
-// ld.global.nc + 4 FFMA per lane, 448 contiguous bytes per warp.
+// Phase 1 of pixel (X, Y) of batch element b (rows a2-a4, a8), run by a whole warp: lane t = (hypothesis m, view v)
+// un-projects the hypothesis, projects it into the view and writes the 4-tap descriptor desc[t]; lanes 0..4 write the
+// normalised xyz of the 5 hypothesis points to xyzs[3 m ..].  SHARE: returns the ballot `eqmask`, bit m*V+v set <=>
+// hypothesis m hits the same texel quad as hypothesis m-1 in view v (npair <= 30: all 32 lanes vote).  `cam` is the
+// batch element's camera block.
+template <bool SHARE>
+__device__ __forceinline__ unsigned fetch_describe(const FusedFetchParams& p, const float* cam, Desc* desc,
+                                                   float* xyzs, int lane, int b, int X, int Y) {
+  const int V = p.V, h = p.h, w = p.w;
+  const int npair = PMVS_NUM_HYP * V;
+  const float interval = cam[CB_INTERVAL];
+  const float nsy = (float)p.hp / (float)h, nsx = (float)p.wp / (float)w;
+  const unsigned zero_tex = (unsigned)(V * h * w) * (unsigned)FETCH_C4;  // the batch element's all-zero texel
+  // (hypothesis, view) pairs this lane describes: t = lane and, for V > 6, lane + 32
+  const int m_a = lane / V, v_a = lane - m_a * V;
+  const int m_b = (lane + 32) / V, v_b = lane + 32 - m_b * V;
+  int ys = (int)floorf((float)Y * nsy);  // nearest upsample row (model.py:153-158; ATen nearest rule)
+  ys = ys < p.hp - 1 ? ys : p.hp - 1;
+  const float py = (float)Y + 0.5f;
+  int xs = (int)floorf((float)X * nsx);
+  xs = xs < p.wp - 1 ? xs : p.wp - 1;
+  const float dprev = __ldg(p.depth_prev + ((size_t)b * p.hp + ys) * p.wp + xs);
+
+  // uv = K_ref^-1 * (x + .5, y + .5, 1)   (functions.py:128-138, model.py:165-170)
+  const float px = (float)X + 0.5f;
+  const float uvx = dot3(cam + CB_KINV + 0, px, py, 1.f);
+  const float uvy = dot3(cam + CB_KINV + 3, px, py, 1.f);
+  const float uvz = dot3(cam + CB_KINV + 6, px, py, 1.f);
+
+  auto world_point = [&](int m, float& wx, float& wy, float& wz) {
+    const float dm = __fadd_rn(dprev, __fmul_rn(interval, (float)(m - 2)));  // model.py:174
+    const float cx = __fsub_rn(__fmul_rn(uvx, dm), cam[CB_T0 + 0]);
+    const float cy = __fsub_rn(__fmul_rn(uvy, dm), cam[CB_T0 + 1]);
+    const float cz = __fsub_rn(__fmul_rn(uvz, dm), cam[CB_T0 + 2]);
+    wx = dot3(cam + CB_R0INV + 0, cx, cy, cz);  // model.py:177
+    wy = dot3(cam + CB_R0INV + 3, cx, cy, cz);
+    wz = dot3(cam + CB_R0INV + 6, cx, cy, cz);
+  };
+
+  unsigned eqmask = 0u;
+  for (int t = lane; t < (SHARE ? 32 : npair); t += 32) {
+    const int m = t < 32 ? m_a : m_b, v = t < 32 ? v_a : v_b;
+    float wx, wy, wz;
+    world_point(m, wx, wy, wz);
+    const float* cv = cam + CB_VIEW + v * CB_VSTRIDE;
+    float u, vv;
+    project(cv, cv + 9, cv + 12, wx, wy, wz, u, vv);
+    const float ix = grid_coord(u, w), iy = grid_coord(vv, h);
+    const bool ok = usable(ix) && usable(iy);
+    const Taps tp = make_taps(ok ? ix : -10.f, ok ? iy : -10.f, w, h);
+    const bool k00 = tp.ok_n && tp.ok_w, k01 = tp.ok_n && tp.ok_e, k10 = tp.ok_s && tp.ok_w, k11 = tp.ok_s && tp.ok_e;
+    const unsigned ov = (unsigned)(v * h * w) * (unsigned)FETCH_C4;  // start of the view
+    const unsigned o00 = ov + (unsigned)(tp.y0 * w + tp.x0) * (unsigned)FETCH_C4;
+    Desc dd;
+    dd.o[0] = k00 ? o00 : zero_tex;
+    dd.o[1] = k01 ? o00 + (unsigned)FETCH_C4 : zero_tex;
+    dd.o[2] = k10 ? o00 + (unsigned)w * (unsigned)FETCH_C4 : zero_tex;
+    dd.o[3] = k11 ? o00 + (unsigned)(w + 1) * (unsigned)FETCH_C4 : zero_tex;
+    const float w0 = k00 ? tp.nw : 0.f, w1 = k01 ? tp.ne : 0.f, w2 = k10 ? tp.sw : 0.f, w3 = k11 ? tp.se : 0.f;
+    if (SHARE) {
+      dd.w[0] = w0; dd.w[1] = w0; dd.w[2] = w1; dd.w[3] = w1;
+      dd.wd[0] = w2; dd.wd[1] = w2; dd.wd[2] = w3; dd.wd[3] = w3;
+    } else {
+      dd.w[0] = w0; dd.w[1] = w1; dd.w[2] = w2; dd.w[3] = w3;
+      dd.wd[0] = dd.wd[1] = dd.wd[2] = dd.wd[3] = 0.f;
+    }
+    if (!SHARE || t < npair) desc[t] = dd;
+    if (SHARE) {
+      // same texel quad as the PREVIOUS hypothesis of the same view (lane t - V)?
+      const unsigned q0 = __shfl_up_sync(0xffffffffu, dd.o[0], V), q1 = __shfl_up_sync(0xffffffffu, dd.o[1], V);
+      const unsigned q2 = __shfl_up_sync(0xffffffffu, dd.o[2], V), q3 = __shfl_up_sync(0xffffffffu, dd.o[3], V);
+      eqmask = __ballot_sync(0xffffffffu, t >= V && t < npair && q0 == dd.o[0] && q1 == dd.o[1] && q2 == dd.o[2] &&
+                                              q3 == dd.o[3]);
+    }
+  }
+  // normalised xyz of the 5 hypothesis points (model.py:46-48,193): lane m computes point m
+  if (lane < PMVS_NUM_HYP) {
+    float wx, wy, wz;
+    world_point(lane, wx, wy, wz);
+    xyzs[lane * 3 + 0] = __fdiv_rn(__fsub_rn(wx, cam[CB_MEAN + 0]), cam[CB_STD + 0]);
+    xyzs[lane * 3 + 1] = __fdiv_rn(__fsub_rn(wy, cam[CB_MEAN + 1]), cam[CB_STD + 1]);
+    xyzs[lane * 3 + 2] = __fdiv_rn(__fsub_rn(wz, cam[CB_MEAN + 2]), cam[CB_STD + 2]);
+  }
+  return eqmask;
+}
+
+// Phase 2 with texel-quad sharing (rows a6-a7), run by lanes 0..27 after phase 1 of the pixel: `src` points at the
+// lane's float4 of the batch element's map; store(m, o) receives the variance of the lane's 4 channels of hypothesis m.
+// Views outermost.  Consecutive hypotheses of a pixel project ~0.1 texel apart along the epipolar line, so a hypothesis
+// usually hits the texel quad of the previous one: the 4 taps are then NOT re-loaded (a warp-uniform test on the ballot
+// of phase 1), about 1.4 quads per view instead of 5.  The arithmetic is the scalar kernel's on fp32 pairs (common.cuh
+// f32x2: IEEE rn per lane, so the results are bit-identical); per hypothesis the views are still accumulated in view
+// order.
+template <bool PREFETCH = false, class Store>
+__device__ __forceinline__ void fetch_variance_share(const float4* src, const Desc* desc, unsigned eqmask, int V,
+                                                     float rV, Store&& store) {
+  f32x2 s1l[PMVS_NUM_HYP], s1h[PMVS_NUM_HYP], s2l[PMVS_NUM_HYP], s2h[PMVS_NUM_HYP];
+#pragma unroll
+  for (int m = 0; m < PMVS_NUM_HYP; ++m) s1l[m] = s1h[m] = s2l[m] = s2h[m] = pack2(0.f, 0.f);
+#pragma unroll 1
+  for (int v = 0; v < V; ++v) {
+    if (PREFETCH && v + 1 < V) {  // the next view's first quad into L1: its loads overlap this view's arithmetic
+      const uint4 o = *reinterpret_cast<const uint4*>(desc[v + 1].o);
+      asm volatile("prefetch.global.L1 [%0];" ::"l"(src + o.x));
+      asm volatile("prefetch.global.L1 [%0];" ::"l"(src + o.y));
+      asm volatile("prefetch.global.L1 [%0];" ::"l"(src + o.z));
+      asm volatile("prefetch.global.L1 [%0];" ::"l"(src + o.w));
+    }
+    float4 t0 = make_float4(0.f, 0.f, 0.f, 0.f), t1 = t0, t2 = t0, t3 = t0;
+#pragma unroll
+    for (int m = 0; m < PMVS_NUM_HYP; ++m) {
+      const Desc* dm = desc + m * V + v;
+      if (m == 0 || !((eqmask >> (m * V + v)) & 1u)) {  // warp-uniform: another texel quad than hypothesis m - 1
+        const uint4 o = *reinterpret_cast<const uint4*>(dm->o);
+        t0 = __ldg(src + o.x); t1 = __ldg(src + o.y); t2 = __ldg(src + o.z); t3 = __ldg(src + o.w);
+      }
+      const float4 wa4 = *reinterpret_cast<const float4*>(dm->w);   // (w0,w0) (w1,w1)
+      const float4 wb4 = *reinterpret_cast<const float4*>(dm->wd);  // (w2,w2) (w3,w3)
+      const struct { f32x2 x, y; } wa = {pack2(wa4.x, wa4.y), pack2(wa4.z, wa4.w)},
+                                   wb = {pack2(wb4.x, wb4.y), pack2(wb4.z, wb4.w)};
+      // ATen grid_sampler_2d accumulation order: NW, NE, SW, SE
+      const f32x2 al = fma2(pack2(t3.x, t3.y), wb.y, fma2(pack2(t2.x, t2.y), wb.x,
+                            fma2(pack2(t1.x, t1.y), wa.y, mul2(pack2(t0.x, t0.y), wa.x))));
+      const f32x2 ah = fma2(pack2(t3.z, t3.w), wb.y, fma2(pack2(t2.z, t2.w), wb.x,
+                            fma2(pack2(t1.z, t1.w), wa.y, mul2(pack2(t0.z, t0.w), wa.x))));
+      // model.py:188-189: sums over views of x and x**2, in view order (square and sum unfused)
+      s1l[m] = add2(s1l[m], al); s1h[m] = add2(s1h[m], ah);
+      s2l[m] = add2(s2l[m], mul2(al, al)); s2h[m] = add2(s2h[m], mul2(ah, ah));
+    }
+  }
+#pragma unroll
+  for (int m = 0; m < PMVS_NUM_HYP; ++m) {
+    float4 s1, s2, o;
+    unpack2(s1l[m], s1.x, s1.y); unpack2(s1h[m], s1.z, s1.w);
+    unpack2(s2l[m], s2.x, s2.y); unpack2(s2h[m], s2.z, s2.w);
+    float a;
+    a = __fmul_rn(s1.x, rV); o.x = __fsub_rn(__fmul_rn(s2.x, rV), __fmul_rn(a, a));
+    a = __fmul_rn(s1.y, rV); o.y = __fsub_rn(__fmul_rn(s2.y, rV), __fmul_rn(a, a));
+    a = __fmul_rn(s1.z, rV); o.z = __fsub_rn(__fmul_rn(s2.z, rV), __fmul_rn(a, a));
+    a = __fmul_rn(s1.w, rV); o.w = __fsub_rn(__fmul_rn(s2.w, rV), __fmul_rn(a, a));
+    store(m, o);
+  }
+}
+
+// rows a2-a9; a CTA covers (4 * p.ppw) x 2 pixels, one pixel per warp at a time: phase 1 (fetch_describe), then
+// phase 2: lanes 0..27 each own one float4 of the 112 channels; for every hypothesis the views are walked in order and
+// the lane keeps the sum / sum of squares of its channels (model.py:188-189), so there is no cross-lane reduction; one
+// tap = one 128-bit ld.global.nc + 4 FFMA per lane, 448 contiguous bytes per warp.
 template <bool SHARE, int MINB>
 __global__ void __launch_bounds__(FETCH_WARPS * 32, MINB) fused_fetch_kernel(const FusedFetchParams p) {
   __shared__ __align__(16) float cam[cam_block_floats(PMVS_MAX_VIEWS)];
@@ -340,18 +485,11 @@ __global__ void __launch_bounds__(FETCH_WARPS * 32, MINB) fused_fetch_kernel(con
   const int npair = PMVS_NUM_HYP * V;
   Desc* desc = reinterpret_cast<Desc*>(dyn_smem) + (size_t)warp * npair;
   float* xyzs = reinterpret_cast<float*>(dyn_smem + fetch_smem_bytes(V)) + warp * 16;
-  const float interval = cam[CB_INTERVAL];
-  const float nsy = (float)p.hp / (float)h, nsx = (float)p.wp / (float)w;
   const int hs = p.hs, wsub = p.ws;
   const int Npts = PMVS_NUM_HYP * hs * wsub;
   const float rV = __frcp_rn((float)V);
   const size_t fstep = (size_t)hs * wsub * PMVS_FEAT_CH;  // next hypothesis
-  const unsigned zero_tex = (unsigned)(V * h * w) * (unsigned)FETCH_C4;  // the batch element's all-zero texel
   const float4* src = reinterpret_cast<const float4*>(p.src) + (size_t)b * ((size_t)V * h * w + 1) * FETCH_C4 + lane;
-  // SHARE: bit m*V+v of `eqmask` set <=> hypothesis m hits the same texel quad as hypothesis m-1 in view v
-  // (hypothesis, view) pairs this lane describes: t = lane and, for V > 6, lane + 32
-  const int m_a = lane / V, v_a = lane - m_a * V;
-  const int m_b = (lane + 32) / V, v_b = lane + 32 - m_b * V;
   // lane -> (hypothesis, float4 #j of the 24 tiled xyz values) and (hypothesis, component) for the
   // epilogue stores; float4 #j starts at component (4j) % 3 = j % 3
   const int em = lane / 6, ej = lane - em * 6, eph = ej % 3;
@@ -363,9 +501,6 @@ __global__ void __launch_bounds__(FETCH_WARPS * 32, MINB) fused_fetch_kernel(con
   if (Y >= h) return;  // warp-uniform; no CTA-wide barrier below
   const int yy = p.rlog2 >= 0 ? Y >> p.rlog2 : Y / p.ratio;
   const int ii = Y - yy * p.ratio;
-  int ys = (int)floorf((float)Y * nsy);  // nearest upsample row (model.py:153-158; ATen nearest rule)
-  ys = ys < p.hp - 1 ? ys : p.hp - 1;
-  const float py = (float)Y + 0.5f;
   const int X0 = blockIdx.x * p.ppw * 4 + (warp & 3);
 
   for (int k = 0; k < p.ppw; ++k) {
@@ -379,71 +514,8 @@ __global__ void __launch_bounds__(FETCH_WARPS * 32, MINB) fused_fetch_kernel(con
       if (sc < 0 || sc >= p.sub_count) continue;  // warp-uniform
     }
 
-    int xs = (int)floorf((float)X * nsx);
-    xs = xs < p.wp - 1 ? xs : p.wp - 1;
-    const float dprev = __ldg(p.depth_prev + ((size_t)b * p.hp + ys) * p.wp + xs);
-
-    // uv = K_ref^-1 * (x + .5, y + .5, 1)   (functions.py:128-138, model.py:165-170)
-    const float px = (float)X + 0.5f;
-    const float uvx = dot3(cam + CB_KINV + 0, px, py, 1.f);
-    const float uvy = dot3(cam + CB_KINV + 3, px, py, 1.f);
-    const float uvz = dot3(cam + CB_KINV + 6, px, py, 1.f);
-
-    auto world_point = [&](int m, float& wx, float& wy, float& wz) {
-      const float dm = __fadd_rn(dprev, __fmul_rn(interval, (float)(m - 2)));  // model.py:174
-      const float cx = __fsub_rn(__fmul_rn(uvx, dm), cam[CB_T0 + 0]);
-      const float cy = __fsub_rn(__fmul_rn(uvy, dm), cam[CB_T0 + 1]);
-      const float cz = __fsub_rn(__fmul_rn(uvz, dm), cam[CB_T0 + 2]);
-      wx = dot3(cam + CB_R0INV + 0, cx, cy, cz);  // model.py:177
-      wy = dot3(cam + CB_R0INV + 3, cx, cy, cz);
-      wz = dot3(cam + CB_R0INV + 6, cx, cy, cz);
-    };
-
     // ---- phase 1: one lane per (hypothesis, view) builds its sampling descriptor --------------
-    unsigned eqmask = 0u;
-    for (int t = lane; t < (SHARE ? 32 : npair); t += 32) {
-      const int m = t < 32 ? m_a : m_b, v = t < 32 ? v_a : v_b;
-      float wx, wy, wz;
-      world_point(m, wx, wy, wz);
-      const float* cv = cam + CB_VIEW + v * CB_VSTRIDE;
-      float u, vv;
-      project(cv, cv + 9, cv + 12, wx, wy, wz, u, vv);
-      const float ix = grid_coord(u, w), iy = grid_coord(vv, h);
-      const bool ok = usable(ix) && usable(iy);
-      const Taps tp = make_taps(ok ? ix : -10.f, ok ? iy : -10.f, w, h);
-      const bool k00 = tp.ok_n && tp.ok_w, k01 = tp.ok_n && tp.ok_e, k10 = tp.ok_s && tp.ok_w, k11 = tp.ok_s && tp.ok_e;
-      const unsigned ov = (unsigned)(v * h * w) * (unsigned)FETCH_C4;  // start of the view
-      const unsigned o00 = ov + (unsigned)(tp.y0 * w + tp.x0) * (unsigned)FETCH_C4;
-      Desc dd;
-      dd.o[0] = k00 ? o00 : zero_tex;
-      dd.o[1] = k01 ? o00 + (unsigned)FETCH_C4 : zero_tex;
-      dd.o[2] = k10 ? o00 + (unsigned)w * (unsigned)FETCH_C4 : zero_tex;
-      dd.o[3] = k11 ? o00 + (unsigned)(w + 1) * (unsigned)FETCH_C4 : zero_tex;
-      const float w0 = k00 ? tp.nw : 0.f, w1 = k01 ? tp.ne : 0.f, w2 = k10 ? tp.sw : 0.f, w3 = k11 ? tp.se : 0.f;
-      if (SHARE) {
-        dd.w[0] = w0; dd.w[1] = w0; dd.w[2] = w1; dd.w[3] = w1;
-        dd.wd[0] = w2; dd.wd[1] = w2; dd.wd[2] = w3; dd.wd[3] = w3;
-      } else {
-        dd.w[0] = w0; dd.w[1] = w1; dd.w[2] = w2; dd.w[3] = w3;
-        dd.wd[0] = dd.wd[1] = dd.wd[2] = dd.wd[3] = 0.f;
-      }
-      if (!SHARE || t < npair) desc[t] = dd;
-      if (SHARE) {
-        // same texel quad as the PREVIOUS hypothesis of the same view (lane t - V)?  (npair <= 30: all 32 lanes vote)
-        const unsigned q0 = __shfl_up_sync(0xffffffffu, dd.o[0], V), q1 = __shfl_up_sync(0xffffffffu, dd.o[1], V);
-        const unsigned q2 = __shfl_up_sync(0xffffffffu, dd.o[2], V), q3 = __shfl_up_sync(0xffffffffu, dd.o[3], V);
-        eqmask = __ballot_sync(0xffffffffu, t >= V && t < npair && q0 == dd.o[0] && q1 == dd.o[1] && q2 == dd.o[2] &&
-                                                q3 == dd.o[3]);
-      }
-    }
-    // normalised xyz of the 5 hypothesis points (model.py:46-48,193): lane m computes point m
-    if (lane < PMVS_NUM_HYP) {
-      float wx, wy, wz;
-      world_point(lane, wx, wy, wz);
-      xyzs[lane * 3 + 0] = __fdiv_rn(__fsub_rn(wx, cam[CB_MEAN + 0]), cam[CB_STD + 0]);
-      xyzs[lane * 3 + 1] = __fdiv_rn(__fsub_rn(wy, cam[CB_MEAN + 1]), cam[CB_STD + 1]);
-      xyzs[lane * 3 + 2] = __fdiv_rn(__fsub_rn(wz, cam[CB_MEAN + 2]), cam[CB_STD + 2]);
-    }
+    const unsigned eqmask = fetch_describe<SHARE>(p, cam, desc, xyzs, lane, b, X, Y);
     __syncwarp();
 
     // ---- phase 2: fetch + variance over views ---------------------------------------------------
@@ -452,52 +524,8 @@ __global__ void __launch_bounds__(FETCH_WARPS * 32, MINB) fused_fetch_kernel(con
     const int cloud = (ii * p.ratio + jj - p.sub_begin) * p.B + b;
     float* frow0 = p.feature + ((size_t)cloud * Npts + (size_t)yy * wsub + xx) * PMVS_FEAT_CH;  // hypothesis 0
     if (SHARE) {
-      // Views outermost.  Consecutive hypotheses of a pixel project ~0.1 texel apart along the epipolar line, so a
-      // hypothesis usually hits the texel quad of the previous one: the 4 taps are then NOT re-loaded (a warp-uniform
-      // test on the ballot of phase 1), about 1.4 quads per view instead of 5.  The arithmetic is the scalar kernel's
-      // on fp32 pairs (common.cuh f32x2: IEEE rn per lane, so the results are bit-identical); per hypothesis the
-      // views are still accumulated in view order.
-      if (lane < FETCH_C4) {
-        f32x2 s1l[PMVS_NUM_HYP], s1h[PMVS_NUM_HYP], s2l[PMVS_NUM_HYP], s2h[PMVS_NUM_HYP];
-#pragma unroll
-        for (int m = 0; m < PMVS_NUM_HYP; ++m) s1l[m] = s1h[m] = s2l[m] = s2h[m] = pack2(0.f, 0.f);
-#pragma unroll 1
-        for (int v = 0; v < V; ++v) {
-          float4 t0 = make_float4(0.f, 0.f, 0.f, 0.f), t1 = t0, t2 = t0, t3 = t0;
-#pragma unroll
-          for (int m = 0; m < PMVS_NUM_HYP; ++m) {
-            const Desc* dm = desc + m * V + v;
-            if (m == 0 || !((eqmask >> (m * V + v)) & 1u)) {  // warp-uniform: another texel quad than hypothesis m - 1
-              const uint4 o = *reinterpret_cast<const uint4*>(dm->o);
-              t0 = __ldg(src + o.x); t1 = __ldg(src + o.y); t2 = __ldg(src + o.z); t3 = __ldg(src + o.w);
-            }
-            const float4 wa4 = *reinterpret_cast<const float4*>(dm->w);   // (w0,w0) (w1,w1)
-            const float4 wb4 = *reinterpret_cast<const float4*>(dm->wd);  // (w2,w2) (w3,w3)
-            const struct { f32x2 x, y; } wa = {pack2(wa4.x, wa4.y), pack2(wa4.z, wa4.w)},
-                                         wb = {pack2(wb4.x, wb4.y), pack2(wb4.z, wb4.w)};
-            // ATen grid_sampler_2d accumulation order: NW, NE, SW, SE
-            const f32x2 al = fma2(pack2(t3.x, t3.y), wb.y, fma2(pack2(t2.x, t2.y), wb.x,
-                                  fma2(pack2(t1.x, t1.y), wa.y, mul2(pack2(t0.x, t0.y), wa.x))));
-            const f32x2 ah = fma2(pack2(t3.z, t3.w), wb.y, fma2(pack2(t2.z, t2.w), wb.x,
-                                  fma2(pack2(t1.z, t1.w), wa.y, mul2(pack2(t0.z, t0.w), wa.x))));
-            // model.py:188-189: sums over views of x and x**2, in view order (square and sum unfused)
-            s1l[m] = add2(s1l[m], al); s1h[m] = add2(s1h[m], ah);
-            s2l[m] = add2(s2l[m], mul2(al, al)); s2h[m] = add2(s2h[m], mul2(ah, ah));
-          }
-        }
-#pragma unroll
-        for (int m = 0; m < PMVS_NUM_HYP; ++m) {
-          float4 s1, s2, o;
-          unpack2(s1l[m], s1.x, s1.y); unpack2(s1h[m], s1.z, s1.w);
-          unpack2(s2l[m], s2.x, s2.y); unpack2(s2h[m], s2.z, s2.w);
-          float a;
-          a = __fmul_rn(s1.x, rV); o.x = __fsub_rn(__fmul_rn(s2.x, rV), __fmul_rn(a, a));
-          a = __fmul_rn(s1.y, rV); o.y = __fsub_rn(__fmul_rn(s2.y, rV), __fmul_rn(a, a));
-          a = __fmul_rn(s1.z, rV); o.z = __fsub_rn(__fmul_rn(s2.z, rV), __fmul_rn(a, a));
-          a = __fmul_rn(s1.w, rV); o.w = __fsub_rn(__fmul_rn(s2.w, rV), __fmul_rn(a, a));
-          st4(frow0 + m * fstep + lane * 4, o);
-        }
-      }
+      if (lane < FETCH_C4)
+        fetch_variance_share(src, desc, eqmask, V, rV, [&](int m, float4 o) { st4(frow0 + m * fstep + lane * 4, o); });
     } else
     if (lane < FETCH_C4) {
       const Desc* dp = desc;
@@ -545,6 +573,179 @@ __global__ void __launch_bounds__(FETCH_WARPS * 32, MINB) fused_fetch_kernel(con
       p.xyz[((size_t)cloud * 3 + comp) * Npts + (m * hs + yy) * wsub + xx] = xyzs[lane];
     }
     __syncwarp();  // descriptors / xyz are rewritten for the next pixel
+  }
+}
+
+// rows a2-a9 and the first contraction of EdgeConvNoC(136, 32), LE = F0 * W12^T, in one persistent launch: the
+// 136-channel rows F0 never leave the SM.  One CTA per SM:
+//   * 16 fetch warps compute rows exactly as fused_fetch_kernel<SHARE = true> does (the same device functions, so the
+//     values are bit-identical), one pixel and its 5 hypotheses at a time, and write them into a ring of 64-row tiles
+//     in the layout gemm_tma_kernel's TMA boxes have: per 32-column chunk a 64 x 32 fp32 K-major SWIZZLE_128B plane,
+//     zeros in the K padding 136..159.  A tile holds 12 consecutive pixels of the [B, h, w] grid (rows 5 * slot + m)
+//     and 4 dead rows; layer 0 has no input BatchNorm, so its rows need not belong to one sub-cloud.  Next to the
+//     tile the fetch warps write the LE row of each of its rows (-1: none).  The planar xyz still goes to global
+//     memory for the kNN;
+//   * one consumer warpgroup runs gemm_tma_kernel's chunk sequence (mma_chunk_3xtf32, the weight planes stationary in
+//     shared memory, the same instruction shapes and order), so every LE element is bit for bit what gemm_136x64
+//     computes from F0, and stores from the fragments.  The column statistics of LE are not computed: the EdgeConv
+//     tile kernels read the central-half statistics of layers 1 and 2 only.
+// Warp w takes pixels w, w + 16, .. of the CTA's range.  Before it writes a pixel of tile j the warp has waited for the
+// `empty` barrier of every tile up to j in order, so no barrier it waits on is more than one phase behind; it arrives on
+// `full` (12 arrivals per tile, invalid pixels included), and the consumer waits on `full` and hands the tile back once
+// it has read it.  The fetch is bound by tap latency, not by L1 capacity: 8 warps (no setmaxnreg) took longer for the
+// fetch alone (MMAs and LE stores compiled out) than fused_fetch + gemm_136x64 together, 12 warps were slower than 16,
+// and a 2-tile ring with the shared-memory carveout lowered to leave twice the L1 changed nothing (DESIGN.md 3.1).  The
+// fused kernel therefore prefetches the next view's first texel quad into L1 while it accumulates a view.
+namespace fg {
+constexpr int PIX = 12;                        // pixels per 64-row tile (60 rows + 4 dead)
+constexpr int NCH = 5;                         // 32-column chunks of the 136 columns (K padded to 160)
+constexpr int K = PMVS_FEAT_CH;
+constexpr int COUT = 64;                       // LE = [local | edge], 2 x 32
+constexpr int W_CHUNK = 2 * COUT * 128;        // [W_hi ; W_lo] of one chunk
+constexpr int PLANE = 64 * 128;                // one chunk of a tile, 8 KB
+constexpr int STAGE = NCH * PLANE;             // 40 KB
+constexpr int MAXPAIR = 30;                    // (hypothesis, view) pairs with texel-quad sharing: 5 V <= 30
+static_assert(PIX * PMVS_NUM_HYP <= 64 && NCH * 32 >= K && K % 8 == 0, "tile geometry");
+constexpr int NST = 3;                         // tiles in the ring
+constexpr int FW = 16;                         // fetch warps
+constexpr int THREADS = FW * 32 + 128;         // + one consumer warpgroup
+// registers a thread: at launch (640 threads), then per role after setmaxnreg
+constexpr int LAUNCH_REGS = (65536 / THREADS) & ~7, FETCH_REGS = 88, CONS_REGS = 128;
+// [weight planes | tile ring | LE rows of the ring | descriptors and xyz of each fetch warp | barriers]
+constexpr int SM_RING = NCH * W_CHUNK, SM_ROWS = SM_RING + NST * STAGE, SM_DESC = SM_ROWS + NST * 64 * 8,
+              SM_XYZ = SM_DESC + FW * MAXPAIR * (int)sizeof(Desc), SM_BAR = SM_XYZ + FW * 16 * 4,
+              SMEM = SM_BAR + 2 * NST * 8;
+static_assert(FW % 4 == 0, "fetch warps form whole warpgroups");
+static_assert(FETCH_REGS * FW * 32 + CONS_REGS * 128 <= LAUNCH_REGS * THREADS, "register budget");
+static_assert(SMEM <= 227 * 1024, "fetch_gemm_kernel exceeds the shared memory of a block");
+}  // namespace fg
+
+__global__ void __launch_bounds__(fg::THREADS, 1)
+    fetch_gemm_kernel(const FusedFetchParams p, const float* __restrict__ w12, float* __restrict__ le) {
+  using namespace fg;
+  using namespace wg;
+  extern __shared__ __align__(1024) unsigned char smem[];  // SWIZZLE_128B planes need 1024-byte alignment
+  const uint32_t sbase = smem_u32(smem);
+  const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
+  long long* rows = reinterpret_cast<long long*>(smem + SM_ROWS);
+  auto bar_full = [&](int s) { return sbase + SM_BAR + 8u * (uint32_t)s; };
+  auto bar_empty = [&](int s) { return sbase + SM_BAR + 8u * (uint32_t)(NST + s); };
+  const int V = p.V, h = p.h, w = p.w, hw = h * w;
+  const long long npix = (long long)p.B * hw;
+  // contiguous, balanced range of tiles
+  const long long tiles = (npix + PIX - 1) / PIX;
+  const long long t0 = blockIdx.x * tiles / gridDim.x;
+  const int ntile = (int)((blockIdx.x + 1) * tiles / gridDim.x - t0);
+
+  if (tid == 0) {
+    for (int s = 0; s < NST; ++s) {
+      mbar_init(bar_full(s), PIX);
+      mbar_init(bar_empty(s), 4);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  for (int i = tid; i < NST * STAGE / 16; i += THREADS)
+    asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(sbase + SM_RING + 16 * i), "r"(0) : "memory");
+  for (int i = tid; i < NST * 64; i += THREADS) rows[i] = -1;
+  store_weight_planes<COUT>(sbase, w12, K, tid, THREADS);
+  fence_proxy_async();  // the weight planes are read by the tensor core's async proxy
+  __syncthreads();
+
+  if (warp < FW) {
+    // =============================== fetch warps ==========================================================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(FETCH_REGS));
+    Desc* desc = reinterpret_cast<Desc*>(smem + SM_DESC) + warp * MAXPAIR;
+    float* xyzs = reinterpret_cast<float*>(smem + SM_XYZ) + warp * 16;
+    const int hs = p.hs, wsub = p.ws;
+    const int Npts = PMVS_NUM_HYP * hs * wsub;
+    const float rV = __frcp_rn((float)V);
+    const int em = lane / 6, ej = lane - em * 6, eph = ej % 3;  // tiled xyz, as in fused_fetch_kernel
+    const int e0 = em * 3 + eph, e1 = em * 3 + (eph + 1) % 3, e2 = em * 3 + (eph + 2) % 3;
+    int freed = -1;  // tiles up to this one are known to be free for writing
+    for (int q = warp; q < ntile * PIX; q += FW) {
+      const int j = q / PIX, slot = q - j * PIX, s = j % NST;
+      for (; freed < j; ++freed) mbar_wait(bar_empty((freed + 1) % NST), (uint32_t)((((freed + 1) / NST) & 1) ^ 1));
+      const long long pix = t0 * PIX + q;
+      long long* trow = rows + s * 64 + slot * PMVS_NUM_HYP;
+      bool ok = pix < npix;
+      int b = 0, X = 0, Y = 0, cloud = 0, n0 = 0;
+      if (ok) {
+        b = (int)(pix / hw);
+        const int rem = (int)(pix - (long long)b * hw);
+        Y = rem / w;
+        X = rem - Y * w;
+        const int yy = p.rlog2 >= 0 ? Y >> p.rlog2 : Y / p.ratio, xx = p.rlog2 >= 0 ? X >> p.rlog2 : X / p.ratio;
+        const int sc = (Y - yy * p.ratio) * p.ratio + (X - xx * p.ratio) - p.sub_begin;
+        ok = sc >= 0 && sc < p.sub_count;  // sub-cloud sharding, as in fused_fetch_kernel
+        cloud = sc * p.B + b;
+        n0 = yy * wsub + xx;
+      }
+      if (ok) {  // warp-uniform
+        const unsigned eqmask =
+            fetch_describe<true>(p, p.cam_blocks + (size_t)b * cam_block_floats(V), desc, xyzs, lane, b, X, Y);
+        __syncwarp();
+        const uint32_t tile = sbase + SM_RING + s * STAGE;
+        const int r0 = slot * PMVS_NUM_HYP;
+        if (lane < FETCH_C4) {
+          const float4* src = reinterpret_cast<const float4*>(p.src) + (size_t)b * ((size_t)V * hw + 1) * FETCH_C4 + lane;
+          const uint32_t dst = tile + (lane >> 3) * PLANE;  // channels 4 lane .. 4 lane + 3: chunk lane / 8, piece lane % 8
+          fetch_variance_share<true>(src, desc, eqmask, V, rV, [&](int m, float4 o) {
+            asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(dst + swz128(r0 + m, lane & 7)), "f"(o.x),
+                         "f"(o.y), "f"(o.z), "f"(o.w)
+                         : "memory");
+          });
+        }
+        if (lane < PMVS_NUM_HYP * 6) {  // channels 112 + 4 ej: float4 #28 + ej of the row
+          const float4 o = make_float4(xyzs[e0], xyzs[e1], xyzs[e2], xyzs[e0]);
+          const int c4 = FETCH_C4 + ej;
+          asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(tile + (c4 >> 3) * PLANE + swz128(r0 + em, c4 & 7)),
+                       "f"(o.x), "f"(o.y), "f"(o.z), "f"(o.w)
+                       : "memory");
+        }
+        if (lane < PMVS_NUM_HYP * 3) {
+          const int m = lane / 3, comp = lane - m * 3;
+          p.xyz[((size_t)cloud * 3 + comp) * Npts + m * hs * wsub + n0] = xyzs[lane];
+        }
+        if (lane < PMVS_NUM_HYP) trow[lane] = (long long)cloud * Npts + lane * hs * wsub + n0;
+      } else if (lane < PMVS_NUM_HYP) {
+        trow[lane] = -1;
+      }
+      __syncwarp();  // the tile is written; descriptors / xyz are rewritten for the next pixel
+      if (lane == 0) mbar_arrive(bar_full(s));
+    }
+    return;
+  }
+
+  // =============================== consumer warpgroup ==================================================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONS_REGS));
+  const int r = (warp - FW) * 16 + (lane >> 2), q = lane & 3;  // fragment rows r, r + 8
+  const uint32_t fbase = r * 128 + q * 4, fx = (r & 7) << 4;
+  const int fcol = 2 * q;
+  float acc[COUT];
+  uint32_t fh[16], fl[16];
+  for (int j = 0; j < ntile; ++j) {
+    const int s = j % NST;
+    mbar_wait(bar_full(s), (uint32_t)((j / NST) & 1));
+    const uint32_t st = sbase + SM_RING + s * STAGE + fbase;
+#pragma unroll
+    for (int c = 0; c < NCH - 1; ++c) mma_chunk_3xtf32<COUT, false, 4>(acc, fh, fl, st + c * PLANE, fx, nullptr, sbase + c * W_CHUNK, c);
+    mma_chunk_3xtf32<COUT, false, (K - (NCH - 1) * 32) / 8>(acc, fh, fl, st + (NCH - 1) * PLANE, fx, nullptr,
+                                                            sbase + (NCH - 1) * W_CHUNK, NCH - 1);
+    fence_regs(acc);
+    const long long y0 = rows[s * 64 + r], y1 = rows[s * 64 + r + 8];
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bar_empty(s));  // this warp has read the tile
+    // epilogue from the fragments, as in gemm_tma_kernel: a row of LE is 256 contiguous bytes
+    float* o0 = le + y0 * COUT + fcol;
+    float* o1 = le + y1 * COUT + fcol;
+#pragma unroll
+    for (int i = 0; i < COUT / 8; ++i) {
+      float v[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) v[e] = acc[4 * i + e] + acc[COUT / 2 + 4 * i + e];
+      if (y0 >= 0) *reinterpret_cast<float2*>(o0 + 8 * i) = make_float2(v[0], v[1]);
+      if (y1 >= 0) *reinterpret_cast<float2*>(o1 + 8 * i) = make_float2(v[2], v[3]);
+    }
   }
 }
 
@@ -652,8 +853,9 @@ size_t warp_source_bytes(int B, int V, int h, int w) {
   return (size_t)B * ((size_t)V * h * w + 1) * FETCH_CH * sizeof(float);
 }
 
-int launch_fused_fetch(const FusedFetchParams& p0, cudaStream_t st) {
-  FusedFetchParams p = p0;
+// the launcher-derived fields of FusedFetchParams (sub-grid size, log2(ratio)) and the shape limits of both fetch kernels
+static int fetch_setup(const FusedFetchParams& p0, FusedFetchParams& p) {
+  p = p0;
   const long long npix = (long long)p.h * p.w;
   // tap offsets are 32-bit float4 offsets inside one batch element's [V, h, w, 112] map
   PMVS_REQUIRE((npix * p.V + 1) * FETCH_C4 < (1ll << 32), "fused_fetch: V=%d x %dx%d too large", p.V, p.h, p.w);
@@ -661,19 +863,45 @@ int launch_fused_fetch(const FusedFetchParams& p0, cudaStream_t st) {
   p.hs = p.h / p.ratio; p.ws = p.w / p.ratio;
   p.rlog2 = -1;
   for (int q = 0; q < 16; ++q) if ((1 << q) == p.ratio) p.rlog2 = q;
+  return PMVS_OK;
+}
+
+int launch_fused_fetch(const FusedFetchParams& p0, cudaStream_t st) {
+  FusedFetchParams p;
+  PMVS_TRY(fetch_setup(p0, p));
+  const long long npix = (long long)p.h * p.w;
   // several consecutive pixels of a row per warp once there are enough pixels to fill the machine
   const long long per = npix / ((long long)sm_count() * FETCH_WARPS * 8);
   p.ppw = per >= 4 ? 4 : (per >= 2 ? 2 : 1);
   dim3 grid(cdiv(p.w, 4 * p.ppw), cdiv(p.h, 2), p.B);  // CTA = (4 * ppw) x 2 pixels
   const size_t smem = fetch_smem_total(p.V);
   prof_begin("fused_fetch", st);
-  if (opt(OPT_FETCH) == 1 && PMVS_NUM_HYP * p.V <= 30)
+  // option 3 (fetch_gemm_kernel) runs this kernel where it does not apply
+  if ((opt(OPT_FETCH) == 1 || opt(OPT_FETCH) == 3) && PMVS_NUM_HYP * p.V <= 30)
     fused_fetch_kernel<true, 3><<<grid, FETCH_WARPS * 32, smem, st>>>(p);
   else if (opt(OPT_FETCH) == 2 && PMVS_NUM_HYP * p.V <= 30)
     fused_fetch_kernel<true, 2><<<grid, FETCH_WARPS * 32, smem, st>>>(p);
   else
     fused_fetch_kernel<false, 4><<<grid, FETCH_WARPS * 32, smem, st>>>(p);
   return check_launch("fused_fetch_kernel", st);
+}
+
+int launch_fetch_gemm(const FusedFetchParams& p0, const float* w12, float* le, cudaStream_t st) {
+  FusedFetchParams p;
+  PMVS_TRY(fetch_setup(p0, p));
+  if (PMVS_NUM_HYP * p.V > fg::MAXPAIR) return -1;  // no texel-quad sharing: one descriptor pass does not cover the pairs
+  int dev = 0, optin = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess ||
+      cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess || optin < fg::SMEM)
+    return -1;
+  static unsigned long long smem_done = 0;
+  if (ensure_dyn_smem(fetch_gemm_kernel, fg::SMEM, smem_done, "fetch_gemm") != PMVS_OK) return -1;
+  const long long tiles = ((long long)p.B * p.h * p.w + fg::PIX - 1) / fg::PIX;
+  const int grid = (int)std::min<long long>(tiles, sm_count());
+  // profiled as the fetch it replaces: the contraction runs inside it
+  prof_begin("fused_fetch", st);
+  fetch_gemm_kernel<<<grid, fg::THREADS, fg::SMEM, st>>>(p, w12, le);
+  return check_launch("fetch_gemm_kernel", st);
 }
 
 size_t cam_block_bytes(int B, int V) { return (size_t)B * cam_block_floats(V) * sizeof(float); }

@@ -72,7 +72,6 @@ __device__ __forceinline__ float4 lds128(uint32_t addr) {
   asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
   return v;
 }
-__device__ __forceinline__ float tf32_hi(float x) { return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
 
 struct TileRange {
   int first, count;
@@ -465,7 +464,6 @@ __global__ void __launch_bounds__(tma::THREADS, 1) gemm_tma_kernel(const __grid_
   constexpr bool STACKED = COUT <= 64;
   constexpr int W_CHUNK = 2 * COUT * 128;
   constexpr int ACC_REGS = (STACKED ? 2 * COUT : COUT) / 2;
-  constexpr int BLK = COUT < 64 ? COUT : 64;
   extern __shared__ __align__(1024) unsigned char smem[];
   const uint32_t smem_base = smem_u32(smem);
 
@@ -522,17 +520,7 @@ __global__ void __launch_bounds__(tma::THREADS, 1) gemm_tma_kernel(const __grid_
   double* sRed = (double*)(tail + TAIL_RED) + wgi * 2 * COUT;  // this warpgroup's [sum(COUT) | sumsq(COUT)] of a group
   for (int i = wtid; i < 2 * COUT; i += 128) sRed[i] = 0.0;
   // weights -> shared memory (B operand), as in gemm_ws_kernel
-  for (int e = tid; e < COUT * nch * 8; e += CONS_THREADS) {
-    const int n = e / (nch * 8), rem = e - n * (nch * 8), c = rem >> 3, pc = rem & 7;
-    const int k0 = c * KC + pc * 4;
-    const float4 v = k0 < K ? ldg4(a.w + (size_t)n * K + k0) : make_float4(0.f, 0.f, 0.f, 0.f);
-    float4 hi, lo;
-    hi.x = tf32_hi(v.x); hi.y = tf32_hi(v.y); hi.z = tf32_hi(v.z); hi.w = tf32_hi(v.w);
-    lo.x = __fsub_rn(v.x, hi.x); lo.y = __fsub_rn(v.y, hi.y); lo.z = __fsub_rn(v.z, hi.z); lo.w = __fsub_rn(v.w, hi.w);
-    const uint32_t dst = smem_base + c * W_CHUNK + swz128(n, pc);
-    sts128(dst, hi);
-    sts128(dst + COUT * 128, lo);
-  }
+  store_weight_planes<COUT>(smem_base, a.w, K, tid, CONS_THREADS);
   fence_proxy_async();
   named_bar_sync(1, CONS_THREADS);
 
@@ -582,56 +570,8 @@ __global__ void __launch_bounds__(tma::THREADS, 1) gemm_tma_kernel(const __grid_
     constexpr int ksteps = decltype(KSTEPS)::value;
     const int stage = m % wstages;
     mbar_wait(bar_full(wgi, stage), (uint32_t)((m / wstages) & 1));
-    const uint32_t st = ring + stage * STAGE_BYTES + fbase;
-    float bA[8], bB[8];
-    if (IN_BN) {
-      const float4* t4 = reinterpret_cast<const float4*>(sBN + (c * 4 + q) * 16);
-      const float4 a0 = t4[0], a1 = t4[1], b0 = t4[2], b1 = t4[3];
-      bA[0] = a0.x; bA[1] = a0.y; bA[2] = a0.z; bA[3] = a0.w; bA[4] = a1.x; bA[5] = a1.y; bA[6] = a1.z; bA[7] = a1.w;
-      bB[0] = b0.x; bB[1] = b0.y; bB[2] = b0.z; bB[3] = b0.w; bB[4] = b1.x; bB[5] = b1.y; bB[6] = b1.z; bB[7] = b1.w;
-    }
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      if (j < ksteps) {
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const uint32_t addr = st + ((uint32_t)((2 * j + h) << 4) ^ fx);
-          float v[2];
-          asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v[0]) : "r"(addr) : "memory");
-          asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v[1]) : "r"(addr + 1024) : "memory");
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            float x = v[e];
-            if (IN_BN) x = fmaxf(fmaf(x, bA[2 * j + h], bB[2 * j + h]), 0.f);
-            const float hi = tf32_hi(x);
-            fh[4 * j + 2 * h + e] = __float_as_uint(hi);
-            fl[4 * j + 2 * h + e] = __float_as_uint(__fsub_rn(x, hi));
-          }
-        }
-      }
-    }
-    fence();
-    const uint32_t w_hi = w_base + c * W_CHUNK, w_lo = w_hi + COUT * 128;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      if (j < ksteps) {
-        const uint32_t first = (c | j) != 0 ? 1u : 0u;
-        if (STACKED) {
-          mma_tile_ra<2 * COUT, BLK>(acc, &fh[4 * j], w_hi + j * 32, first);
-          mma_tile_ra<COUT, BLK>(acc + COUT / 2, &fl[4 * j], w_hi + j * 32, 1u);
-        } else {
-          mma_tile_ra<COUT, BLK>(acc, &fl[4 * j], w_hi + j * 32, first);
-          mma_tile_ra<COUT, BLK>(acc, &fh[4 * j], w_lo + j * 32, 1u);
-          mma_tile_ra<COUT, BLK>(acc, &fh[4 * j], w_hi + j * 32, 1u);
-        }
-      }
-    }
-    commit();
-    // The next chunk rewrites the fragments.  A second fragment buffer (wait_group 1) does not fit: ptxas then
-    // serialises every wgmma for lack of registers.  The other warpgroup's MMAs fill the tensor pipe meanwhile.
-    wait<0>();
-    fence_regs(fh);
-    fence_regs(fl);
+    mma_chunk_3xtf32<COUT, IN_BN, ksteps>(acc, fh, fl, ring + stage * STAGE_BYTES + fbase, fx, sBN + (c * 4 + q) * 16,
+                                          w_base + c * W_CHUNK, c);
     // The stage goes back to the producer only now.  Released straight after the loads, the arrive was scheduled
     // ahead of the loads' results and the TMA could overwrite data that had not been read yet.  The fragments went
     // through the MMAs just waited for, so every value read from the stage has arrived.

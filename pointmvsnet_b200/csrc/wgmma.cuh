@@ -1,5 +1,5 @@
-// Hopper warpgroup MMA (wgmma, kind tf32) and mbarrier primitives shared by the two tensor-core GEMMs
-// (gemm_tc.cu, gemm_ws.cu).  Operands are read from shared memory in the K-major SWIZZLE_128B layout: a row of 32 fp32
+// Hopper warpgroup MMA (wgmma, kind tf32) and mbarrier primitives shared by the tensor-core GEMMs
+// (gemm_tc.cu, gemm_ws.cu) and the fused fetch + first contraction (fetch.cu).  Operands are read from shared memory in the K-major SWIZZLE_128B layout: a row of 32 fp32
 // (128 bytes) per matrix row, 16-byte piece p of row r stored at piece p ^ (r & 7) inside 8-row, 1024-byte atoms.
 #pragma once
 #include <stdint.h>
@@ -177,6 +177,91 @@ __device__ __forceinline__ void mma_tile_ra(float* d, const uint32_t* a, uint32_
   static_assert(N % BLK == 0 && (BLK == 16 || BLK == 32 || BLK == 64), "block shape");
 #pragma unroll
   for (int nb = 0; nb < N / BLK; ++nb) mma_tf32_ra<BLK>(d + (BLK / 2) * nb, a, make_desc(b_addr + nb * BLK * 128), accumulate);
+}
+
+// ---- 3xTF32 with stationary weight planes (gemm_tma_kernel in gemm_ws.cu, fetch_gemm_kernel in fetch.cu) ----------
+// hi = the 10 explicit mantissa bits the tensor core reads, lo = x - hi (exact)
+__device__ __forceinline__ float tf32_hi(float x) { return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
+
+// W [cout, K] -> shared memory at `planes` as the B operand: per 32-column chunk c of K, rows [0, cout) hold W_hi and
+// rows [cout, 2 cout) W_lo, K-major SWIZZLE_128B (chunk c starts 2 * cout * 128 bytes after chunk c - 1), zero beyond K.
+// Thread `t` of `nthreads` writes its share; the caller fences (fence_proxy_async) and synchronises.
+template <int COUT>
+__device__ __forceinline__ void store_weight_planes(uint32_t planes, const float* __restrict__ w, int K, int t,
+                                                    int nthreads) {
+  const int nch = (K + 31) / 32;
+  for (int e = t; e < COUT * nch * 8; e += nthreads) {
+    const int n = e / (nch * 8), rem = e - n * (nch * 8), c = rem >> 3, pc = rem & 7;
+    const int k0 = c * 32 + pc * 4;  // K is a multiple of 8: a 16-byte piece is all inside or all padding
+    const float4 v = k0 < K ? __ldg(reinterpret_cast<const float4*>(w + (size_t)n * K + k0)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    float4 hi, lo;
+    hi.x = tf32_hi(v.x); hi.y = tf32_hi(v.y); hi.z = tf32_hi(v.z); hi.w = tf32_hi(v.w);
+    lo.x = __fsub_rn(v.x, hi.x); lo.y = __fsub_rn(v.y, hi.y); lo.z = __fsub_rn(v.z, hi.z); lo.w = __fsub_rn(v.w, hi.w);
+    const uint32_t dst = planes + c * (2 * COUT * 128) + swz128(n, pc);
+    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "f"(hi.x), "f"(hi.y), "f"(hi.z), "f"(hi.w) : "memory");
+    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(dst + COUT * 128), "f"(lo.x), "f"(lo.y), "f"(lo.z), "f"(lo.w)
+                 : "memory");
+  }
+}
+
+// One 32-column chunk c of a 64-row tile, issued by a warpgroup: the thread reads its A fragments (rows r, r + 8 and
+// columns 8 j + q (+ 4) of k-step j, r = 16 * (warp % 4) + lane / 4, q = lane % 4) from the K-major SWIZZLE_128B
+// box at `st` = box + r * 128 + q * 4 (fx = (r & 7) << 4), applies relu(fma(x, A, B)) when IN_BN (bn = the chunk's
+// [A x 8 | B x 8] of this lane % 4), splits hi / lo and issues the chunk's KSTEPS k-steps against the weight planes at
+// w_hi as one wgmma group, then waits for it: the next chunk rewrites fh / fl.
+template <int COUT, bool IN_BN, int KSTEPS>
+__device__ __forceinline__ void mma_chunk_3xtf32(float* acc, uint32_t (&fh)[16], uint32_t (&fl)[16], uint32_t st,
+                                                 uint32_t fx, const float* bn, uint32_t w_hi, int c) {
+  constexpr bool STACKED = COUT <= 64;
+  constexpr int BLK = COUT < 64 ? COUT : 64;  // one wgmma shape for every product into this accumulator
+  float bA[8], bB[8];
+  if (IN_BN) {
+    const float4* t4 = reinterpret_cast<const float4*>(bn);
+    const float4 a0 = t4[0], a1 = t4[1], b0 = t4[2], b1 = t4[3];
+    bA[0] = a0.x; bA[1] = a0.y; bA[2] = a0.z; bA[3] = a0.w; bA[4] = a1.x; bA[5] = a1.y; bA[6] = a1.z; bA[7] = a1.w;
+    bB[0] = b0.x; bB[1] = b0.y; bB[2] = b0.z; bB[3] = b0.w; bB[4] = b1.x; bB[5] = b1.y; bB[6] = b1.z; bB[7] = b1.w;
+  }
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    if (j < KSTEPS) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t addr = st + ((uint32_t)((2 * j + h) << 4) ^ fx);
+        float v[2];
+        asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v[0]) : "r"(addr) : "memory");
+        asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v[1]) : "r"(addr + 1024) : "memory");
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float x = v[e];
+          if (IN_BN) x = fmaxf(fmaf(x, bA[2 * j + h], bB[2 * j + h]), 0.f);
+          const float hi = tf32_hi(x);
+          fh[4 * j + 2 * h + e] = __float_as_uint(hi);
+          fl[4 * j + 2 * h + e] = __float_as_uint(__fsub_rn(x, hi));
+        }
+      }
+    }
+  }
+  fence();
+  const uint32_t w_lo = w_hi + COUT * 128;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    if (j < KSTEPS) {
+      const uint32_t first = (c | j) != 0 ? 1u : 0u;
+      if (STACKED) {
+        mma_tile_ra<2 * COUT, BLK>(acc, &fh[4 * j], w_hi + j * 32, first);
+        mma_tile_ra<COUT, BLK>(acc + COUT / 2, &fl[4 * j], w_hi + j * 32, 1u);
+      } else {
+        mma_tile_ra<COUT, BLK>(acc, &fl[4 * j], w_hi + j * 32, first);
+        mma_tile_ra<COUT, BLK>(acc, &fh[4 * j], w_lo + j * 32, 1u);
+        mma_tile_ra<COUT, BLK>(acc, &fh[4 * j], w_hi + j * 32, 1u);
+      }
+    }
+  }
+  commit();
+  // A second fragment buffer (wait_group 1) does not fit: ptxas then serialises every wgmma for lack of registers.
+  wait<0>();
+  fence_regs(fh);
+  fence_regs(fl);
 }
 
 }  // namespace wg

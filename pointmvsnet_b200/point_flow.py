@@ -255,7 +255,7 @@ class PointFlow(nn.Module):
             check(lib.pmvs_point_flow_iter(C.byref(shape), C.byref(w), C.byref(pyr_ptrs), ptr(depth), ptr(cams),
                                            ptr(itv), ptr(mean_c), ptr(std_c), ptr(depth_out), ptr(prob_out),
                                            ptr(ws), need, stream_ptr()))
-        self._last = (shape, ws)
+        self._last = (shape, ws, depth)  # debug_stages() recomputes the point features from `depth`
         return depth_out, prob_out
 
     def _validate(self, dev, B, V, pyr, depth, interval, mean, std, cams):
@@ -290,10 +290,14 @@ class PointFlow(nn.Module):
     def debug_stages(self):
         """Views of the last iteration's workspace in the REFERENCE layouts (test helper):
         feature [B,136,5,h,w]-equivalent per sub-cloud etc.  Returns a dict of tensors
-        indexed [S, B, ...]."""
-        shape, ws = self._last
+        indexed [S, B, ...].  The fused fetch of PMVS_OPT_FETCH 3 does not write `feature`: it is recomputed here
+        by the unfused fetch kernel from the workspace and the last call's previous depth map, which must not have
+        been modified since."""
+        shape, ws, depth = self._last
         off = (C.c_size_t * 10)()
         check(lib.pmvs_point_flow_debug_offsets(C.byref(shape), C.byref(off)))
+        with torch.cuda.device(ws.device):
+            check(lib.pmvs_point_flow_debug_feature(C.byref(shape), ptr(depth), ptr(ws), stream_ptr()))
         S = shape.sub_count if shape.sub_count > 0 else shape.ratio * shape.ratio
         hs, wsub = shape.flow_h // shape.ratio, shape.flow_w // shape.ratio
         N = 5 * hs * wsub
