@@ -281,6 +281,42 @@ int pmvs_point_flow_debug_offsets(const pmvs_flow_shape* shape, size_t off[10]);
 int pmvs_point_flow_debug_feature(const pmvs_flow_shape* shape, const float* depth_prev, void* workspace,
                                   pmvs_stream_t stream);
 
+/* ---- backward of one PointFlow iteration (train branch, model.py:150-204, 271-293) ------------ */
+/* Output pointers of pmvs_point_flow_backward.  Every output is overwritten, not accumulated.  The parameter
+ * gradients are required; the input gradients may be NULL ("not needed").  ec_dw12[l] is [conv1.weight ; conv2.weight]
+ * stacked as in pmvs_flow_weights.  dpyramids_cl[l] is [B,V,h_l,w_l,C_l] (the forward's channels-last layout),
+ * ddepth_prev [B,1,prev_h,prev_w]. */
+typedef struct pmvs_flow_grads {
+  float* ec_dw12[3];
+  float* ec_dgamma[3];
+  float* ec_dbeta[3];
+  float* mlp_dw[4];
+  float* mlp_dgamma[3];
+  float* mlp_dbeta[3];
+  float* dpyramids_cl[3];
+  float* ddepth_prev;
+} pmvs_flow_grads;
+
+/* bytes of device workspace pmvs_point_flow_backward needs; 0 (with pmvs_last_error) for a shape it does not take.
+ * The backward takes one cloud per call: ratio 1 (every train-branch call and the test branch at scale 0.125) and
+ * sub_count 0. */
+size_t pmvs_point_flow_backward_workspace_bytes(const pmvs_flow_shape* shape);
+
+/* Gradients of one pmvs_point_flow_iter call with respect to the flow parameters, the pyramids and depth_prev, given
+ * grad_depth_out [B,1,h,w] and grad_prob_out [B,5,h,w] (NULL = zero).  The inputs are those of the forward call and
+ * fwd_workspace is its workspace, unchanged since, with the implementation options (pmvs_set_option,
+ * pmvs_set_gemm_mode) as they were for it; it is only read, so the call can be repeated.  BatchNorm uses the batch
+ * statistics the forward computed.  When neither a pyramid nor depth_prev gradient is requested the fetch backward is
+ * skipped.  Deterministic: no floating-point atomics, every sum in an order fixed by the shapes.  The weight gradients
+ * follow pmvs_set_gemm_mode like the stand-alone EdgeConv backward.  workspace:
+ * pmvs_point_flow_backward_workspace_bytes(shape) bytes, 256-byte aligned, device memory. */
+int pmvs_point_flow_backward(const pmvs_flow_shape* shape, const pmvs_flow_weights* weights,
+                             const float* const pyramids_cl[3], const float* depth_prev,
+                             const float* cam_params, const float* interval, const float* mean,
+                             const float* std, const void* fwd_workspace, const float* grad_depth_out,
+                             const float* grad_prob_out, const pmvs_flow_grads* grads, void* workspace,
+                             size_t workspace_bytes, pmvs_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -43,6 +43,14 @@ class FlowShape(C.Structure):
     ]
 
 
+class FlowGrads(C.Structure):
+    _fields_ = [
+        ("ec_dw12", C.c_void_p * 3), ("ec_dgamma", C.c_void_p * 3), ("ec_dbeta", C.c_void_p * 3),
+        ("mlp_dw", C.c_void_p * 4), ("mlp_dgamma", C.c_void_p * 3), ("mlp_dbeta", C.c_void_p * 3),
+        ("dpyramids_cl", C.c_void_p * 3), ("ddepth_prev", C.c_void_p),
+    ]
+
+
 def _sig(name, restype, argtypes):
     fn = getattr(lib, name)
     fn.restype = restype
@@ -81,13 +89,16 @@ _sig("pmvs_point_flow_iter", I, [C.POINTER(FlowShape), C.POINTER(FlowWeights), C
 _sig("pmvs_pyramid_to_channels_last", I, [P, P, I, I, I, I, P])
 _sig("pmvs_point_flow_debug_offsets", I, [C.POINTER(FlowShape), C.POINTER(C.c_size_t * 10)])
 _sig("pmvs_point_flow_debug_feature", I, [C.POINTER(FlowShape), P, P, P])
+_sig("pmvs_point_flow_backward_workspace_bytes", C.c_size_t, [C.POINTER(FlowShape)])
+_sig("pmvs_point_flow_backward", I, [C.POINTER(FlowShape), C.POINTER(FlowWeights), C.POINTER(C.c_void_p * 3),
+                                     P, P, P, P, P, P, P, P, C.POINTER(FlowGrads), P, C.c_size_t, P])
 
 EXPORTED = [
     "pmvs_version", "pmvs_last_error", "pmvs_launch_count", "pmvs_set_option", "pmvs_get_option", "pmvs_profile_enable", "pmvs_profile_collect", "pmvs_set_gemm_mode", "pmvs_get_gemm_mode", "pmvs_gather_knn_forward",
     "pmvs_gather_knn_backward", "pmvs_gather_knn_backward_det_workspace_bytes", "pmvs_gather_knn_backward_det", "pmvs_knn3d", "pmvs_feature_fetch", "pmvs_feature_fetch_backward",
     "pmvs_cost_volume", "pmvs_transpose", "pmvs_idx64_to_idx32", "pmvs_edgeconv_pm", "pmvs_edgeconv_pm_backward_workspace_bytes", "pmvs_edgeconv_pm_backward", "pmvs_linear_pm", "pmvs_point_flow_workspace_bytes",
     "pmvs_point_flow_iter", "pmvs_pyramid_to_channels_last", "pmvs_point_flow_debug_offsets",
-    "pmvs_point_flow_debug_feature",
+    "pmvs_point_flow_debug_feature", "pmvs_point_flow_backward_workspace_bytes", "pmvs_point_flow_backward",
 ]
 
 

@@ -211,6 +211,17 @@ static FusedFetchParams fetch_params(const pmvs_flow_shape* s, const FlowPlan& p
   return f;
 }
 
+int flow_regions(const pmvs_flow_shape* s, FlowRegions& r) {
+  FlowPlan p;
+  PMVS_TRY(make_plan(s, p));
+  r.cam = p.cam; r.feature = p.feature; r.xyz = p.xyz; r.idx = p.idx; r.le = p.le; r.ecat = p.ecat; r.h0 = p.h0;
+  r.h1 = p.h1; r.h2 = p.h2; r.warp_src = p.warp_src; r.cand = p.cand; r.stats = p.stats; r.coef = p.coef;
+  r.total = p.total;
+  for (int l = 0; l < 3; ++l) { r.st_ec[l] = p.st_ec[l]; r.st_ecn[l] = p.st_ecn[l]; r.st_mlp[l] = p.st_mlp[l]; }
+  r.S = p.S;
+  return PMVS_OK;
+}
+
 }  // namespace pmvs
 
 using namespace pmvs;

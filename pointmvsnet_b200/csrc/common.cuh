@@ -181,6 +181,44 @@ size_t inv_lists_bytes(long long B, long long N, long long K);
 int build_inv_lists(const int64_t* idx, int B, int N, int K, void* ws, const int** off, const int** list,
                     const char* prof_name, cudaStream_t st);
 
+// One EdgeConv / EdgeConvNoC layer's backward (edge_bwd.cu), batch-statistic or frozen BatchNorm, for B clouds of N
+// points in one BatchNorm group: dgamma, dbeta, dLE (into `dle`, [B*N, 2*cout]), dX (if dx != NULL) and dW12.  The
+// inverse neighbour lists are the caller's (build_inv_lists), so several layers can share them.  tile_coef != NULL:
+// the ReLU mask of the neighbour half is the tile family's (edge_tile.cu coefficient table of the forward).
+struct EdgeLayerBwd {
+  const float* x;
+  int ldx;
+  const int32_t* idx32;
+  const int* inv_off;
+  const int* inv_list;
+  const float* w12;
+  const float* gamma;
+  const float* beta;
+  float eps;
+  int concat_central, bn_train;
+  const float* le;
+  const double* stats;  // [sum_c | sumsq_c | sum_n | sumsq_n] x cout
+  const float* tile_coef;
+  const float* dy;
+  int lddy;
+  float* dx;
+  int lddx;
+  float* dw12;
+  float* dgamma;
+  float* dbeta;
+  float* dle;
+  char* scratch;  // edge_layer_bwd_scratch_bytes(B*N, cin, cout), 256-byte aligned
+  int B, N, K, cin, cout;
+};
+size_t edge_layer_bwd_scratch_bytes(long long R, int cin, int cout);
+int edge_layer_backward(const EdgeLayerBwd& L, cudaStream_t st);
+// dw [M2, cin] = dy^T x over R rows (dy [R, M2] dense, x [R, ldx]): fixed 1024-row slabs on the tensor cores (3xTF32,
+// or TF32 under gemm mode 1) when the shape has a wgmma kernel, fp32 SIMT otherwise, then the slabs in order in fp64.
+// wpart: weight_grad_scratch_bytes(R, M2, cin).
+size_t weight_grad_scratch_bytes(long long R, int M2, int cin);
+int launch_weight_grad(const float* dy, const float* x, int ldx, int cin, int M2, int R, float* wpart, float* dw,
+                       const char* simt_name, cudaStream_t st);
+
 // EdgeConv statistics / apply on a structured cloud, neighbour rows gathered from a TMA-loaded
 // shared-memory halo tile (edge_tile.cu)
 struct EdgeTileArgs {
@@ -222,6 +260,22 @@ int launch_fused_fetch(const FusedFetchParams& p, cudaStream_t st);
 // Returns -1 when it does not take the call (5 V > 30, or the shared memory cannot be had)
 int launch_fetch_gemm(const FusedFetchParams& p, const float* w12, float* le, cudaStream_t st);
 size_t cam_block_bytes(int B, int V);
+// Backward of the fetch (fetch.cu) for S = 1, ratio 1: from dF0 [B*N, 136] (rows in fetch order) and the depth
+// gradient of the output map, ddup [B,h,w] = d depth_up (the skip plus the xyz columns through the hypothesis depths);
+// with dfv != NULL also the variance columns' gradient per (pixel, hypothesis, view) dfv [B*h*w*5*V, 112] and its tap
+// records rec_idx / rec_w [B*h*w*5*V*4] (texel of the batch element's [V*h*w] map, -1 = none).
+struct FetchBwdParams {
+  FusedFetchParams f;     // the forward's fetch parameters (feature = dF0)
+  const float* ddepth_out;  // [B,h,w]
+  float* ddup;
+  float* dfv;
+  int64_t* rec_idx;
+  float* rec_w;
+};
+int launch_fetch_backward(const FetchBwdParams& p, cudaStream_t st);
+// d warp source [B][V*h*w][112] -> d pyramid level l [B*V, hl, wl, 16 << l] (the transpose of warp_source_kernel)
+int launch_warp_source_backward(const float* dsrc, const int hl[3], const int wl[3], float* const dpyr[3], int B, int V,
+                                int h, int w, cudaStream_t st);
 
 struct HeadArgs {
   const float* h2;        // [S*B*N, 16]
@@ -238,6 +292,17 @@ struct HeadArgs {
   int sub_begin;            // group s of this launch is sub-cloud sub_begin + s of the iteration
 };
 int launch_flow_head(const HeadArgs& a, cudaStream_t st);
+// byte offsets of the regions of pmvs_point_flow_iter's workspace (api.cu make_plan) and the double offsets of the
+// BatchNorm sums inside `stats`, for the backward that reads it
+struct FlowRegions {
+  size_t cam, feature, xyz, idx, le, ecat, h0, h1, h2, warp_src, cand, stats, coef, total;
+  size_t st_ec[3], st_ecn[3], st_mlp[3];
+  int S;
+};
+int flow_regions(const pmvs_flow_shape* s, FlowRegions& r);
+// whether launch_gemm applies a fused input BatchNorm as relu(fma(x, A, B)) (gemm_ws.cu) rather than ATen's
+// ((x - mean) * invstd) * gamma + beta (the other kernels); the two can differ in the last bit of the pre-activation
+bool gemm_in_bn_fma_form(const GemmArgs& a);
 
 struct RunUpdate {
   const double* stats;  // per group: [sum(C), sumsq(C)] at stride `gstride` doubles

@@ -52,7 +52,16 @@ struct BwdArgs {
   const int* list;
   float* dle;  // [R, 2*cout]
   int R, N, K, cout;
+  // NULL: the neighbour pre-activation is edge_nb_pre(e, A, edge_nb_offset(mean, l, A, beta)) (edge_kernel's sequence);
+  // else the tile family's table (edge_tile.cu, [A | B] x cout): fma(e, A, fma(-l, A, B)), the sequence it applied
+  const float* tcoef;
 };
+
+// c0 of the neighbour pre-activation pre = fma(e, A, c0) in the sequence of the family that ran the forward
+__device__ __forceinline__ float bwd_nb_offset(const float* tcoef, int c, int cout, float mean, float l, float A,
+                                               float beta) {
+  return tcoef ? __fmaf_rn(-l, A, __ldg(tcoef + cout + c)) : edge_nb_offset(mean, l, A, beta);
+}
 
 __device__ __forceinline__ float bwd_xhat(float d, float mean, float istd) { return __fmul_rn(__fsub_rn(d, mean), istd); }
 
@@ -107,8 +116,8 @@ __global__ void __launch_bounds__(EB_THREADS) edge_bwd_stats_kernel(const BwdArg
     float A[4], c0[4];
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
-      A[q] = edge_nb_scale(is[q], c_g[1][cl + q]);
-      c0[q] = edge_nb_offset(m[q], l4[q], A[q], c_b[1][cl + q]);
+      A[q] = a.tcoef ? __ldg(a.tcoef + cl + q) : edge_nb_scale(is[q], c_g[1][cl + q]);
+      c0[q] = bwd_nb_offset(a.tcoef, cl + q, COUT, m[q], l4[q], A[q], c_b[1][cl + q]);
     }
     const int32_t* ip = a.idx + (size_t)r * K;
     auto body = [&](int nb) {
@@ -221,7 +230,7 @@ __global__ void __launch_bounds__(EB_THREADS) edge_bwd_dle_kernel(const BwdArgs 
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
     m[q] = cf[1][CF_MEAN][cl + q]; is[q] = cf[1][CF_ISTD][cl + q]; bt[q] = cf[1][CF_BETA][cl + q];
-    A[q] = edge_nb_scale(is[q], cf[1][CF_GAMMA][cl + q]);
+    A[q] = a.tcoef ? __ldg(a.tcoef + cl + q) : edge_nb_scale(is[q], cf[1][CF_GAMMA][cl + q]);
     gm[q] = cf[1][CF_GM][cl + q]; gxm[q] = cf[1][CF_GXM][cl + q];
   }
   const int p0 = blockIdx.x * EB_PTS;
@@ -237,7 +246,7 @@ __global__ void __launch_bounds__(EB_THREADS) edge_bwd_dle_kernel(const BwdArgs 
     const float g4[4] = {gk.x, gk.y, gk.z, gk.w};
     float c0[4], dl[4] = {0.f, 0.f, 0.f, 0.f}, de[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-    for (int q = 0; q < 4; ++q) c0[q] = edge_nb_offset(m[q], l4[q], A[q], bt[q]);
+    for (int q = 0; q < 4; ++q) c0[q] = bwd_nb_offset(a.tcoef, cl + q, COUT, m[q], l4[q], A[q], bt[q]);
     // dlocal: -(sum over j's own K neighbours), k ascending
     const int32_t* ip = a.idx + (size_t)r * K;
     auto own = [&](int nb) {
@@ -285,7 +294,7 @@ __global__ void __launch_bounds__(EB_THREADS) edge_bwd_dle_kernel(const BwdArgs 
       const float ln4[4] = {ln.x, ln.y, ln.z, ln.w}, gn4[4] = {gn.x, gn.y, gn.z, gn.w};
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
-        const float c0n = edge_nb_offset(m[q], ln4[q], A[q], bt[q]);
+        const float c0n = bwd_nb_offset(a.tcoef, cl + q, COUT, m[q], ln4[q], A[q], bt[q]);
         de[q] = __fadd_rn(de[q], bwd_dd(e4j[q], ln4[q], c0n, gn4[q], A[q], m[q], is[q], gm[q], gxm[q]));
       }
     }
@@ -511,7 +520,8 @@ int launch_wgrad_wgmma(const float* dle, const float* x, int ldx, int cin, int M
   PMVS_WG_CASE(64, 136, 144)  // EdgeConvNoC 136 -> 32
   PMVS_WG_CASE(64, 32, 32)    // EdgeConv 32 -> 32
   PMVS_WG_CASE(128, 64, 64)   // EdgeConv 64 -> 64
-  PMVS_WG_CASE(64, 64, 64)
+  PMVS_WG_CASE(64, 64, 64)    // flow_mlp.0.1 (PointFlow backward)
+  PMVS_WG_CASE(64, 224, 224)  // flow_mlp.0.0
   PMVS_WG_CASE(128, 32, 32)
   PMVS_WG_CASE(128, 136, 144)
 #undef PMVS_WG_CASE
@@ -525,23 +535,34 @@ int launch_tile_gemm(const TileGemm& t, int slabs, const char* name, cudaStream_
   return check_launch("tile_gemm_kernel", st);
 }
 
-struct BwdPlan {
+// scratch of one layer's backward (edge_layer_backward), and the stand-alone entry's workspace: the layer scratch, then
+// the inverse lists and dLE
+struct LayerPlan {
   int ctas, slabs;
-  size_t part, coef, inv, dle, w12t, wpart, total;
+  size_t part, coef, w12t, wpart, total;
 };
-BwdPlan bwd_plan(long long B, long long N, long long K, long long cin, long long cout) {
+LayerPlan layer_plan(long long R, long long cin, long long cout) {
   auto up = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  const long long R = B * N;
-  BwdPlan p{};
+  LayerPlan p{};
   p.ctas = (int)((R + EB_PTS - 1) / EB_PTS);
   p.slabs = (int)((R + WG_SLAB - 1) / WG_SLAB);
   size_t o = 0;
   p.part = o; o += up((size_t)p.ctas * 4 * cout * 8);
   p.coef = o; o += up((size_t)2 * CF_ROWS * cout * 4);
-  p.inv = o; o += up(inv_lists_bytes(B, N, K));
-  p.dle = o; o += up((size_t)R * 2 * cout * 4);
   p.w12t = o; o += up((size_t)cin * 2 * cout * 4);
   p.wpart = o; o += up((size_t)p.slabs * 2 * cout * cin * 4);
+  p.total = o;
+  return p;
+}
+struct BwdPlan {
+  size_t inv, dle, total;
+};
+BwdPlan bwd_plan(long long B, long long N, long long K, long long cin, long long cout) {
+  auto up = [](size_t x) { return (x + 255) & ~(size_t)255; };
+  BwdPlan p{};
+  size_t o = layer_plan(B * N, cin, cout).total;
+  p.inv = o; o += up(inv_lists_bytes(B, N, K));
+  p.dle = o; o += up((size_t)B * N * 2 * cout * 4);
   p.total = o;
   return p;
 }
@@ -552,6 +573,92 @@ bool bwd_shape_ok(long long B, long long N, long long K, long long cin, long lon
 }
 
 }  // namespace
+
+size_t weight_grad_scratch_bytes(long long R, int M2, int cin) {
+  return (size_t)((R + WG_SLAB - 1) / WG_SLAB) * M2 * cin * sizeof(float);
+}
+
+int launch_weight_grad(const float* dy, const float* x, int ldx, int cin, int M2, int R, float* wpart, float* dw,
+                       const char* simt_name, cudaStream_t st) {
+  const int slabs = cdiv(R, WG_SLAB);
+  const int rc = launch_wgrad_wgmma(dy, x, ldx, cin, M2, R, slabs, wpart, st);
+  if (rc > 0) return rc;
+  if (rc < 0) {
+    TileGemm t{};
+    t.a = dy; t.a_m = 1; t.a_k = M2; t.b = x; t.b_k = ldx; t.b_n = 1; t.c = wpart; t.ldc = cin;
+    t.c_slab = (long long)M2 * cin; t.M = M2; t.Nn = cin; t.Kd = R; t.kslab = WG_SLAB; t.mt = cdiv(M2, TG_BM);
+    PMVS_TRY(launch_tile_gemm(t, slabs, simt_name, st));
+  }
+  prof_begin("edge_bwd_wgrad_reduce", st);
+  slab_reduce_kernel<<<cdiv((long long)M2 * cin, 256), 256, 0, st>>>(wpart, dw, M2 * cin, slabs);
+  return check_launch("slab_reduce_kernel", st);
+}
+
+size_t edge_layer_bwd_scratch_bytes(long long R, int cin, int cout) { return layer_plan(R, cin, cout).total; }
+
+int edge_layer_backward(const EdgeLayerBwd& L, cudaStream_t st) {
+  const int cout = L.cout, cin = L.cin, R = L.B * L.N, C2 = 2 * cout;
+  const LayerPlan p = layer_plan(R, cin, cout);
+  auto at = [&](size_t off) { return L.scratch + off; };
+  BwdArgs a{};
+  a.le = L.le; a.idx = L.idx32; a.stats = L.stats; a.gamma = L.gamma; a.beta = L.beta; a.eps = L.eps;
+  a.concat_central = L.concat_central ? 1 : 0; a.bn_train = L.bn_train ? 1 : 0; a.dy = L.dy; a.lddy = L.lddy;
+  a.part = (double*)at(p.part); a.coef = (float*)at(p.coef); a.dgamma = L.dgamma; a.dbeta = L.dbeta;
+  a.off = L.inv_off; a.list = L.inv_list;
+  a.dle = L.dle; a.R = R; a.N = L.N; a.K = L.K; a.cout = cout; a.tcoef = L.tile_coef;
+
+  // 1. sums of g and g * xhat -> dgamma, dbeta, coefficient table
+  static const char* const sn[4] = {"edge_bwd_stats_16", "edge_bwd_stats_32", "edge_bwd_stats_64", "edge_bwd_stats_128"};
+  static const char* const dn[4] = {"edge_bwd_dle_16", "edge_bwd_dle_32", "edge_bwd_dle_64", "edge_bwd_dle_128"};
+  const int ci = cout == 16 ? 0 : (cout == 32 ? 1 : (cout == 64 ? 2 : 3));
+  prof_begin(sn[ci], st);
+#define PMVS_BWD_CASE(KERNEL, C)                                             \
+  case C:                                                                    \
+    if (L.K == 16) KERNEL<C, 16><<<p.ctas, EB_THREADS, 0, st>>>(a);          \
+    else KERNEL<C, 0><<<p.ctas, EB_THREADS, 0, st>>>(a);                     \
+    break;
+  switch (cout) {
+    PMVS_BWD_CASE(edge_bwd_stats_kernel, 16)
+    PMVS_BWD_CASE(edge_bwd_stats_kernel, 32)
+    PMVS_BWD_CASE(edge_bwd_stats_kernel, 64)
+    PMVS_BWD_CASE(edge_bwd_stats_kernel, 128)
+  }
+  PMVS_TRY(check_launch("edge_bwd_stats_kernel", st));
+  prof_begin("edge_bwd_finish", st);
+  edge_bwd_finish_kernel<<<cout, FIN_THREADS, 0, st>>>(a, p.ctas);
+  PMVS_TRY(check_launch("edge_bwd_finish_kernel", st));
+
+  // 2. dLE
+  prof_begin(dn[ci], st);
+  switch (cout) {
+    PMVS_BWD_CASE(edge_bwd_dle_kernel, 16)
+    PMVS_BWD_CASE(edge_bwd_dle_kernel, 32)
+    PMVS_BWD_CASE(edge_bwd_dle_kernel, 64)
+    PMVS_BWD_CASE(edge_bwd_dle_kernel, 128)
+  }
+#undef PMVS_BWD_CASE
+  PMVS_TRY(check_launch("edge_bwd_dle_kernel", st));
+
+  // 3. dX = dLE * W12
+  if (L.dx != nullptr) {
+    if (C2 <= 224) {
+      float* w12t = (float*)at(p.w12t);
+      PMVS_TRY(launch_transpose(L.w12, w12t, 1, C2, cin, st));
+      GemmArgs g{};
+      g.x = a.dle; g.ldx = C2; g.w = w12t; g.y = L.dx; g.ldy = L.lddx;
+      g.groups = 1; g.rows_per_group = R; g.cin = C2; g.cout = cin; g.eps = L.eps;
+      PMVS_TRY(launch_gemm(g, st));
+    } else {  // the contraction is longer than the GEMM kernels take
+      TileGemm t{};
+      t.a = a.dle; t.a_m = C2; t.a_k = 1; t.b = L.w12; t.b_k = cin; t.b_n = 1; t.c = L.dx; t.ldc = L.lddx; t.c_slab = 0;
+      t.M = R; t.Nn = cin; t.Kd = C2; t.kslab = C2; t.mt = cdiv(R, TG_BM);
+      PMVS_TRY(launch_tile_gemm(t, 1, "edge_bwd_dx_simt", st));
+    }
+  }
+
+  // 4. dW12 = dLE^T X over fixed row slabs, then the slabs in order
+  return launch_weight_grad(a.dle, L.x, L.ldx, cin, C2, R, (float*)at(p.wpart), L.dw12, "edge_bwd_wgrad_simt", st);
+}
 
 }  // namespace pmvs
 
@@ -585,79 +692,12 @@ extern "C" int pmvs_edgeconv_pm_backward(const float* x, int ldx, const int32_t*
   }
   cudaStream_t st = (cudaStream_t)stream;
   char* ws = (char*)workspace;
-  const int R = B * N, C2 = 2 * cout;
-  BwdArgs a{};
-  a.le = le; a.idx = idx32; a.stats = stats; a.gamma = gamma; a.beta = beta; a.eps = eps;
-  a.concat_central = concat_central ? 1 : 0; a.bn_train = bn_train ? 1 : 0; a.dy = dy; a.lddy = lddy;
-  a.part = (double*)(ws + p.part); a.coef = (float*)(ws + p.coef); a.dgamma = dgamma; a.dbeta = dbeta;
-  a.dle = (float*)(ws + p.dle); a.R = R; a.N = N; a.K = K; a.cout = cout;
-
-  // 1. sums of g and g * xhat -> dgamma, dbeta, coefficient table
-  static const char* const sn[4] = {"edge_bwd_stats_16", "edge_bwd_stats_32", "edge_bwd_stats_64", "edge_bwd_stats_128"};
-  static const char* const dn[4] = {"edge_bwd_dle_16", "edge_bwd_dle_32", "edge_bwd_dle_64", "edge_bwd_dle_128"};
-  const int ci = cout == 16 ? 0 : (cout == 32 ? 1 : (cout == 64 ? 2 : 3));
-  prof_begin(sn[ci], st);
-#define PMVS_BWD_CASE(KERNEL, C)                                             \
-  case C:                                                                    \
-    if (K == 16) KERNEL<C, 16><<<p.ctas, EB_THREADS, 0, st>>>(a);            \
-    else KERNEL<C, 0><<<p.ctas, EB_THREADS, 0, st>>>(a);                     \
-    break;
-  switch (cout) {
-    PMVS_BWD_CASE(edge_bwd_stats_kernel, 16)
-    PMVS_BWD_CASE(edge_bwd_stats_kernel, 32)
-    PMVS_BWD_CASE(edge_bwd_stats_kernel, 64)
-    PMVS_BWD_CASE(edge_bwd_stats_kernel, 128)
-  }
-  PMVS_TRY(check_launch("edge_bwd_stats_kernel", st));
-  prof_begin("edge_bwd_finish", st);
-  edge_bwd_finish_kernel<<<cout, FIN_THREADS, 0, st>>>(a, p.ctas);
-  PMVS_TRY(check_launch("edge_bwd_finish_kernel", st));
-
-  // 2. inverse neighbour lists
-  PMVS_TRY(build_inv_lists(idx64, B, N, K, ws + p.inv, &a.off, &a.list, "edge_bwd_lists", st));
-
-  // 3. dLE
-  prof_begin(dn[ci], st);
-  switch (cout) {
-    PMVS_BWD_CASE(edge_bwd_dle_kernel, 16)
-    PMVS_BWD_CASE(edge_bwd_dle_kernel, 32)
-    PMVS_BWD_CASE(edge_bwd_dle_kernel, 64)
-    PMVS_BWD_CASE(edge_bwd_dle_kernel, 128)
-  }
-#undef PMVS_BWD_CASE
-  PMVS_TRY(check_launch("edge_bwd_dle_kernel", st));
-
-  // 4. dX = dLE * W12
-  if (dx != nullptr) {
-    if (C2 <= 224) {
-      float* w12t = (float*)(ws + p.w12t);
-      PMVS_TRY(launch_transpose(w12, w12t, 1, C2, cin, st));
-      GemmArgs g{};
-      g.x = a.dle; g.ldx = C2; g.w = w12t; g.y = dx; g.ldy = lddx;
-      g.groups = 1; g.rows_per_group = R; g.cin = C2; g.cout = cin; g.eps = eps;
-      PMVS_TRY(launch_gemm(g, st));
-    } else {  // the contraction is longer than the GEMM kernels take
-      TileGemm t{};
-      t.a = a.dle; t.a_m = C2; t.a_k = 1; t.b = w12; t.b_k = cin; t.b_n = 1; t.c = dx; t.ldc = lddx; t.c_slab = 0;
-      t.M = R; t.Nn = cin; t.Kd = C2; t.kslab = C2; t.mt = cdiv(R, TG_BM);
-      PMVS_TRY(launch_tile_gemm(t, 1, "edge_bwd_dx_simt", st));
-    }
-  }
-
-  // 5. dW12 = dLE^T X over fixed row slabs, then the slabs in order
-  {
-    float* wpart = (float*)(ws + p.wpart);
-    const int rc = launch_wgrad_wgmma(a.dle, x, ldx, cin, C2, R, p.slabs, wpart, st);
-    if (rc > 0) return rc;
-    if (rc < 0) {
-      TileGemm t{};
-      t.a = a.dle; t.a_m = 1; t.a_k = C2; t.b = x; t.b_k = ldx; t.b_n = 1; t.c = wpart; t.ldc = cin;
-      t.c_slab = (long long)C2 * cin; t.M = C2; t.Nn = cin; t.Kd = R; t.kslab = WG_SLAB; t.mt = cdiv(C2, TG_BM);
-      PMVS_TRY(launch_tile_gemm(t, p.slabs, "edge_bwd_wgrad_simt", st));
-    }
-    prof_begin("edge_bwd_wgrad_reduce", st);
-    slab_reduce_kernel<<<cdiv((long long)C2 * cin, 256), 256, 0, st>>>(wpart, dw12, C2 * cin, p.slabs);
-    PMVS_TRY(check_launch("slab_reduce_kernel", st));
-  }
-  return PMVS_OK;
+  EdgeLayerBwd L{};
+  L.x = x; L.ldx = ldx; L.idx32 = idx32; L.w12 = w12; L.gamma = gamma; L.beta = beta; L.eps = eps;
+  L.concat_central = concat_central; L.bn_train = bn_train; L.le = le; L.stats = stats; L.dy = dy; L.lddy = lddy;
+  L.dx = dx; L.lddx = lddx; L.dw12 = dw12; L.dgamma = dgamma; L.dbeta = dbeta;
+  L.dle = (float*)(ws + p.dle); L.B = B; L.N = N; L.K = K; L.cin = cin; L.cout = cout;
+  PMVS_TRY(build_inv_lists(idx64, B, N, K, ws + p.inv, &L.inv_off, &L.inv_list, "edge_bwd_lists", st));
+  L.scratch = ws;
+  return edge_layer_backward(L, st);
 }

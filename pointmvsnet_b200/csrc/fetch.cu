@@ -906,6 +906,184 @@ int launch_fetch_gemm(const FusedFetchParams& p0, const float* w12, float* le, c
 
 size_t cam_block_bytes(int B, int V) { return (size_t)B * cam_block_floats(V) * sizeof(float); }
 
+// ---------------------------------------------------------------------------------------
+// backward of rows a2-a9 (PointFlow backward, S = 1): one warp per pixel recomputes the forward's descriptors
+// (fetch_describe), then
+//   * xyz columns: d xyz[m] = sum of the 8 tiled copies of each component, and xyz = (R0^-1 (uv d_m - t0) - mean) / std
+//     is linear in d_m = depth_up + interval (m - 2), so d depth_up += sum_m sum_c d xyz_c / std_c (R0^-1 uv)_c;
+//   * variance columns (dfv != NULL): var = mean_v f_v^2 - (mean_v f_v)^2, so d f_v = dvar * 2 (f_v - mean) / V with
+//     f_v recomputed from the 4 taps (the forward's arithmetic), written per (pixel, hypothesis, view), plus the 4 tap
+//     records (texel, weight) of each (hypothesis, view) for the deterministic texel sums.
+// The coordinates carry no gradient (feature_fetcher.py:29).
+__global__ void __launch_bounds__(FETCH_WARPS * 32) fetch_bwd_kernel(const FetchBwdParams q) {
+  extern __shared__ __align__(16) unsigned char dyn_smem[];
+  const FusedFetchParams& p = q.f;
+  const int V = p.V, h = p.h, w = p.w, npair = PMVS_NUM_HYP * V;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  Desc* desc = reinterpret_cast<Desc*>(dyn_smem) + (size_t)warp * npair;
+  float* xyzs = reinterpret_cast<float*>(dyn_smem + fetch_smem_bytes(V)) + warp * 16;
+  const long long pix = (long long)blockIdx.x * FETCH_WARPS + warp;
+  if (pix >= (long long)p.B * h * w) return;  // warp-uniform
+  const int b = (int)(pix / ((long long)h * w)), pp = (int)(pix - (long long)b * h * w);
+  const int Y = pp / w, X = pp - Y * w;
+  const float* cam = p.cam_blocks + (size_t)b * cam_block_floats(V);
+  fetch_describe<false>(p, cam, desc, xyzs, lane, b, X, Y);
+  __syncwarp();
+  const int HW = h * w, N = PMVS_NUM_HYP * HW;
+  const float* drow0 = p.feature + ((size_t)b * N + pp) * PMVS_FEAT_CH;  // hypothesis 0; + m * HW rows
+  // ---- depth through the xyz columns
+  float dd = 0.f;
+  if (lane < PMVS_NUM_HYP) {
+    const float* dr = drow0 + (size_t)lane * HW * PMVS_FEAT_CH + 112;
+    float dx3[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+    for (int c = 0; c < 24; ++c) dx3[c % 3] = __fadd_rn(dx3[c % 3], __ldg(dr + c));
+    const float px = (float)X + 0.5f, py = (float)Y + 0.5f;
+    const float uvx = dot3(cam + CB_KINV + 0, px, py, 1.f);
+    const float uvy = dot3(cam + CB_KINV + 3, px, py, 1.f);
+    const float uvz = dot3(cam + CB_KINV + 6, px, py, 1.f);
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+      dd = fmaf(__fdiv_rn(dx3[c], cam[CB_STD + c]), dot3(cam + CB_R0INV + 3 * c, uvx, uvy, uvz), dd);
+  }
+  float dsum = 0.f;
+#pragma unroll
+  for (int m = 0; m < PMVS_NUM_HYP; ++m) dsum = __fadd_rn(dsum, __shfl_sync(0xffffffffu, dd, m));
+  if (lane == 0) q.ddup[pix] = __fadd_rn(__ldg(q.ddepth_out + pix), dsum);
+  if (q.dfv == nullptr) return;
+  // ---- tap records of this pixel: record (m V + v) * 4 + tap
+  const unsigned zero_tex = (unsigned)(V * h * w) * (unsigned)FETCH_C4;
+  const size_t rbase = (size_t)pix * npair;
+  for (int t = lane; t < npair; t += 32) {
+    const Desc dt = desc[t];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      q.rec_idx[(rbase + t) * 4 + k] = dt.o[k] == zero_tex ? -1 : (int64_t)(dt.o[k] / FETCH_C4);
+      q.rec_w[(rbase + t) * 4 + k] = dt.w[k];
+    }
+  }
+  if (lane >= FETCH_C4) return;
+  const float4* src = reinterpret_cast<const float4*>(p.src) + (size_t)b * ((size_t)V * h * w + 1) * FETCH_C4 + lane;
+  const float rV = __frcp_rn((float)V);
+#pragma unroll 1
+  for (int m = 0; m < PMVS_NUM_HYP; ++m) {
+    float4 f[PMVS_MAX_VIEWS];
+    float4 s1 = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int v = 0; v < PMVS_MAX_VIEWS; ++v) {
+      if (v < V) {
+        const Desc dv = desc[m * V + v];
+        const float4 t0 = __ldg(src + dv.o[0]), t1 = __ldg(src + dv.o[1]);
+        const float4 t2 = __ldg(src + dv.o[2]), t3 = __ldg(src + dv.o[3]);
+        float4 a;
+        a.x = fmaf(t3.x, dv.w[3], fmaf(t2.x, dv.w[2], fmaf(t1.x, dv.w[1], __fmul_rn(t0.x, dv.w[0]))));
+        a.y = fmaf(t3.y, dv.w[3], fmaf(t2.y, dv.w[2], fmaf(t1.y, dv.w[1], __fmul_rn(t0.y, dv.w[0]))));
+        a.z = fmaf(t3.z, dv.w[3], fmaf(t2.z, dv.w[2], fmaf(t1.z, dv.w[1], __fmul_rn(t0.z, dv.w[0]))));
+        a.w = fmaf(t3.w, dv.w[3], fmaf(t2.w, dv.w[2], fmaf(t1.w, dv.w[1], __fmul_rn(t0.w, dv.w[0]))));
+        f[v] = a;
+        s1.x = __fadd_rn(s1.x, a.x); s1.y = __fadd_rn(s1.y, a.y);
+        s1.z = __fadd_rn(s1.z, a.z); s1.w = __fadd_rn(s1.w, a.w);
+      }
+    }
+    const float4 dv4 = ldg4(drow0 + (size_t)m * HW * PMVS_FEAT_CH + lane * 4);
+    // 2 dvar / V, then times (f_v - mean)
+    const float4 g = make_float4(__fmul_rn(2.f * dv4.x, rV), __fmul_rn(2.f * dv4.y, rV), __fmul_rn(2.f * dv4.z, rV),
+                                 __fmul_rn(2.f * dv4.w, rV));
+    const float4 mu = make_float4(__fmul_rn(s1.x, rV), __fmul_rn(s1.y, rV), __fmul_rn(s1.z, rV), __fmul_rn(s1.w, rV));
+#pragma unroll
+    for (int v = 0; v < PMVS_MAX_VIEWS; ++v) {
+      if (v < V) {
+        const float4 a = f[v];
+        st4(q.dfv + ((rbase + m * V + v) * FETCH_C4 + lane) * 4,
+            make_float4(__fmul_rn(g.x, __fsub_rn(a.x, mu.x)), __fmul_rn(g.y, __fsub_rn(a.y, mu.y)),
+                        __fmul_rn(g.z, __fsub_rn(a.z, mu.z)), __fmul_rn(g.w, __fsub_rn(a.w, mu.w))));
+      }
+    }
+  }
+}
+
+int launch_fetch_backward(const FetchBwdParams& q0, cudaStream_t st) {
+  FetchBwdParams q = q0;
+  PMVS_TRY(fetch_setup(q0.f, q.f));
+  PMVS_REQUIRE(q.f.ratio == 1 && q.f.sub_count == 1 && q.f.sub_begin == 0, "fetch_backward: S = 1 only");
+  const long long npix = (long long)q.f.B * q.f.h * q.f.w;
+  prof_begin("fetch_bwd", st);
+  fetch_bwd_kernel<<<cdiv(npix, FETCH_WARPS), FETCH_WARPS * 32, fetch_smem_total(q.f.V), st>>>(q);
+  return check_launch("fetch_bwd_kernel", st);
+}
+
+// transpose of warp_source_kernel: every texel (yi, xi) of level l gathers the output pixels whose bilinear window
+// holds it.  The source index is monotone in the output index, so those pixels lie in a window of rows
+// [(yi - .5) / sy - .5, (yi + 1.5) / sy - .5] (one row of margin each side for rounding) and likewise for columns; each
+// candidate's taps are recomputed with the forward's arithmetic and matched exactly.  Rows then columns ascending.
+struct WarpSourceBwd {
+  const float* dsrc;  // [B][V*h*w + 1][112] (the trailing texel of each batch element is not read)
+  float* dpyr;        // [B*V, hl, wl, C]
+  int hl, wl, C, coff, h, w, V;
+  float sy, sx;
+};
+__device__ __forceinline__ void src_index(float s, int o, int n_in, int& i0, int& i1, float& l0, float& l1) {
+  float f = __fsub_rn(__fmul_rn(s, (float)o + 0.5f), 0.5f);
+  f = f < 0.f ? 0.f : f;
+  i0 = (int)f;
+  i0 = i0 > n_in - 1 ? n_in - 1 : i0;
+  i1 = i0 + (i0 < n_in - 1 ? 1 : 0);
+  l1 = __fsub_rn(f, (float)i0);
+  l0 = __fsub_rn(1.f, l1);
+}
+__global__ void __launch_bounds__(256) warp_source_bwd_kernel(const WarpSourceBwd a) {
+  const int C4 = a.C / 4;
+  const long long e = (long long)blockIdx.x * 256 + threadIdx.x;
+  const long long per_view = (long long)a.hl * a.wl * C4;
+  const int bv = blockIdx.y;
+  if (e >= per_view) return;
+  const int c4 = (int)(e % C4);
+  const int xi = (int)((e / C4) % a.wl), yi = (int)(e / ((long long)C4 * a.wl));
+  const int bb = bv / a.V;
+  const float4* src = reinterpret_cast<const float4*>(a.dsrc) + ((size_t)bv * a.h * a.w + bb) * FETCH_C4 + a.coff / 4 + c4;
+  int ylo = (int)floorf(((float)yi - 0.5f) / a.sy - 0.5f) - 1, yhi = (int)ceilf(((float)yi + 1.5f) / a.sy - 0.5f) + 1;
+  int xlo = (int)floorf(((float)xi - 0.5f) / a.sx - 0.5f) - 1, xhi = (int)ceilf(((float)xi + 1.5f) / a.sx - 0.5f) + 1;
+  ylo = max(ylo, 0); xlo = max(xlo, 0); yhi = min(yhi, a.h - 1); xhi = min(xhi, a.w - 1);
+  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int y = ylo; y <= yhi; ++y) {
+    int y0, y1;
+    float ly0, ly1;
+    src_index(a.sy, y, a.hl, y0, y1, ly0, ly1);
+    const float wy = (y0 == yi ? ly0 : 0.f) + (y1 == yi ? ly1 : 0.f);
+    if (y0 != yi && y1 != yi) continue;
+    for (int x = xlo; x <= xhi; ++x) {
+      int x0, x1;
+      float lx0, lx1;
+      src_index(a.sx, x, a.wl, x0, x1, lx0, lx1);
+      if (x0 != xi && x1 != xi) continue;
+      const float wx = (x0 == xi ? lx0 : 0.f) + (x1 == xi ? lx1 : 0.f);
+      const float wt = __fmul_rn(wy, wx);
+      const float4 g = __ldg(src + (size_t)(y * a.w + x) * FETCH_C4);
+      acc.x = fmaf(g.x, wt, acc.x); acc.y = fmaf(g.y, wt, acc.y);
+      acc.z = fmaf(g.z, wt, acc.z); acc.w = fmaf(g.w, wt, acc.w);
+    }
+  }
+  st4(a.dpyr + ((size_t)bv * a.hl * a.wl + (size_t)yi * a.wl + xi) * a.C + c4 * 4, acc);
+}
+
+int launch_warp_source_backward(const float* dsrc, const int hl[3], const int wl[3], float* const dpyr[3], int B, int V,
+                                int h, int w, cudaStream_t st) {
+  const int coff[3] = {0, 16, 48};
+  for (int l = 0; l < 3; ++l) {
+    if (dpyr[l] == nullptr) continue;
+    WarpSourceBwd a{};
+    a.dsrc = dsrc; a.dpyr = dpyr[l]; a.hl = hl[l]; a.wl = wl[l]; a.C = 16 << l; a.coff = coff[l];
+    a.h = h; a.w = w; a.V = V;
+    a.sy = (float)hl[l] / (float)h; a.sx = (float)wl[l] / (float)w;  // launch_warp_source's scales
+    const long long per_view = (long long)hl[l] * wl[l] * (a.C / 4);
+    PMVS_REQUIRE(B * V <= 65535, "warp_source_backward: B*V too large");
+    prof_begin("warp_source_bwd", st);
+    warp_source_bwd_kernel<<<dim3(cdiv(per_view, 256), B * V), 256, 0, st>>>(a);
+    PMVS_TRY(check_launch("warp_source_bwd_kernel", st));
+  }
+  return PMVS_OK;
+}
+
 }  // namespace pmvs
 
 extern "C" int pmvs_feature_fetch(const float* feature_maps, const float* pts, const float* intrinsics,

@@ -724,6 +724,14 @@ static int launch_gemm_ws_any(const GemmArgs& a, cudaStream_t st, const char* na
   return -1;
 }
 
+bool gemm_in_bn_fma_form(const GemmArgs& a) {
+  if (opt(OPT_GEMM) == 0 || pmvs_get_gemm_mode() != 3) return false;  // launch_gemm's dispatch
+  if (a.cin % 8 != 0 || a.cin > ws::MAXK || a.ldx % 4 != 0 || a.ldy % 2 != 0 || a.groups <= 0 || a.rows_per_group <= 0) return false;
+  if (((uintptr_t)a.x & 15) || ((uintptr_t)a.w & 15) || ((uintptr_t)a.y & 7)) return false;
+  if ((long long)a.groups * cdiv(a.rows_per_group, ws::NT) >= (1ll << 31) / ws::MAXK) return false;
+  return a.cout == 16 || a.cout == 32 || a.cout == 64 || a.cout == 128;
+}
+
 // returns -1 when this path does not apply (caller falls back to gemm_tc / SIMT); under PMVS_OPT_GEMM = 3 with
 // PMVS_OPT_GEMM_STRICT = 1 a launch that gemm_tma_kernel does not take is an error instead
 int launch_gemm_ws(const GemmArgs& a, cudaStream_t st, const char* name) {

@@ -19,13 +19,16 @@ _backward_enabled = False
 
 
 def enable_backward(enabled=True):
-    """Process-wide switch: while on, ``EdgeConv`` / ``EdgeConvNoC`` called with grad enabled (and a feature or
-    parameter that requires grad) run through an autograd Function whose backward is the fused CUDA backward;
-    while off (the default) such calls raise ``NotImplementedError``.  Returns the previous setting.
+    """Process-wide switch: while on, ``EdgeConv`` / ``EdgeConvNoC`` and the fused ``PointFlow`` called with grad
+    enabled (and an input or parameter that requires grad) run through autograd Functions whose backwards are the
+    fused CUDA backwards (``pmvs_edgeconv_pm_backward``, ``pmvs_point_flow_backward``); while off (the default) such
+    calls raise ``NotImplementedError``.  Returns the previous setting.
 
-    It is opt-in because a grad-enabled forward keeps the layer's [B*N, 2*out] ``LE`` activations, the neighbour
-    indices (int32 and int64), the points-major input and the fp64 batch sums alive until backward runs.  Under
-    ``torch.no_grad()`` the switch has no effect.  The fused ``PointFlow`` stays forward-only either way."""
+    It is opt-in because a grad-enabled forward keeps activations alive until backward runs: for a stand-alone layer
+    its [B*N, 2*out] ``LE``, the neighbour indices (int32 and int64), the points-major input and the fp64 batch sums;
+    for ``PointFlow`` the iteration's whole workspace (``pmvs_point_flow_workspace_bytes``).  ``PointFlow`` takes one
+    cloud per call under autograd (the train branch, or the test branch at scale 0.125).  Under ``torch.no_grad()``
+    the switch has no effect."""
     global _backward_enabled
     prev = _backward_enabled
     _backward_enabled = bool(enabled)

@@ -1,8 +1,9 @@
 """PointFlow: the ``point_flow`` closure of the reference (pointmvsnet/model.py:150-295)
 as an nn.Module, executed by libpmvs_b200.so.
 
-FORWARD ONLY (inference, as test.py runs it: under torch.no_grad() with the module in train() mode so that
-BatchNorm uses batch statistics); calling it with autograd enabled on trainable parameters raises.
+Inference runs as test.py runs it: under torch.no_grad() with the module in train() mode so that BatchNorm uses batch
+statistics.  Training (the train branch, one cloud per call) runs through an autograd Function whose backward is
+``pmvs_point_flow_backward`` once ``networks.enable_backward()`` is on; without it a grad-enabled call raises.
 
 One call = one refinement iteration = ~16 kernel launches enqueued by a single C-ABI
 call (``pmvs_point_flow_iter``); ``PointFlowPass`` runs the reference's iteration loop
@@ -16,9 +17,11 @@ import ctypes as C
 
 import torch
 import torch.nn as nn
+from torch.autograd.function import once_differentiable
 
 from . import _lib
-from ._lib import lib, check, stream_ptr, ptr, require_cuda, FlowShape, FlowWeights
+from . import networks
+from ._lib import lib, check, stream_ptr, ptr, require_cuda, FlowShape, FlowWeights, FlowGrads
 from .networks import EdgeConv, EdgeConvNoC
 from .nn.mlp import SharedMLP
 
@@ -153,6 +156,9 @@ class PointFlow(nn.Module):
             if t.dtype == torch.float32 and t.permute(0, 1, 3, 4, 2).is_contiguous():
                 res.append(t.permute(0, 1, 3, 4, 2))
                 continue
+            if torch.is_grad_enabled() and t.requires_grad:
+                res.append(_ToChannelsLast.apply(t))
+                continue
             src = _lib.f32c(t)
             dst = out[l] if out is not None else torch.empty(B, V, h, w, Cc, device=t.device, dtype=torch.float32)
             with torch.cuda.device(t.device):
@@ -211,24 +217,69 @@ class PointFlow(nn.Module):
                                       "batch-statistics BatchNorm, test.py:58); call .train() on it")
         if torch.is_grad_enabled() and (estimated_depth_map.requires_grad or
                                         any(p.requires_grad for p in self.parameters())):
-            # Forward only: the fused path has no backward, so a training loop would run and silently never
-            # update flow_edge_conv / flow_mlp.  Inference runs under torch.no_grad() (test.py:62).
-            raise NotImplementedError("pointmvsnet_b200 PointFlow is forward-only; wrap the call in torch.no_grad() "
-                                      "(training the flow modules needs the stand-alone operators)")
-        dev = estimated_depth_map.device
+            if not networks._backward_enabled:
+                # without the switch a training loop would run and silently never update flow_edge_conv / flow_mlp.
+                # Inference runs under torch.no_grad() (test.py:62).
+                raise NotImplementedError("pointmvsnet_b200 PointFlow is forward-only; wrap the call in torch.no_grad() "
+                                          "(training the flow modules needs the stand-alone operators)")
+        given = pyramids_channels_last if pyramids_channels_last is not None else (
+            [feature_pyramids[k] for k in PYR_KEYS] if isinstance(feature_pyramids, dict) else list(feature_pyramids))
+        grad_call = networks._backward_enabled and torch.is_grad_enabled() and (
+            estimated_depth_map.requires_grad or any(t.requires_grad for t in given) or
+            any(p.requires_grad for p in self.parameters()))
+        if grad_call:
+            if sub_range is not None or _ratio_for(image_scale, is_test) != 1:
+                raise NotImplementedError("PointFlow backward: one cloud per call only (the train branch, or the test "
+                                          "branch at scale 0.125); got image_scale %r, is_test %r, sub_range %r"
+                                          % (image_scale, is_test, sub_range))
+            for name, t in (("cam_params_list", cam_params_list), ("interval", interval), ("mean", mean), ("std", std)):
+                if t.requires_grad:
+                    raise RuntimeError("PointFlow backward: %s requires grad, but the fused path does not "
+                                       "differentiate it (the reference's fetch coordinates are under no_grad)" % name)
+            if out is not None:
+                raise RuntimeError("PointFlow: `out` buffers are for inference (no_grad) calls")
         if pyramids_channels_last is None:
             pyramids_channels_last = self.pyramids_to_channels_last(feature_pyramids)
-        pyr = pyramids_channels_last
+        pyr = list(pyramids_channels_last)
+        if grad_call:
+            params = self._grad_params()
+            return _PointFlowFn.apply(self, (interval, image_scale, cam_params_list, mean, std, is_test, img_hw,
+                                             interval_scale), estimated_depth_map, pyr[0], pyr[1], pyr[2], *params)
+        return self._run(estimated_depth_map, interval, image_scale, cam_params_list, mean, std, is_test, img_hw,
+                         pyr, out, interval_scale, sub_range, None)
+
+    def _grad_params(self):
+        """The 22 parameters the backward fills, in pmvs_flow_grads order."""
+        ps = []
+        for ec in self.flow_edge_conv:
+            ps += [ec.conv1.weight, ec.conv2.weight, ec.bn.weight, ec.bn.bias]
+        mlp = self.flow_mlp[0]
+        for l in range(3):
+            ps += [mlp[l].conv.weight, mlp[l].bn.weight, mlp[l].bn.bias]
+        return ps + [self.flow_mlp[1].weight]
+
+    def _run(self, estimated_depth_map, interval, image_scale, cam_params_list, mean, std, is_test, img_hw, pyr, out,
+             interval_scale, sub_range, ctx):
+        """The forward launches.  ctx None: the module's shared workspace; else (an autograd context) a workspace of
+        the call's own, kept with what the backward reads."""
+        dev = estimated_depth_map.device
         B, V = cam_params_list.shape[:2]
         pyr_hw = [(int(t.shape[2]), int(t.shape[3])) for t in pyr]
         if img_hw is None:
             img_hw = (pyr_hw[0][0] * 2, pyr_hw[0][1] * 2)  # conv1 is at half resolution (networks.py:84-124)
-        depth = _lib.f32c(estimated_depth_map)
+        depth = _lib.f32c(estimated_depth_map.detach())
+        pyr = [t.detach() for t in pyr]
         self._validate(dev, B, V, pyr, depth, interval, mean, std, cam_params_list)
         shape = self.make_shape(B, V, pyr_hw, tuple(depth.shape[2:]), img_hw, image_scale, is_test, interval_scale,
                                 sub_range)
-        ws, need = self._workspace(shape, dev)
-        w, _keep = self._weights(dev)
+        if ctx is None:
+            ws, need = self._workspace(shape, dev)
+        else:
+            need = lib.pmvs_point_flow_workspace_bytes(C.byref(shape))
+            if need == 0:
+                raise RuntimeError("libpmvs_b200: " + lib.pmvs_last_error().decode())
+            ws = torch.empty(need, device=dev, dtype=torch.uint8)
+        w, keep = self._weights(dev)
         track = self.update_running_stats and self.training
         bns = self._bn_modules()
         for l in range(3):
@@ -247,15 +298,19 @@ class PointFlow(nn.Module):
             for t, shp in ((depth_out, (B, 1, h, wd)), (prob_out, (B, 5, h, wd))):
                 if tuple(t.shape) != shp or t.dtype != torch.float32 or t.device != dev or not t.is_contiguous():
                     raise RuntimeError("PointFlow: `out` tensors must be contiguous fp32 %s on %s" % (shp, dev))
-        cams = _lib.f32c(cam_params_list)
-        itv = _lib.f32c(interval.reshape(-1))
-        mean_c, std_c = _lib.f32c(mean), _lib.f32c(std)
+        cams = _lib.f32c(cam_params_list.detach())
+        itv = _lib.f32c(interval.detach().reshape(-1))
+        mean_c, std_c = _lib.f32c(mean.detach()), _lib.f32c(std.detach())
         pyr_ptrs = (C.c_void_p * 3)(*[t.data_ptr() for t in pyr])
         with torch.cuda.device(dev):
             check(lib.pmvs_point_flow_iter(C.byref(shape), C.byref(w), C.byref(pyr_ptrs), ptr(depth), ptr(cams),
                                            ptr(itv), ptr(mean_c), ptr(std_c), ptr(depth_out), ptr(prob_out),
                                            ptr(ws), need, stream_ptr()))
         self._last = (shape, ws, depth)  # debug_stages() recomputes the point features from `depth`
+        if ctx is not None:
+            ctx.fwd_tensors = (depth, pyr[0], pyr[1], pyr[2], cams, itv, mean_c, std_c, ws)
+            # the weight struct points into `keep` (fp32 copies of the parameters), which must outlive the backward
+            ctx.fwd = (shape, w, keep, int(B), tuple(depth.shape))
         return depth_out, prob_out
 
     def _validate(self, dev, B, V, pyr, depth, interval, mean, std, cams):
@@ -403,3 +458,100 @@ class PointFlowPass(object):
     def replay(self):
         self.graph.replay()
         return self.outs
+
+
+class _ToChannelsLast(torch.autograd.Function):
+    """[B,V,C,h,w] -> [B,V,h,w,C] with pmvs_pyramid_to_channels_last; the backward is the reverse transpose."""
+
+    @staticmethod
+    def forward(ctx, t):
+        B, V, Cc, h, w = t.shape
+        ctx.dtype = t.dtype
+        src = _lib.f32c(t.detach())
+        dst = torch.empty(B, V, h, w, Cc, device=t.device, dtype=torch.float32)
+        with torch.cuda.device(t.device):
+            check(lib.pmvs_pyramid_to_channels_last(ptr(src), ptr(dst), B * V, Cc, h, w, stream_ptr()))
+        return dst
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        B, V, h, w, Cc = g.shape
+        g = _lib.f32c(g)
+        out = torch.empty(B, V, Cc, h, w, device=g.device, dtype=torch.float32)
+        with torch.cuda.device(g.device):
+            check(lib.pmvs_transpose(ptr(g), ptr(out), B * V, h * w, Cc, stream_ptr()))
+        return out.to(ctx.dtype)
+
+
+class _PointFlowFn(torch.autograd.Function):
+    """One grad-enabled PointFlow iteration.  Inputs are the depth map, the three channels-last pyramid levels and the
+    module's 22 parameters, so their .grad fill; the forward keeps its own workspace until backward."""
+
+    @staticmethod
+    def forward(ctx, mod, args, depth, pyr0, pyr1, pyr2, *params):
+        interval, image_scale, cams, mean, std, is_test, img_hw, interval_scale = args
+        ctx.dtypes = (depth.dtype,) + tuple(p.dtype for p in params)
+        res = mod._run(depth, interval, image_scale, cams, mean, std, is_test, img_hw, [pyr0, pyr1, pyr2], None,
+                       interval_scale, None, ctx)
+        # the parameters too: an in-place update before backward is then autograd's version error
+        ctx.save_for_backward(*ctx.fwd_tensors, *params)
+        del ctx.fwd_tensors
+        return res
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_depth, g_prob):
+        saved = ctx.saved_tensors
+        depth, p0, p1, p2, cams, itv, mean_c, std_c, ws = saved[:9]
+        ps = saved[9:]
+        shape, w, keep, B, dshape = ctx.fwd
+        dev = depth.device
+        need = ctx.needs_input_grad
+        gr = FlowGrads()
+        grads = [torch.empty(p.shape, device=dev, dtype=torch.float32) if p.dim() != 3 else None for p in ps]
+        dw12 = []
+        for l in range(3):
+            c = ps[4 * l].shape[0]
+            t = torch.empty(2 * c, ps[4 * l].shape[1], device=dev, dtype=torch.float32)
+            dw12.append(t)
+            gr.ec_dw12[l] = t.data_ptr()
+            gr.ec_dgamma[l] = grads[4 * l + 2].data_ptr()
+            gr.ec_dbeta[l] = grads[4 * l + 3].data_ptr()
+        mlp_w = []
+        for l in range(3):
+            t = torch.empty(ps[12 + 3 * l].shape[:2], device=dev, dtype=torch.float32)
+            mlp_w.append(t)
+            gr.mlp_dw[l] = t.data_ptr()
+            gr.mlp_dgamma[l] = grads[13 + 3 * l].data_ptr()
+            gr.mlp_dbeta[l] = grads[14 + 3 * l].data_ptr()
+        w3 = torch.empty(ps[21].shape[:2], device=dev, dtype=torch.float32)
+        mlp_w.append(w3)
+        gr.mlp_dw[3] = w3.data_ptr()
+        dpyr = [torch.empty(p.shape, device=dev, dtype=torch.float32) if need[3 + l] else None
+                for l, p in enumerate((p0, p1, p2))]
+        for l in range(3):
+            gr.dpyramids_cl[l] = ptr(dpyr[l])
+        ddepth = torch.empty(dshape, device=dev, dtype=torch.float32) if need[2] else None
+        gr.ddepth_prev = ptr(ddepth)
+        gd = _lib.f32c(g_depth) if g_depth is not None else torch.zeros(B, 1, shape.flow_h, shape.flow_w, device=dev)
+        gp = _lib.f32c(g_prob) if g_prob is not None else None
+        nbytes = lib.pmvs_point_flow_backward_workspace_bytes(C.byref(shape))
+        if nbytes == 0:
+            raise RuntimeError("libpmvs_b200: " + lib.pmvs_last_error().decode())
+        bws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+        pyr_ptrs = (C.c_void_p * 3)(p0.data_ptr(), p1.data_ptr(), p2.data_ptr())
+        with torch.cuda.device(dev):
+            check(lib.pmvs_point_flow_backward(C.byref(shape), C.byref(w), C.byref(pyr_ptrs), ptr(depth), ptr(cams),
+                                               ptr(itv), ptr(mean_c), ptr(std_c), ptr(ws), ptr(gd), ptr(gp),
+                                               C.byref(gr), ptr(bws), nbytes, stream_ptr()))
+        out = []
+        for l in range(3):
+            c = ps[4 * l].shape[0]
+            out += [dw12[l][:c].unsqueeze(-1), dw12[l][c:].unsqueeze(-1), grads[4 * l + 2], grads[4 * l + 3]]
+        for l in range(3):
+            out += [mlp_w[l].unsqueeze(-1), grads[13 + 3 * l], grads[14 + 3 * l]]
+        out.append(w3.unsqueeze(-1))
+        out = [g.to(dt) if n else None for g, dt, n in zip(out, ctx.dtypes[1:], need[6:])]
+        dd = ddepth.to(ctx.dtypes[0]) if ddepth is not None else None
+        return (None, None, dd) + tuple(dpyr) + tuple(out)
