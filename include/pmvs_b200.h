@@ -141,6 +141,19 @@ int pmvs_cost_volume(const float* features, const float* cam_params, float* cost
                      size_t workspace_bytes, int B, int V, int C, int h, int w, int D, int is_test,
                      pmvs_stream_t stream);
 
+/* Backward of pmvs_cost_volume with respect to the features (the cameras get no gradient: the reference computes the
+ * fetch coordinates under no_grad, feature_fetcher.py:29).  grad_cost [B,C,D,h,w] -> grad_features [B,V,C,h,w], every
+ * element written.  View 0 gets sum_d g 2 (f_0 - mean) / V (its un-warped feature; its fetched samples are overwritten
+ * in the forward and get nothing); view v >= 1 gets, per texel, the bilinear-weighted sum of g 2 (f_v - mean) / V over
+ * the plane points whose unmasked taps hit it.  The taps are the forward's, bit for bit.  Deterministic: no
+ * floating-point atomics, every sum in an order fixed by the shapes.  No allocation, no synchronisation.  Limits: those
+ * of pmvs_cost_volume and (V-1)*4*D*h*w < 2^31.  workspace: pmvs_cost_volume_backward_workspace_bytes(...) bytes,
+ * 256-byte aligned, device memory. */
+size_t pmvs_cost_volume_backward_workspace_bytes(int B, int V, int C, int h, int w, int D); /* 0 + pmvs_last_error on a bad shape */
+int pmvs_cost_volume_backward(const float* features, const float* cam_params, const float* grad_cost,
+                              float* grad_features, void* workspace, size_t workspace_bytes, int B, int V, int C,
+                              int h, int w, int D, int is_test, pmvs_stream_t stream);
+
 /* ---- layout helpers used by the module-level API --------------------------------- */
 /* batched 2-D transpose: in [batch, R, C] -> out [batch, C, R] */
 int pmvs_transpose(const float* in, float* out, int batch, int R, int C, pmvs_stream_t stream);

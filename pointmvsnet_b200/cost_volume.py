@@ -8,20 +8,59 @@ import torch
 from ._lib import lib, check, stream_ptr, ptr, require_cuda, f32c
 
 
-def build_cost_volume(feature_list, cam_params_list, is_test=True):
-    """feature_list [B,V,C,h,w] (coarse_img_conv "conv3" of every view, reference view first),
-    cam_params_list [B,V,2,4,4] at full image resolution -> cost_volume [B,C,D,h,w]
-    (model.py:113) with D = cam_params_list[0,0,1,3,2]."""
-    require_cuda(feature_list, cam_params_list)
-    if feature_list.dim() != 5 or cam_params_list.dim() != 5:
-        raise RuntimeError("build_cost_volume: feature_list [B,V,C,h,w], cam_params_list [B,V,2,4,4]")
-    feats = f32c(feature_list)
-    cams = f32c(cam_params_list)
+def _forward(feats, cams, D, is_test):
     B, V, Cc, h, w = feats.shape
-    D = int(cams[0, 0, 1, 3, 2].item())  # model.py:65 (the reference syncs here too)
     cost = torch.empty(B, Cc, D, h, w, device=feats.device, dtype=torch.float32)
     ws = torch.empty(B * (28 + 24 * V), device=feats.device, dtype=torch.float32)
     with torch.cuda.device(feats.device):
         check(lib.pmvs_cost_volume(ptr(feats), ptr(cams), ptr(cost), ptr(ws), ws.numel() * 4, B, V, Cc, h, w, D,
                                    1 if is_test else 0, stream_ptr()))
     return cost
+
+
+class _CostVolumeFn(torch.autograd.Function):
+    """build_cost_volume under autograd: the backward is pmvs_cost_volume_backward (deterministic, no atomics).
+    It keeps only its inputs: the contiguous fp32 features the forward read and the cameras."""
+
+    @staticmethod
+    def forward(ctx, feats, cams, D, is_test):
+        ctx.save_for_backward(feats, cams)
+        ctx.D, ctx.is_test = D, is_test
+        return _forward(feats, cams, D, is_test)
+
+    @staticmethod
+    def backward(ctx, grad_cost):
+        feats, cams = ctx.saved_tensors
+        B, V, Cc, h, w = feats.shape
+        g = f32c(grad_cost)
+        grad = torch.empty_like(feats)
+        nbytes = int(lib.pmvs_cost_volume_backward_workspace_bytes(B, V, Cc, h, w, ctx.D))
+        if nbytes == 0:
+            check(1)
+        ws = torch.empty(nbytes, device=feats.device, dtype=torch.uint8)  # the caching allocator aligns to 512 bytes
+        with torch.cuda.device(feats.device):
+            check(lib.pmvs_cost_volume_backward(ptr(feats), ptr(cams), ptr(g), ptr(grad), ptr(ws), nbytes, B, V, Cc,
+                                                h, w, ctx.D, 1 if ctx.is_test else 0, stream_ptr()))
+        return grad, None, None, None
+
+
+def build_cost_volume(feature_list, cam_params_list, is_test=True):
+    """feature_list [B,V,C,h,w] (coarse_img_conv "conv3" of every view, reference view first),
+    cam_params_list [B,V,2,4,4] at full image resolution -> cost_volume [B,C,D,h,w]
+    (model.py:113) with D = cam_params_list[0,0,1,3,2].
+
+    Differentiable in ``feature_list``: with grad enabled and ``feature_list`` requiring grad, the result has a
+    ``grad_fn`` whose backward is the fused, deterministic pmvs_cost_volume_backward.  No opt-in switch is needed
+    (unlike ``networks.enable_backward()`` for EdgeConv / PointFlow, which keep activations alive): the graph holds
+    nothing beyond the inputs.  ``cam_params_list`` gets no gradient - the reference computes the fetch coordinates
+    under no_grad (feature_fetcher.py:29).  Under no_grad, or for inputs that do not require grad, the call is the
+    plain forward."""
+    require_cuda(feature_list, cam_params_list)
+    if feature_list.dim() != 5 or cam_params_list.dim() != 5:
+        raise RuntimeError("build_cost_volume: feature_list [B,V,C,h,w], cam_params_list [B,V,2,4,4]")
+    feats = f32c(feature_list)
+    cams = f32c(cam_params_list)
+    D = int(cams[0, 0, 1, 3, 2].item())  # model.py:65 (the reference syncs here too)
+    if torch.is_grad_enabled() and feature_list.requires_grad:
+        return _CostVolumeFn.apply(feats, cams.detach(), D, bool(is_test))
+    return _forward(feats, cams, D, is_test)

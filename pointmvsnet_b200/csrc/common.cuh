@@ -180,6 +180,11 @@ int launch_edge_apply(const EdgeArgs& a, cudaStream_t st);
 size_t inv_lists_bytes(long long B, long long N, long long K);
 int build_inv_lists(const int64_t* idx, int B, int N, int K, void* ws, const int** off, const int** list,
                     const char* prof_name, cudaStream_t st);
+// Per-texel sums of tap records (gather_det.cu), in list order: texel t of batch element b gets
+// out[b*out_bstride + t*out_tstride + c] = sum over records p of texel t of rec_w[b][p] * g[b][p/4][c], c < C (C % 4 == 0).
+// off / list: build_inv_lists over the B x nrec record texels with K = 4 (source rows nrec/4 >= T).
+int launch_texel_sum(const int* off, const int* list, const float* rec_w, const float* g, float* out, int T, int nrec,
+                     int B, int C, long long out_bstride, int out_tstride, const char* prof_name, cudaStream_t st);
 
 // One EdgeConv / EdgeConvNoC layer's backward (edge_bwd.cu), batch-statistic or frozen BatchNorm, for B clouds of N
 // points in one BatchNorm group: dgamma, dbeta, dLE (into `dle`, [B*N, 2*cout]), dX (if dx != NULL) and dW12.  The
@@ -260,6 +265,8 @@ int launch_fused_fetch(const FusedFetchParams& p, cudaStream_t st);
 // Returns -1 when it does not take the call (5 V > 30, or the shared memory cannot be had)
 int launch_fetch_gemm(const FusedFetchParams& p, const float* w12, float* le, cudaStream_t st);
 size_t cam_block_bytes(int B, int V);
+// the shape limits of pmvs_cost_volume (C % 16, V <= PMVS_MAX_VIEWS, D*h*w < 2^31, B <= 65535), messages prefixed `what`
+int cost_volume_check_shape(const char* what, int B, int V, int C, int h, int w, int D);
 // Backward of the fetch (fetch.cu) for S = 1, ratio 1: from dF0 [B*N, 136] (rows in fetch order) and the depth
 // gradient of the output map, ddup [B,h,w] = d depth_up (the skip plus the xyz columns through the hypothesis depths);
 // with dfv != NULL also the variance columns' gradient per (pixel, hypothesis, view) dfv [B*h*w*5*V, 112] and its tap

@@ -14,22 +14,10 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "projection.cuh"
 #include "wgmma.cuh"
 
 namespace pmvs {
-
-// ---------------------------------------------------------------------------------------
-// camera block, one per batch element (floats)
-// ---------------------------------------------------------------------------------------
-constexpr int CB_KINV = 0;    // inverse of the scaled reference intrinsics, 3x3 row-major
-constexpr int CB_R0INV = 9;   // inverse reference rotation
-constexpr int CB_T0 = 18;     // reference translation
-constexpr int CB_MEAN = 21;
-constexpr int CB_STD = 24;
-constexpr int CB_INTERVAL = 27;
-constexpr int CB_VIEW = 28;   // per view: R[9], t[3], K[9] (scaled), pad[3]
-constexpr int CB_VSTRIDE = 24;
-__host__ __device__ constexpr int cam_block_floats(int V) { return CB_VIEW + CB_VSTRIDE * V; }
 
 __device__ void inv3x3(const double* m, double* o) {
   const double a = m[0], b = m[1], c = m[2], d = m[3], e = m[4], f = m[5], g = m[6], h = m[7], i = m[8];
@@ -94,60 +82,8 @@ __global__ void cam_setup_kernel(const float* __restrict__ cam_params, const flo
 }
 
 // ---------------------------------------------------------------------------------------
-// shared projection math (feature_fetcher.py:36-53 + grid_sample's un-normalisation)
+// (1) stand-alone FeatureFetcher (projection arithmetic: projection.cuh)
 // ---------------------------------------------------------------------------------------
-__device__ __forceinline__ float dot3(const float* r, float x, float y, float z) {
-  return fmaf(r[2], z, fmaf(r[1], y, __fmul_rn(r[0], x)));
-}
-
-// pixel coordinate in the sampled map (align_corners=True round trip, feature_fetcher.py:51-53
-// then ATen grid_sampler_unnormalize): ((g + 1) / 2) * (size - 1), g = (u - .5)/(size-1)*2 - 1
-__device__ __forceinline__ float grid_coord(float u, int size) {
-  const float sm1 = (float)(size - 1);
-  const float g = __fsub_rn(__fmul_rn(__fdiv_rn(__fsub_rn(u, 0.5f), sm1), 2.f), 1.f);
-  return __fmul_rn(__fmul_rn(__fadd_rn(g, 1.f), 0.5f), sm1);  // x / 2 == x * 0.5 exactly
-}
-
-__device__ __forceinline__ void project(const float* R, const float* t, const float* K, float wx, float wy, float wz,
-                                        float& u, float& v) {
-  float xc = wx, yc = wy, zc = wz;
-  if (R != nullptr) {
-    xc = __fadd_rn(dot3(R + 0, wx, wy, wz), t[0]);
-    yc = __fadd_rn(dot3(R + 3, wx, wy, wz), t[1]);
-    zc = __fadd_rn(dot3(R + 6, wx, wy, wz), t[2]);
-  }
-  const float nx = __fdiv_rn(xc, zc), ny = __fdiv_rn(yc, zc);
-  u = dot3(K + 0, nx, ny, 1.f);
-  v = dot3(K + 3, nx, ny, 1.f);
-}
-
-__device__ __forceinline__ bool usable(float c) { return fabsf(c) < 1.0e8f; }  // false for NaN/inf
-
-// ---------------------------------------------------------------------------------------
-// (1) stand-alone FeatureFetcher
-// ---------------------------------------------------------------------------------------
-struct Taps {
-  int x0, y0;
-  float nw, ne, sw, se;
-  bool ok_w, ok_e, ok_n, ok_s;
-};
-__device__ __forceinline__ Taps make_taps(float ix, float iy, int W, int H) {
-  Taps t;
-  const float fx = floorf(ix), fy = floorf(iy);
-  t.x0 = (int)fx;
-  t.y0 = (int)fy;
-  const float ex = fx + 1.f, ey = fy + 1.f;
-  t.nw = __fmul_rn(__fsub_rn(ex, ix), __fsub_rn(ey, iy));
-  t.ne = __fmul_rn(__fsub_rn(ix, fx), __fsub_rn(ey, iy));
-  t.sw = __fmul_rn(__fsub_rn(ex, ix), __fsub_rn(iy, fy));
-  t.se = __fmul_rn(__fsub_rn(ix, fx), __fsub_rn(iy, fy));
-  t.ok_w = t.x0 >= 0 && t.x0 < W;
-  t.ok_e = t.x0 + 1 >= 0 && t.x0 + 1 < W;
-  t.ok_n = t.y0 >= 0 && t.y0 < H;
-  t.ok_s = t.y0 + 1 >= 0 && t.y0 + 1 < H;
-  return t;
-}
-
 template <bool BACKWARD>
 __global__ void __launch_bounds__(256)
     feature_fetch_kernel(const float* __restrict__ maps, const float* __restrict__ pts, const float* __restrict__ Kmat,
@@ -752,11 +688,11 @@ __global__ void __launch_bounds__(fg::THREADS, 1)
 // ---------------------------------------------------------------------------------------
 // (3) coarse-stage plane sweep: fetch + variance -> cost volume  (reference model.py:81-113)
 // ---------------------------------------------------------------------------------------
-// One thread per hypothesis point (d, y, x); channels in chunks of 16 so that sum / sum of squares
+// One thread per hypothesis point (d, y, x); channels in chunks of CV_CH so that sum / sum of squares
 // stay in registers; the source-view projection is recomputed per chunk (cheap next to 64 taps).
 // The reference view contributes its un-warped feature (model.py:103-106).  NCHW reads and the
-// [B,C,D,h,w] writes are coalesced across x.
-constexpr int CV_CH = 16;
+// [B,C,D,h,w] writes are coalesced across x.  The plane point and the taps come from projection.cuh,
+// which the backward (cost_volume_bwd.cu) shares.
 __global__ void __launch_bounds__(256)
     cost_volume_kernel(const float* __restrict__ feat, const float* __restrict__ cam_params,
                        const float* __restrict__ cam_blocks, float* __restrict__ cost, int V, int C, int h, int w,
@@ -770,21 +706,8 @@ __global__ void __launch_bounds__(256)
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= D * hw) return;
   const int d = p / hw, pix = p - d * hw;
-  const int y = pix / w, x = pix - y * w;
-  // depth hypotheses: torch.linspace(depth_start, depth_end, D) (model.py:81-85; ATen's symmetric rule)
-  const float* cp = cam_params + ((size_t)(b * V) * 2 + 1) * 16 + 12;
-  const float dstart = cp[0], dint = cp[1];
-  const float dend = __fadd_rn(dstart, __fmul_rn((float)(D - 1), dint));  // model.py:67
-  const float step = D > 1 ? __fdiv_rn(__fsub_rn(dend, dstart), (float)(D - 1)) : 0.f;
-  const float depth = d < D / 2 ? __fadd_rn(dstart, __fmul_rn(step, (float)d))
-                                : __fsub_rn(dend, __fmul_rn(step, (float)(D - 1 - d)));
-  const float px = (float)x + 0.5f, py = (float)y + 0.5f;
-  const float cx = __fsub_rn(__fmul_rn(dot3(cam + CB_KINV + 0, px, py, 1.f), depth), cam[CB_T0 + 0]);
-  const float cy = __fsub_rn(__fmul_rn(dot3(cam + CB_KINV + 3, px, py, 1.f), depth), cam[CB_T0 + 1]);
-  const float cz = __fsub_rn(__fmul_rn(dot3(cam + CB_KINV + 6, px, py, 1.f), depth), cam[CB_T0 + 2]);
-  const float wx = dot3(cam + CB_R0INV + 0, cx, cy, cz);
-  const float wy = dot3(cam + CB_R0INV + 3, cx, cy, cz);
-  const float wz = dot3(cam + CB_R0INV + 6, cx, cy, cz);
+  float wx, wy, wz;
+  cv_world_point(cam, cam_params, b, V, D, h, w, p, wx, wy, wz);
   const float fV = (float)V;
   const size_t plane = (size_t)hw;
   for (int c0 = 0; c0 < C; c0 += CV_CH) {
@@ -797,12 +720,7 @@ __global__ void __launch_bounds__(256)
       s2[c] = __fmul_rn(f0, f0);
     }
     for (int v = 1; v < V; ++v) {
-      const float* cv = cam + CB_VIEW + v * CB_VSTRIDE;
-      float u, vv;
-      project(cv, cv + 9, cv + 12, wx, wy, wz, u, vv);
-      const float ix = grid_coord(u, w), iy = grid_coord(vv, h);
-      const bool ok = usable(ix) && usable(iy);
-      const Taps tp = make_taps(ok ? ix : -10.f, ok ? iy : -10.f, w, h);
+      const Taps tp = cv_view_taps(cam + CB_VIEW + v * CB_VSTRIDE, wx, wy, wz, w, h);
       const float* m = feat + ((size_t)(b * V + v) * C + c0) * plane + (size_t)tp.y0 * w + tp.x0;
 #pragma unroll
       for (int c = 0; c < CV_CH; ++c) {
@@ -905,6 +823,13 @@ int launch_fetch_gemm(const FusedFetchParams& p0, const float* w12, float* le, c
 }
 
 size_t cam_block_bytes(int B, int V) { return (size_t)B * cam_block_floats(V) * sizeof(float); }
+
+int cost_volume_check_shape(const char* what, int B, int V, int C, int h, int w, int D) {
+  PMVS_REQUIRE(B > 0 && B <= 65535 && V > 0 && V <= PMVS_MAX_VIEWS && h > 1 && w > 1 && D > 0, "%s: bad shape", what);
+  PMVS_REQUIRE(C > 0 && C % CV_CH == 0, "%s: channels must be a multiple of %d", what, CV_CH);
+  PMVS_REQUIRE((long long)D * h * w < (1ll << 31), "%s: volume too large", what);
+  return PMVS_OK;
+}
 
 // ---------------------------------------------------------------------------------------
 // backward of rows a2-a9 (PointFlow backward, S = 1): one warp per pixel recomputes the forward's descriptors
@@ -1124,9 +1049,7 @@ extern "C" int pmvs_cost_volume(const float* features, const float* cam_params, 
                                 pmvs_stream_t stream) {
   using namespace pmvs;
   PMVS_REQUIRE(features && cam_params && cost && workspace, "cost_volume: NULL pointer");
-  PMVS_REQUIRE(B > 0 && B <= 65535 && V > 0 && V <= PMVS_MAX_VIEWS && h > 1 && w > 1 && D > 0, "cost_volume: bad shape");
-  PMVS_REQUIRE(C > 0 && C % CV_CH == 0, "cost_volume: channels must be a multiple of %d", CV_CH);
-  PMVS_REQUIRE((long long)D * h * w < (1ll << 31), "cost_volume: volume too large");
+  PMVS_TRY(cost_volume_check_shape("cost_volume", B, V, C, h, w, D));
   if (workspace_bytes < cam_block_bytes(B, V)) {
     set_error("cost_volume: workspace %zu bytes < required %zu", workspace_bytes, cam_block_bytes(B, V));
     return PMVS_ERR_WORKSPACE;

@@ -259,32 +259,6 @@ __global__ void __launch_bounds__(256) add_cols_kernel(float* __restrict__ y, in
   st4(yp, make_float4(__fadd_rn(o.x, v.x), __fadd_rn(o.y, v.y), __fadd_rn(o.z, v.z), __fadd_rn(o.w, v.w)));
 }
 
-// d warp source texel t of batch element b = sum over its tap records p (ascending) of w[p] * dfv[p / 4]; one warp per
-// texel, lanes 0..27 a float4 of the 112 channels
-__global__ void __launch_bounds__(256) texel_sum_kernel(const int* __restrict__ off, const int* __restrict__ list,
-                                                        const float* __restrict__ rec_w, const float* __restrict__ dfv,
-                                                        float* __restrict__ dsrc, int T, int nrec, int B) {
-  const long long wi = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (wi >= (long long)B * T || lane >= 28) return;
-  const int b = (int)(wi / T), t = (int)(wi - (long long)b * T);
-  const int nsrc = nrec / 4;  // (pixel, hypothesis, view) entries of a batch element
-  const int* o = off + (size_t)b * (nsrc + 1);
-  const int* lst = list + (size_t)b * nrec;
-  const float* wb = rec_w + (size_t)b * nrec;
-  const float* fb = dfv + (size_t)b * nsrc * 112;
-  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-  for (int q = o[t]; q < o[t + 1]; ++q) {
-    const int p = __ldg(lst + q);
-    const float wt = __ldg(wb + p);
-    const float4 g = ldg4(fb + (size_t)(p >> 2) * 112 + lane * 4);
-    acc.x = fmaf(g.x, wt, acc.x); acc.y = fmaf(g.y, wt, acc.y);
-    acc.z = fmaf(g.z, wt, acc.z); acc.w = fmaf(g.w, wt, acc.w);
-  }
-  // [B][V*h*w + 1][112]: the layout of the forward's warp source
-  st4(dsrc + ((size_t)b * (T + 1) + t) * 112 + lane * 4, acc);
-}
-
 // transpose of the nearest resize (model.py:153-158, flow_head_kernel / fetch_describe's index rule): previous pixel
 // (yp, xp) gathers the flow pixels Y, X with min(floor(Y * hp / h), hp - 1) == yp (and likewise in x), rows then
 // columns ascending
@@ -610,10 +584,9 @@ extern "C" int pmvs_point_flow_backward(const pmvs_flow_shape* shape, const pmvs
     const int* rlist = nullptr;
     PMVS_TRY(build_inv_lists((const int64_t*)(ws + p.rec_idx), B, nrec / 4, 4, ws + p.rec_inv, &roff, &rlist,
                              "flow_bwd_tap_lists", st));
-    prof_begin("texel_sum", st);
-    texel_sum_kernel<<<cdiv((long long)B * T * 32, 256), 256, 0, st>>>(roff, rlist, F(p.rec_w), F(p.dfv), F(p.dsrc), T,
-                                                                      nrec, B);
-    PMVS_TRY(check_launch("texel_sum_kernel", st));
+    // d warp source [B][V*h*w + 1][112]: the layout of the forward's warp source
+    PMVS_TRY(launch_texel_sum(roff, rlist, F(p.rec_w), F(p.dfv), F(p.dsrc), T, nrec, B, 112, (long long)(T + 1) * 112,
+                              112, "texel_sum", st));
     PMVS_TRY(launch_warp_source_backward(F(p.dsrc), shape->pyr_h, shape->pyr_w, grads->dpyramids_cl, B, shape->V, h,
                                          w, st));
   }

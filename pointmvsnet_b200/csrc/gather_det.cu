@@ -198,6 +198,46 @@ int build_inv_lists(const int64_t* idx, int B, int N, int K, void* workspace, co
   return PMVS_OK;
 }
 
+// Per-texel sums of tap records (the deterministic transpose of a bilinear fetch): texel t of batch element b gets
+//   out[b * out_bstride + t * out_tstride + c] = sum over its records p (list order, ascending) of w[p] * g[p / 4][c]
+// with `off` / `list` from build_inv_lists over the records (4 taps per source row), rec_w [B][nrec] and g [B][nrec/4][C]
+// channel-contiguous.  One warp per texel, each lane a float4 of the C channels.
+__global__ void __launch_bounds__(256) texel_sum_kernel(const int* __restrict__ off, const int* __restrict__ list,
+                                                        const float* __restrict__ rec_w, const float* __restrict__ g,
+                                                        float* __restrict__ out, int T, int nrec, int B, int C,
+                                                        long long out_bstride, int out_tstride) {
+  const long long wi = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (wi >= (long long)B * T) return;
+  const int b = (int)(wi / T), t = (int)(wi - (long long)b * T);
+  const int nsrc = nrec / 4;  // source rows of a batch element
+  const int* o = off + (size_t)b * (nsrc + 1);
+  const int* lst = list + (size_t)b * nrec;
+  const float* wb = rec_w + (size_t)b * nrec;
+  const float* gb = g + (size_t)b * nsrc * C;
+  for (int c4 = lane; c4 < C / 4; c4 += 32) {
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int q = o[t]; q < o[t + 1]; ++q) {
+      const int p = __ldg(lst + q);
+      const float wt = __ldg(wb + p);
+      const float4 v = ldg4(gb + (size_t)(p >> 2) * C + c4 * 4);
+      acc.x = fmaf(v.x, wt, acc.x); acc.y = fmaf(v.y, wt, acc.y);
+      acc.z = fmaf(v.z, wt, acc.z); acc.w = fmaf(v.w, wt, acc.w);
+    }
+    st4(out + b * out_bstride + (size_t)t * out_tstride + c4 * 4, acc);
+  }
+}
+
+int launch_texel_sum(const int* off, const int* list, const float* rec_w, const float* g, float* out, int T, int nrec,
+                     int B, int C, long long out_bstride, int out_tstride, const char* prof_name, cudaStream_t st) {
+  PMVS_REQUIRE(C > 0 && C % 4 == 0 && nrec % 4 == 0, "texel_sum: C and nrec must be multiples of 4");
+  if ((long long)B * T == 0) return PMVS_OK;
+  prof_begin(prof_name, st);
+  texel_sum_kernel<<<cdiv((long long)B * T * 32, 256), 256, 0, st>>>(off, list, rec_w, g, out, T, nrec, B, C,
+                                                                      out_bstride, out_tstride);
+  return check_launch("texel_sum_kernel", st);
+}
+
 }  // namespace pmvs
 
 using namespace pmvs;
