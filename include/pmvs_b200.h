@@ -129,6 +129,25 @@ int pmvs_feature_fetch(const float* feature_maps, const float* pts, const float*
 int pmvs_feature_fetch_backward(const float* grad_out, const float* pts, const float* intrinsics,
                                 const float* extrinsics, float* grad_maps, int B, int V, int C,
                                 int H, int W, int N, pmvs_stream_t stream);
+/* The same gradient with a FIXED summation order (FeatureFetcher's backward under
+ * torch.use_deterministic_algorithms(True)).  Every unmasked tap of every point is a record (texel, weight w), zero
+ * weights included; grad_maps[b,v,c,t] (every element written) is the fp32 sum, starting from 0, of the rounded products
+ * fl(w * grad_out[b,v,c,n]) of the records that hit texel t, added one rounding at a time in ascending (n, tap) order,
+ * taps in the order nw, ne, sw, se.  That is exactly what a sequential CPU loop over the records in that order computes,
+ * and the same products the atomic entry adds in an arbitrary order.  The taps are the forward's, bit for bit.  The
+ * result depends only on the (b, v)'s own inputs, not on B, V, the layouts of other views or the launch geometry.  No
+ * allocation, no synchronisation.  Limits: those of pmvs_feature_fetch (H, W > 1, B*V <= 65535) and
+ * 4*max(N, H*W) < 2^31.  workspace: pmvs_feature_fetch_backward_det_workspace_bytes(...) bytes, 256-byte aligned, device
+ * memory. */
+size_t pmvs_feature_fetch_backward_det_workspace_bytes(int B, int V, int C, int H, int W, int N); /* 0 + pmvs_last_error on a bad shape */
+int pmvs_feature_fetch_backward_det(const float* grad_out, const float* pts, const float* intrinsics,
+                                    const float* extrinsics, float* grad_maps, int B, int V, int C, int H, int W, int N,
+                                    void* workspace, size_t workspace_bytes, pmvs_stream_t stream);
+/* The forward's taps as records: texel [B,V,N,4] int64 (y*W + x of the nw, ne, sw, se tap, -1 where the tap is masked:
+ * outside the map, or a non-finite projection) and weight [B,V,N,4] (the bilinear weights, also where masked).  The
+ * records pmvs_feature_fetch_backward_det sums over. */
+int pmvs_feature_fetch_taps(const float* pts, const float* intrinsics, const float* extrinsics, int64_t* texel,
+                            float* weight, int B, int V, int H, int W, int N, pmvs_stream_t stream);
 
 /* ---- (next row, SURVEY 8f-1) coarse-stage plane sweep: fetch + variance  (model.py:54-113) ------ */
 /* features [B,V,C,h,w] (coarse_img_conv conv3 per view, view 0 = reference), cam_params

@@ -75,6 +75,9 @@ _sig("pmvs_gather_knn_backward_det", I, [P, P, P, I, I, I, I, P, C.c_size_t, P])
 _sig("pmvs_knn3d", I, [P, P, P, I, I, I, I, I, I, P])
 _sig("pmvs_feature_fetch", I, [P, P, P, P, P, I, I, I, I, I, I, P])
 _sig("pmvs_feature_fetch_backward", I, [P, P, P, P, P, I, I, I, I, I, I, P])
+_sig("pmvs_feature_fetch_backward_det_workspace_bytes", C.c_size_t, [I, I, I, I, I, I])
+_sig("pmvs_feature_fetch_backward_det", I, [P, P, P, P, P, I, I, I, I, I, I, P, C.c_size_t, P])
+_sig("pmvs_feature_fetch_taps", I, [P, P, P, P, P, I, I, I, I, I, P])
 _sig("pmvs_cost_volume", I, [P, P, P, P, C.c_size_t, I, I, I, I, I, I, I, P])
 _sig("pmvs_cost_volume_backward_workspace_bytes", C.c_size_t, [I, I, I, I, I, I])
 _sig("pmvs_cost_volume_backward", I, [P, P, P, P, P, C.c_size_t, I, I, I, I, I, I, I, P])
@@ -98,6 +101,7 @@ _sig("pmvs_point_flow_backward", I, [C.POINTER(FlowShape), C.POINTER(FlowWeights
 EXPORTED = [
     "pmvs_version", "pmvs_last_error", "pmvs_launch_count", "pmvs_set_option", "pmvs_get_option", "pmvs_profile_enable", "pmvs_profile_collect", "pmvs_set_gemm_mode", "pmvs_get_gemm_mode", "pmvs_gather_knn_forward",
     "pmvs_gather_knn_backward", "pmvs_gather_knn_backward_det_workspace_bytes", "pmvs_gather_knn_backward_det", "pmvs_knn3d", "pmvs_feature_fetch", "pmvs_feature_fetch_backward",
+    "pmvs_feature_fetch_backward_det_workspace_bytes", "pmvs_feature_fetch_backward_det", "pmvs_feature_fetch_taps",
     "pmvs_cost_volume", "pmvs_cost_volume_backward_workspace_bytes", "pmvs_cost_volume_backward", "pmvs_transpose", "pmvs_idx64_to_idx32", "pmvs_edgeconv_pm", "pmvs_edgeconv_pm_backward_workspace_bytes", "pmvs_edgeconv_pm_backward", "pmvs_linear_pm", "pmvs_point_flow_workspace_bytes",
     "pmvs_point_flow_iter", "pmvs_pyramid_to_channels_last", "pmvs_point_flow_debug_offsets",
     "pmvs_point_flow_debug_feature", "pmvs_point_flow_backward_workspace_bytes", "pmvs_point_flow_backward",

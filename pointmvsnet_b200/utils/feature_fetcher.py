@@ -1,5 +1,7 @@
 """FeatureFetcher: differentiable homography warp + bilinear multi-view fetch
-(reference utils/feature_fetcher.py:8-60), one sm_90a kernel per direction."""
+(reference utils/feature_fetcher.py:8-60), one sm_90a kernel per direction.  Under
+torch.use_deterministic_algorithms(True) (warn_only included), checked when the backward runs, the gradient of the maps
+is summed in a fixed order (pmvs_feature_fetch_backward_det) instead of by the atomicAdd scatter."""
 import torch
 import torch.nn as nn
 
@@ -28,10 +30,21 @@ class _Fetch(torch.autograd.Function):
         p, K, E = ctx.saved_tensors
         B, V, Cc, H, W, N = ctx.shape
         g = f32c(grad_out)
+        E = E if ctx.has_ext else None
         grad_maps = torch.empty(B, V, Cc, H, W, device=g.device, dtype=torch.float32)
+        if torch.are_deterministic_algorithms_enabled():
+            # fixed summation order (pmvs_feature_fetch_backward_det) in place of the atomicAdd scatter
+            nbytes = int(lib.pmvs_feature_fetch_backward_det_workspace_bytes(B, V, Cc, H, W, N))
+            if nbytes == 0:
+                check(1)
+            ws = torch.empty(nbytes, device=g.device, dtype=torch.uint8)  # the caching allocator aligns to 512 bytes
+            with torch.cuda.device(g.device):
+                check(lib.pmvs_feature_fetch_backward_det(ptr(g), ptr(p), ptr(K), ptr(E), ptr(grad_maps), B, V, Cc, H,
+                                                          W, N, ptr(ws), nbytes, stream_ptr()))
+            return grad_maps, None, None, None
         with torch.cuda.device(g.device):
-            check(lib.pmvs_feature_fetch_backward(ptr(g), ptr(p), ptr(K), ptr(E) if ctx.has_ext else None,
-                                                  ptr(grad_maps), B, V, Cc, H, W, N, stream_ptr()))
+            check(lib.pmvs_feature_fetch_backward(ptr(g), ptr(p), ptr(K), ptr(E), ptr(grad_maps), B, V, Cc, H, W, N,
+                                                  stream_ptr()))
         return grad_maps, None, None, None
 
 
