@@ -173,6 +173,27 @@ int pmvs_cost_volume_backward(const float* features, const float* cam_params, co
                               float* grad_features, void* workspace, size_t workspace_bytes, int B, int V, int C,
                               int h, int w, int D, int is_test, pmvs_stream_t stream);
 
+/* ---- depth-map fusion (the step the reference hands to the external fusibile binary, tools/depthfusion.py:173-192) */
+/* A fusibile-style fusion with this library's own rule (DESIGN 3.10); not bit-compatible with fusibile, and no normal
+ * test.  depth [V,H,W]: a pixel is valid iff 0 < d <= FLT_MAX.  cam_block [V,40] (host-built by
+ * utils/depthfusion.py:fusion_camera_block): Kinv[9], Rinv[9], t[3], R[9], K[9], pad, fp32, K at the depth maps'
+ * resolution.  Reference views r are taken in ascending order; a valid pixel of r that no accepted point has claimed
+ * (used[r,y,x] == 0 at r's turn) is checked against every other view j in ascending order: back-project at the pixel
+ * centre, project into j, read depth[j] at the floored position, back-project that pixel centre, project into r; j is
+ * consistent when both projections are in front of their camera, the round trip lands within reproj_thresh pixels and
+ * the depths agree within depth_thresh * depth[j].  count_out[r,y,x] = the number of consistent views (-1 where the
+ * pixel is not processed); xyz_out[r,y,x] = (X + sum_j Y_j) / (count + 1), summed in ascending j (0 where count = -1).
+ * A pixel with count >= num_consistent is accepted and sets used = 1 at the pixel of every consistent j.  Every
+ * operation is one fp32 rounding (no FMA contraction), so the result is a function of the inputs alone.  used_out
+ * [V,H,W] (may be NULL) receives the final used map.  Limits: V, H, W >= 1, V*H*W < 2^31, num_consistent >= 1,
+ * thresholds finite and >= 0.  One launch per view, no allocation, no synchronisation; the used map lives in the
+ * workspace (pmvs_fuse_depth_maps_workspace_bytes(V, H, W) bytes, 256-byte aligned, device memory) and is zeroed
+ * inside with an async memset. */
+size_t pmvs_fuse_depth_maps_workspace_bytes(int V, int H, int W); /* 0 + pmvs_last_error on a bad shape */
+int pmvs_fuse_depth_maps(const float* depth, const float* cam_block, int V, int H, int W, int num_consistent,
+                         float depth_thresh, float reproj_thresh, int* count_out, float* xyz_out,
+                         unsigned char* used_out, void* workspace, size_t workspace_bytes, pmvs_stream_t stream);
+
 /* ---- layout helpers used by the module-level API --------------------------------- */
 /* batched 2-D transpose: in [batch, R, C] -> out [batch, C, R] */
 int pmvs_transpose(const float* in, float* out, int batch, int R, int C, pmvs_stream_t stream);

@@ -112,3 +112,66 @@ def make_flow_params(seed=1):
         p["mlp%d_beta" % i] = 0.1 * torch.randn(cout, generator=g)
     p["mlp3_w"] = xavier(1, 16)
     return p
+
+
+def make_fusion_scene(views, height, width, seed=0, noise=0.0, holes=0.0, bad=0, tilt=(0.08, -0.05),
+                      bump_radius=60.0, cap=0.25):
+    """A DTU-like scene for depth-map fusion (numpy; nothing is read from disk).
+
+    Cameras sit on a spherical cap of half-angle `cap` (radians) 650 mm from the target (0, 0, 650) and look at it;
+    K is at the map size (2892.33 px focal length at 1600 px width).  The surface is the plane
+    z = 650 + tilt[0] x + tilt[1] y with a sphere of radius `bump_radius` (0: none) bulging 40 mm out of it towards
+    the cameras, so that the bump hides parts of the plane from some views.  Depth maps are ray-cast in float64 at the
+    pixel centres (0 where a ray misses) and then rounded to fp32.  Optional, all seeded: relative Gaussian noise of
+    standard deviation `noise`, a fraction `holes` of pixels set to 0, and `bad` pixels per view set to NaN, +inf,
+    -inf or a negative depth.
+    -> {"depth": float32 [V,H,W], "cams": float64 [V,2,4,4] (the library's camera layout, depth range in row
+    [1,3]), "images": uint8 RGB [V,H,W,3]}"""
+    import numpy as np
+    rng = np.random.default_rng(seed)
+    target = np.array([0.0, 0.0, 650.0])
+    f = 2892.33 * width / 1600.0
+    K = np.array([[f, 0.0, width / 2.0], [0.0, f, height / 2.0], [0.0, 0.0, 1.0]])
+    normal = np.array([-tilt[0], -tilt[1], 1.0])  # plane: normal . P = 650
+    centre = np.array([20.0, -10.0, 650.0 - 40.0 + bump_radius])
+    ys, xs = np.meshgrid(np.arange(height) + 0.5, np.arange(width) + 0.5, indexing="ij")
+    pix = np.stack([xs.reshape(-1), ys.reshape(-1), np.ones(height * width)])
+    cams = np.zeros((views, 2, 4, 4))
+    depth = np.zeros((views, height, width), dtype=np.float32)
+    for v in range(views):
+        theta = cap * math.sqrt((v + 0.5) / views) + 0.01 * rng.standard_normal()
+        phi = 2.399963 * v + 0.05 * rng.standard_normal()
+        c = target + 650.0 * np.array([math.sin(theta) * math.cos(phi), math.sin(theta) * math.sin(phi),
+                                       -math.cos(theta)])
+        z = (target - c) / np.linalg.norm(target - c)
+        x = np.cross([0.0, -1.0, 0.0], z)
+        x /= np.linalg.norm(x)
+        R = np.stack([x, np.cross(z, x), z])
+        cams[v, 0, :3, :3] = R
+        cams[v, 0, :3, 3] = -R @ c
+        cams[v, 0, 3, 3] = 1.0
+        cams[v, 1, :3, :3] = K
+        cams[v, 1, 3] = (425.0, 2.5, 192.0, 425.0 + 2.5 * 191.0)
+        # rays c + s dw with camera-space direction (Kinv pix), whose z is 1, so s is the depth
+        dw = R.T @ (np.linalg.inv(K) @ pix)
+        s = (650.0 - normal @ c) / (normal @ dw)
+        s = np.where(s > 0, s, np.inf)
+        if bump_radius > 0:
+            oc = c - centre
+            a, b = np.sum(dw * dw, axis=0), 2.0 * (oc @ dw)
+            disc = b * b - 4.0 * a * (oc @ oc - bump_radius ** 2)
+            s1 = (-b - np.sqrt(np.maximum(disc, 0.0))) / (2.0 * a)
+            s = np.where((disc >= 0) & (s1 > 0) & (s1 < s), s1, s)
+        d = np.where(np.isfinite(s), s, 0.0)
+        if noise > 0:
+            d = d * (1.0 + noise * rng.standard_normal(d.shape))
+        depth[v] = d.reshape(height, width).astype(np.float32)
+    flat = depth.reshape(views, -1)
+    if holes > 0:
+        flat[rng.random(flat.shape) < holes] = 0.0
+    specials = np.array([np.nan, np.inf, -np.inf, -650.0], dtype=np.float32)
+    for v in range(views):
+        for k in range(bad):
+            flat[v, rng.integers(0, flat.shape[1])] = specials[k % 4]
+    images = rng.integers(0, 256, size=(views, height, width, 3), dtype=np.uint8)
+    return {"depth": depth, "cams": cams, "images": images}
