@@ -194,6 +194,44 @@ int pmvs_fuse_depth_maps(const float* depth, const float* cam_block, int V, int 
                          float depth_thresh, float reproj_thresh, int* count_out, float* xyz_out,
                          unsigned char* used_out, void* workspace, size_t workspace_bytes, pmvs_stream_t stream);
 
+/* ---- point-cloud evaluation (DESIGN 3.11): accuracy / completeness of a fused cloud against a reference scan ---- */
+/* The library's own DTU-style rule, not claimed to reproduce the DTU MATLAB evaluation's numbers.  xyz arrays are
+ * [n,3] fp32 device memory; a point with a non-finite coordinate is never kept by thinning and is nobody's neighbour.
+ * d2(p, q) = (dx*dx + dy*dy) + dz*dz with dx = q.x - p.x, every operation one fp32 rounding (no FMA contraction).
+ * Both searches run over a hashed grid of side `cell`, a power of two in [2^-60, 2^60]; the results do not depend on
+ * it (it only sets the speed: about dst for thinning, max_dist / 16 for distances).  Counts n, nq, nt are in
+ * [0, 2^31 - 1).  No floating-point atomics, no allocation, no synchronisation; results do not depend on thread order.
+ *
+ * Greedy radius thinning: visit the points in the order `order` (int64 [n], a permutation of 0..n-1); a visited point
+ * that has not been removed is kept and removes every q with d2 <= fl(dst*dst).  Computed as rounds of the parallel
+ * greedy maximal independent set, whose outcome equals the sequential one: in round r an undecided point with a
+ * neighbour kept before r is removed, and one with no such neighbour and no neighbour still undecided at the start of
+ * r earlier in the order is kept.  One call runs rounds [first_round, first_round + rounds); call it with first_round =
+ * 0, then again with first_round advanced by `rounds` while undecided[rounds - 1] > 0 (a round after the last useful
+ * one returns at once).  state [n] int32 (device) carries the rounds between calls: 0 undecided, 2r+2 kept in round
+ * r, 2r+3 removed in round r, 1 removed (non-finite); kept = state > 0 && even.  undecided [rounds] int32 (device):
+ * points still undecided after each round of the call.  dst finite > 0; first_round + rounds <= 2^29.  workspace:
+ * pmvs_thin_cloud_workspace_bytes(n) bytes, 256-byte aligned, device memory (the grid is rebuilt by every call). */
+size_t pmvs_thin_cloud_workspace_bytes(int n); /* 0 + pmvs_last_error on a bad shape */
+int pmvs_thin_cloud(const float* xyz, const int64_t* order, int n, float dst, float cell, int first_round, int rounds,
+                    int* state, int* undecided, void* workspace, size_t workspace_bytes, pmvs_stream_t stream);
+/* Exact nearest-neighbour distances: dist[i] = sqrt(min over the target of d2(query_i, t)) (correctly rounded) when
+ * that is <= max_dist, +inf otherwise (also for an empty target), NaN for a query with a non-finite coordinate.
+ * max_dist finite >= 0.  workspace: pmvs_nearest_distances_workspace_bytes(nt) bytes, 256-byte aligned, device
+ * memory. */
+size_t pmvs_nearest_distances_workspace_bytes(int nt); /* 0 + pmvs_last_error on a bad shape */
+int pmvs_nearest_distances(const float* query, int nq, const float* target, int nt, float max_dist, float cell,
+                           float* dist, void* workspace, size_t workspace_bytes, pmvs_stream_t stream);
+/* Filters of the evaluation, flags [n] uint8 (device): bit 0 "in the box" fl(bb[c] - margin) <= p_c <
+ * fl(bb[3+c] + margin) on every axis; bit 1 "observed": in the box and, with a mask, g_c = rintf((p_c - bb[c]) / res)
+ * inside mask_dims with obs_mask[(g0*dims1 + g1)*dims2 + g2] != 0; bit 2 "above the plane" ((P0 x + P1 y) + P2 z) + P3
+ * > 0.  Each operation is one fp32 rounding.  A filter not given (bb / plane NULL) passes every finite point; a point
+ * with a non-finite coordinate gets 0.  bb [6] (BB[0] xyz then BB[1] xyz), mask_dims [3] and plane [4] are HOST
+ * arrays read during the call; obs_mask is device memory, C order, and needs bb, mask_dims and res finite > 0. */
+int pmvs_cloud_filter(const float* xyz, int n, const float* bb, float margin, const unsigned char* obs_mask,
+                      const int* mask_dims, float res, const float* plane, unsigned char* flags,
+                      pmvs_stream_t stream);
+
 /* ---- layout helpers used by the module-level API --------------------------------- */
 /* batched 2-D transpose: in [batch, R, C] -> out [batch, C, R] */
 int pmvs_transpose(const float* in, float* out, int batch, int R, int C, pmvs_stream_t stream);

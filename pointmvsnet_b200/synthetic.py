@@ -175,3 +175,21 @@ def make_fusion_scene(views, height, width, seed=0, noise=0.0, holes=0.0, bad=0,
             flat[v, rng.integers(0, flat.shape[1])] = specials[k % 4]
     images = rng.integers(0, 256, size=(views, height, width, 3), dtype=np.uint8)
     return {"depth": depth, "cams": cams, "images": images}
+
+
+def make_reference_cloud(spacing, extent=((-200.0, 200.0), (-160.0, 160.0)), tilt=(0.08, -0.05), bump_radius=60.0):
+    """The analytic surface of make_fusion_scene (same `tilt` and `bump_radius`) sampled on an x-y grid of the given
+    spacing (mm) over `extent` ((x0, x1), (y0, y1)): z = min(plane, front of the sphere bump), the part the cameras see.
+    Points are computed in float64 and rounded once -> numpy float32 [N,3].  On the plane the 3-D spacing is
+    spacing * sqrt(1 + tilt^2); on the bump's flanks it grows with the slope."""
+    import numpy as np
+    xs = np.arange(extent[0][0], extent[0][1] + 0.5 * spacing, spacing)
+    ys = np.arange(extent[1][0], extent[1][1] + 0.5 * spacing, spacing)
+    x, y = np.meshgrid(xs, ys, indexing="ij")
+    z = 650.0 + tilt[0] * x + tilt[1] * y
+    if bump_radius > 0:
+        cx, cy, cz = 20.0, -10.0, 650.0 - 40.0 + bump_radius
+        r2 = bump_radius ** 2 - (x - cx) ** 2 - (y - cy) ** 2
+        front = cz - np.sqrt(np.maximum(r2, 0.0))
+        z = np.where((r2 >= 0) & (front < z), front, z)
+    return np.stack([x.reshape(-1), y.reshape(-1), z.reshape(-1)], axis=1).astype(np.float32)
