@@ -232,6 +232,41 @@ int pmvs_cloud_filter(const float* xyz, int n, const float* bb, float margin, co
                       const int* mask_dims, float res, const float* plane, unsigned char* flags,
                       pmvs_stream_t stream);
 
+/* ---- coarse stage: VolumeConv and the depth regression (DESIGN 3.12; networks.py:127-167, model.py:115-130) ---- */
+/* The 11 layers in the reference's attribute order: conv0_1, conv1_0, conv2_0, conv3_0, conv1_1, conv2_1, conv3_1,
+ * conv4_0, conv5_0, conv6_0, conv6_2.  weight[l] is the PyTorch tensor as stored: Conv3d [Cout, Cin, 3, 3, 3] (l != 7,
+ * 8, 9), ConvTranspose3d [Cin, Cout, 3, 3, 3] (l = 7, 8, 9).  The BatchNorm arrays cover the first ten layers (conv6_2
+ * has none); running_mean / running_var are read in eval mode only and never written. */
+typedef struct pmvs_volume_weights {
+  const float* weight[11];
+  const float* gamma[10];
+  const float* beta[10];
+  const float* running_mean[10];
+  const float* running_var[10];
+  float eps[10];
+} pmvs_volume_weights;
+
+/* x [B, Cin, D, H, W] fp32 (the layout of the cost volume) -> out [B, 1, D, H, W]: the forward of VolumeConv with
+ * BatchNorm on batch statistics (train != 0; biased variance for normalising) or on the running statistics (train ==
+ * 0).  In train mode batch_sums (fp64 device memory, may be NULL) receives, per BatchNorm layer in the order above,
+ * the sums and then the sums of squares of that layer's convolution output over B * D' * H' * W' (D' = D >> level):
+ * [sum[Cout_l], sumsq[Cout_l]] for l = 0..9, 576 doubles for (64, 8); the caller updates its running statistics from
+ * them.  Supported: (in_channels, base_channels) = (64, 8), D, H, W positive multiples of 8, D*H*W <= 2^30, B <= 8192.
+ * fp32 FMA arithmetic; reductions in a fixed order (no floating-point atomics), so two calls give the same bits.  22
+ * launches, no allocation, no synchronisation; workspace: pmvs_volume_conv_workspace_bytes(...) bytes, 256-byte
+ * aligned, device memory. */
+size_t pmvs_volume_conv_workspace_bytes(int B, int in_channels, int base_channels, int D, int H, int W); /* 0 + error */
+int pmvs_volume_conv(const float* x, const pmvs_volume_weights* weights, int train, float* out, double* batch_sums,
+                     void* workspace, size_t workspace_bytes, int B, int in_channels, int base_channels, int D, int H,
+                     int W, pmvs_stream_t stream);
+/* filtered [B, D, H, W] fp32 (VolumeConv's output), cams [B, V, 2, 4, 4] fp32, both device memory -> depth_out and
+ * prob_out [B, H, W]: p = softmax(-filtered) over D, depth = sum_d depth_d p_d with depth_d = torch.linspace(start,
+ * end, D) as computed on a CUDA device, end = start + (D - 1) * interval in fp32, start / interval =
+ * cams[b, 0, 1, 3, 0:2] read on the device; prob = p[clamp(floor(t))] + p[clamp(ceil(t))], t = (depth - start) /
+ * interval.  The [B, D, H, W] probability volume is never written.  One launch. */
+int pmvs_coarse_depth(const float* filtered, const float* cams, int B, int V, int D, int H, int W, float* depth_out,
+                      float* prob_out, pmvs_stream_t stream);
+
 /* ---- layout helpers used by the module-level API --------------------------------- */
 /* batched 2-D transpose: in [batch, R, C] -> out [batch, C, R] */
 int pmvs_transpose(const float* in, float* out, int batch, int R, int C, pmvs_stream_t stream);

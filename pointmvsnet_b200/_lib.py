@@ -51,6 +51,13 @@ class FlowGrads(C.Structure):
     ]
 
 
+class VolumeWeights(C.Structure):
+    _fields_ = [
+        ("weight", C.c_void_p * 11), ("gamma", C.c_void_p * 10), ("beta", C.c_void_p * 10),
+        ("running_mean", C.c_void_p * 10), ("running_var", C.c_void_p * 10), ("eps", C.c_float * 10),
+    ]
+
+
 def _sig(name, restype, argtypes):
     fn = getattr(lib, name)
     fn.restype = restype
@@ -88,6 +95,9 @@ _sig("pmvs_thin_cloud", I, [P, P, I, F, F, I, I, P, P, P, C.c_size_t, P])
 _sig("pmvs_nearest_distances_workspace_bytes", C.c_size_t, [I])
 _sig("pmvs_nearest_distances", I, [P, I, P, I, F, F, P, P, C.c_size_t, P])
 _sig("pmvs_cloud_filter", I, [P, I, P, F, P, P, F, P, P, P])
+_sig("pmvs_volume_conv_workspace_bytes", C.c_size_t, [I, I, I, I, I, I])
+_sig("pmvs_volume_conv", I, [P, C.POINTER(VolumeWeights), I, P, P, P, C.c_size_t, I, I, I, I, I, I, P])
+_sig("pmvs_coarse_depth", I, [P, P, I, I, I, I, I, P, P, P])
 _sig("pmvs_transpose", I, [P, P, I, I, I, P])
 _sig("pmvs_idx64_to_idx32", I, [P, P, LL, P])
 _sig("pmvs_edgeconv_pm", I, [P, I, P, P, P, P, F, I, I, P, I, P, P, I, I, I, I, I, I, P])
@@ -112,6 +122,7 @@ EXPORTED = [
     "pmvs_cost_volume", "pmvs_cost_volume_backward_workspace_bytes", "pmvs_cost_volume_backward",
     "pmvs_fuse_depth_maps_workspace_bytes", "pmvs_fuse_depth_maps", "pmvs_thin_cloud_workspace_bytes",
     "pmvs_thin_cloud", "pmvs_nearest_distances_workspace_bytes", "pmvs_nearest_distances", "pmvs_cloud_filter",
+    "pmvs_volume_conv_workspace_bytes", "pmvs_volume_conv", "pmvs_coarse_depth",
     "pmvs_transpose", "pmvs_idx64_to_idx32", "pmvs_edgeconv_pm", "pmvs_edgeconv_pm_backward_workspace_bytes", "pmvs_edgeconv_pm_backward", "pmvs_linear_pm", "pmvs_point_flow_workspace_bytes",
     "pmvs_point_flow_iter", "pmvs_pyramid_to_channels_last", "pmvs_point_flow_debug_offsets",
     "pmvs_point_flow_debug_feature", "pmvs_point_flow_backward_workspace_bytes", "pmvs_point_flow_backward",

@@ -2,7 +2,8 @@
 features at the D depth-hypothesis planes of the reference view and reduce them to the variance cost
 volume the 3-D U-Net consumes - one fused sm_90a kernel instead of FeatureFetcher + three passes
 over the [B,V,C,D*h*w] tensor (503 MB at 640x512, V=4, D=96).  This is the row immediately before the
-PointFlow path (SURVEY.md section 8f-1); the reference model calls it once per forward."""
+PointFlow path (SURVEY.md section 8f-1); the reference model calls it once per forward.  ``coarse_depth`` is the
+regression that follows VolumeConv (model.py:117-130)."""
 import torch
 
 from ._lib import lib, check, stream_ptr, ptr, require_cuda, f32c
@@ -64,3 +65,48 @@ def build_cost_volume(feature_list, cam_params_list, is_test=True):
     if torch.is_grad_enabled() and feature_list.requires_grad:
         return _CostVolumeFn.apply(feats, cams.detach(), D, bool(is_test))
     return _forward(feats, cams, D, is_test)
+
+
+def coarse_depth(filtered_cost, cam_params_list):
+    """The coarse depth regression (model.py:117-130) in one sm_90a kernel (``pmvs_coarse_depth``).
+
+    filtered_cost: VolumeConv's output, [B,1,D,h,w] or [B,D,h,w], float32; cam_params_list [B,V,2,4,4] float32.
+    Returns (coarse_depth_map, coarse_prob_map), both [B,1,h,w]:
+      p = softmax(-filtered_cost) over D, coarse_depth_map = sum_d depth_d p_d, where depth_d are the planes
+      ``torch.linspace(start, start + (D-1) * interval, D)`` gives on a CUDA device (start, interval =
+      cam_params_list[:, 0, 1, 3, 0:2], read on the device: no host synchronisation);
+      coarse_prob_map = p at floor(t) plus p at ceil(t), t = (depth - start) / interval, both clamped to [0, D-1]
+      (``get_propability_map``).
+    The [B,D,h,w] probability volume is never written.  Forward-only: raises ``NotImplementedError`` with grad
+    enabled and an input requiring grad."""
+    if torch.is_grad_enabled() and (filtered_cost.requires_grad or cam_params_list.requires_grad):
+        raise NotImplementedError("pointmvsnet_b200 coarse_depth is forward-only; wrap the call in torch.no_grad()")
+    if filtered_cost.dim() == 5:
+        if filtered_cost.shape[1] != 1:
+            raise RuntimeError("coarse_depth: a 5-D filtered_cost must be [B,1,D,h,w], got %s"
+                               % (tuple(filtered_cost.shape),))
+        vol = filtered_cost.squeeze(1)
+    elif filtered_cost.dim() == 4:
+        vol = filtered_cost
+    else:
+        raise RuntimeError("coarse_depth: filtered_cost must be [B,1,D,h,w] or [B,D,h,w], got %s"
+                           % (tuple(filtered_cost.shape),))
+    if vol.dtype != torch.float32 or cam_params_list.dtype != torch.float32:
+        raise RuntimeError("coarse_depth: filtered_cost and cam_params_list must be float32")
+    B, D, H, W = vol.shape
+    if cam_params_list.dim() != 5 or cam_params_list.shape[0] != B or tuple(cam_params_list.shape[2:]) != (2, 4, 4):
+        raise RuntimeError("coarse_depth: cam_params_list must be [B,V,2,4,4] with B = %d, got %s"
+                           % (B, tuple(cam_params_list.shape)))
+    if min(B, D, H, W, cam_params_list.shape[1]) < 1:
+        raise RuntimeError("coarse_depth: empty input %s" % (tuple(vol.shape),))
+    require_cuda(vol, cam_params_list)
+    if cam_params_list.device != vol.device:
+        raise RuntimeError("coarse_depth: filtered_cost and cam_params_list must be on the same device")
+    vol = vol.contiguous()
+    cams = cam_params_list.contiguous()
+    depth = torch.empty(B, 1, H, W, device=vol.device, dtype=torch.float32)
+    prob = torch.empty(B, 1, H, W, device=vol.device, dtype=torch.float32)
+    with torch.cuda.device(vol.device):
+        check(lib.pmvs_coarse_depth(ptr(vol), ptr(cams), B, cams.shape[1], D, H, W, ptr(depth), ptr(prob),
+                                    stream_ptr()))
+    return depth, prob

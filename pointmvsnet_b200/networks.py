@@ -1,4 +1,4 @@
-"""EdgeConv / EdgeConvNoC (reference networks.py:9-81), CUDA-branch semantics.
+"""EdgeConv / EdgeConvNoC (reference networks.py:9-81), CUDA-branch semantics, and VolumeConv (networks.py:127-167).
 
 Same constructor, parameter names (``conv1``, ``conv2``, ``bn``) and forward signature as
 the reference, so its checkpoints load unchanged.  The forward runs three sm_90a kernels
@@ -7,12 +7,14 @@ data; the [B,C,N,K] tensors of the reference are never materialised.
 
 By default the layers are forward-only and raise under autograd.  ``enable_backward()`` turns on a fused, deterministic
 backward (``pmvs_edgeconv_pm_backward``) so that a model built from these layers trains."""
+import ctypes
+
 import torch
 import torch.nn as nn
 from torch.autograd.function import once_differentiable
 
-from ._lib import lib, check, stream_ptr, ptr, require_cuda, f32c
-from .nn.conv import Conv2d
+from ._lib import lib, check, stream_ptr, ptr, require_cuda, f32c, VolumeWeights
+from .nn.conv import Conv2d, Conv3d, Deconv3d
 
 _SUPPORTED_COUT = (16, 32, 64, 128)
 _backward_enabled = False
@@ -253,4 +255,144 @@ def stack_views_channels_last(per_view, keys=("conv1", "conv2", "conv3"), out=No
         for v, d in enumerate(per_view):
             buf[:, v].copy_(d[k].permute(0, 2, 3, 1))  # NHWC -> NHWC: a plain contiguous copy for a channels-last source
         res[k] = buf.permute(0, 1, 4, 2, 3)
+    return res
+
+
+# the layers of VolumeConv in the order of pmvs_volume_weights (include/pmvs_b200.h)
+_VOLUME_LAYERS = ("conv0_1", "conv1_0", "conv2_0", "conv3_0", "conv1_1", "conv2_1", "conv3_1", "conv4_0", "conv5_0",
+                  "conv6_0", "conv6_2")
+_VOLUME_SUPPORTED = (64, 8)
+
+
+class VolumeConv(nn.Module):
+    """The coarse stage's 3-D U-Net (reference networks.py:127-167, ``coarse_vol_conv`` at model.py:27,115):
+    cost volume [B, in_channels, D, h, w] -> filtered volume [B, 1, D, h, w].
+
+    Same constructor, attribute names (``conv0_1`` ... ``conv6_2``) and ``out_channels`` as the reference, so
+    ``coarse_vol_conv.*`` checkpoint keys load unchanged.  The forward runs all 11 layers through
+    ``pmvs_volume_conv`` (fp32 direct convolutions on sm_90a, DESIGN 3.12) on the current stream.  BatchNorm follows
+    the module's mode: batch statistics in train mode (test.py:58 keeps the model there), with the running statistics
+    and ``num_batches_tracked`` updated as ``nn.BatchNorm3d`` does, each layer with its own momentum and eps; the
+    running statistics in eval mode.  ``momentum=None`` gives BatchNorm's cumulative average.
+
+    Supported: (in_channels, base_channels) = (64, 8), the shipped configuration; D, h, w multiples of 8 (the
+    reference fails at its skip additions otherwise).  Forward-only: with grad enabled and the input or a parameter
+    requiring grad it raises ``NotImplementedError``; wrap inference in ``torch.no_grad()``."""
+
+    def __init__(self, in_channels, base_channels):
+        super().__init__()
+        b = base_channels
+        self.in_channels = in_channels
+        self.out_channels = base_channels * 8
+        self.base_channels = base_channels
+        self.conv1_0 = Conv3d(in_channels, b * 2, 3, stride=2, padding=1)
+        self.conv2_0 = Conv3d(b * 2, b * 4, 3, stride=2, padding=1)
+        self.conv3_0 = Conv3d(b * 4, b * 8, 3, stride=2, padding=1)
+        self.conv0_1 = Conv3d(in_channels, b, 3, 1, padding=1)
+        self.conv1_1 = Conv3d(b * 2, b * 2, 3, 1, padding=1)
+        self.conv2_1 = Conv3d(b * 4, b * 4, 3, 1, padding=1)
+        self.conv3_1 = Conv3d(b * 8, b * 8, 3, 1, padding=1)
+        self.conv4_0 = Deconv3d(b * 8, b * 4, 3, 2, padding=1, output_padding=1)
+        self.conv5_0 = Deconv3d(b * 4, b * 2, 3, 2, padding=1, output_padding=1)
+        self.conv6_0 = Deconv3d(b * 2, b, 3, 2, padding=1, output_padding=1)
+        self.conv6_2 = nn.Conv3d(b, 1, 3, padding=1, bias=False)
+
+    def _bns(self):
+        return [getattr(self, n).bn for n in _VOLUME_LAYERS[:10]]
+
+    def forward(self, x):
+        if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters())):
+            raise NotImplementedError("pointmvsnet_b200 VolumeConv is forward-only; wrap the call in torch.no_grad() "
+                                      "(its backward is not implemented)")
+        if x.dim() != 5 or x.dtype != torch.float32:
+            raise RuntimeError("VolumeConv: input must be a float32 [B, C, D, h, w] tensor, got %s %s"
+                               % (x.dtype, tuple(x.shape)))
+        B, C, D, H, W = x.shape
+        if (self.in_channels, self.base_channels) != _VOLUME_SUPPORTED:
+            raise RuntimeError("VolumeConv: (in_channels, base_channels) = (%d, %d) is not supported; the fused "
+                               "kernels serve (64, 8)" % (self.in_channels, self.base_channels))
+        if C != self.in_channels:
+            raise RuntimeError("VolumeConv: input has %d channels, the module expects %d" % (C, self.in_channels))
+        if B < 1 or min(D, H, W) < 8 or D % 8 or H % 8 or W % 8:
+            raise RuntimeError("VolumeConv: D, h, w = %d, %d, %d must be positive multiples of 8" % (D, H, W))
+        bns = self._bns()
+        modes = set(bn.training or not bn.track_running_stats for bn in bns)
+        if len(modes) != 1:
+            raise RuntimeError("VolumeConv: its BatchNorm layers must all be in train mode or all in eval mode")
+        train = modes.pop()
+        if train and B * (D // 8) * (H // 8) * (W // 8) < 2:
+            raise RuntimeError("VolumeConv: in train mode the coarsest level needs more than 1 value per channel "
+                               "(B*D*h*w/512 = %d)" % (B * (D // 8) * (H // 8) * (W // 8)))
+        require_cuda(x, *self.parameters())
+        dev = x.device
+        if any(t.device != dev for t in list(self.parameters()) + list(self.buffers())):
+            raise RuntimeError("VolumeConv: the module's parameters and buffers must be on the input's device")
+        keep = []
+
+        def p32(t):
+            t = f32c(t.detach())
+            keep.append(t)
+            return t.data_ptr()
+
+        wt = VolumeWeights()
+        for l, name in enumerate(_VOLUME_LAYERS):
+            m = getattr(self, name)
+            wt.weight[l] = p32(m.weight if name == "conv6_2" else m.conv.weight)
+        for l, bn in enumerate(bns):
+            wt.gamma[l], wt.beta[l], wt.eps[l] = p32(bn.weight), p32(bn.bias), float(bn.eps)
+            if not train:
+                wt.running_mean[l], wt.running_var[l] = p32(bn.running_mean), p32(bn.running_var)
+        xin = x.contiguous()
+        out = torch.empty(B, 1, D, H, W, device=dev, dtype=torch.float32)
+        couts = [bn.num_features for bn in bns]
+        sums = torch.empty(2 * sum(couts), device=dev, dtype=torch.float64) if train else None
+        with torch.cuda.device(dev):
+            nbytes = int(lib.pmvs_volume_conv_workspace_bytes(B, C, self.base_channels, D, H, W))
+            if nbytes == 0:
+                check(1)
+            ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)  # the caching allocator aligns to 512 bytes
+            check(lib.pmvs_volume_conv(ptr(xin), ctypes.byref(wt), 1 if train else 0, ptr(out), ptr(sums),
+                                       ptr(ws), nbytes, B, C, self.base_channels, D, H, W, stream_ptr()))
+        if train:
+            key = (B, D, H, W, str(dev))
+            if getattr(self, "_pmvs_counts", (None,))[0] != key:  # one small upload per shape, not per call
+                n = torch.cat([torch.full((c,), float(B * (D >> l) * (H >> l) * (W >> l)), dtype=torch.float64)
+                               for c, l in zip(couts, _LEVEL)]).to(dev)
+                object.__setattr__(self, "_pmvs_counts", (key, n))
+            _update_running_3d(bns, sums, couts, self._pmvs_counts[1])
+        return out
+
+
+# output level of each BatchNorm layer of VolumeConv (each level halves D, h and w)
+_LEVEL = (0, 1, 2, 3, 1, 2, 3, 2, 1, 0)
+
+
+def _update_running_3d(bns, sums, couts, n):
+    """nn.BatchNorm3d's train-mode side effect for every layer, from the fp64 batch sums [sum; sumsq] per layer and
+    the per-channel value counts n (device); without a host read (momentum=None: the cumulative average
+    1 / num_batches_tracked)."""
+    s = torch.cat([sums[2 * o:2 * o + 2 * c].view(2, c) for o, c in zip(_offsets(couts), couts)], dim=1)
+    mean = s[0] / n
+    var = ((s[1] / n - mean * mean).clamp_(min=0) * (n / (n - 1.0))).float()
+    mean = mean.float()
+    off = 0
+    for bn, c in zip(bns, couts):
+        if bn.track_running_stats and bn.running_mean is not None:
+            bn.num_batches_tracked.add_(1)
+            m, v = mean[off:off + c], var[off:off + c]
+            if bn.momentum is None:
+                f = 1.0 / bn.num_batches_tracked.float()
+                bn.running_mean.add_((m - bn.running_mean) * f)
+                bn.running_var.add_((v - bn.running_var) * f)
+            else:
+                bn.running_mean.mul_(1 - bn.momentum).add_(m, alpha=bn.momentum)
+                bn.running_var.mul_(1 - bn.momentum).add_(v, alpha=bn.momentum)
+        off += c
+
+
+def _offsets(couts):
+    o, res = 0, []
+    for c in couts:
+        res.append(o)
+        o += c
     return res
