@@ -18,7 +18,11 @@ DTU_STD = (84.45612252, 93.22252387, 80.08551226)  # dataset.py:27
 
 
 def make_cameras(batch, views, height, width, num_depth=96, dtype=torch.float32):
-    """cam_params_list [B,V,2,4,4] at FULL image resolution (isTest=True convention)."""
+    """cam_params_list [B,V,2,4,4] at FULL image resolution (isTest=True convention).
+
+    One rig replicated over views and batch: every view has the same K, and every batch element the same cameras
+    and depth range.  A kernel that reads another view's K or batch element 0's cameras computes the same numbers
+    from these; tests/camera_variety.py builds cameras that differ per view and per batch element."""
     s_int = 4.24 if num_depth == 48 else 2.13  # config.py:28 / configs/dtu_wde3.yaml:12
     cams = torch.zeros(batch, views, 2, 4, 4, dtype=torch.float64)
     f = 2892.33 * width / 1600.0
@@ -115,23 +119,25 @@ def make_flow_params(seed=1):
 
 
 def make_fusion_scene(views, height, width, seed=0, noise=0.0, holes=0.0, bad=0, tilt=(0.08, -0.05),
-                      bump_radius=60.0, cap=0.25):
+                      bump_radius=60.0, cap=0.25, focal_jitter=0.0, centre_jitter=0.0):
     """A DTU-like scene for depth-map fusion (numpy; nothing is read from disk).
 
     Cameras sit on a spherical cap of half-angle `cap` (radians) 650 mm from the target (0, 0, 650) and look at it;
-    K is at the map size (2892.33 px focal length at 1600 px width).  The surface is the plane
-    z = 650 + tilt[0] x + tilt[1] y with a sphere of radius `bump_radius` (0: none) bulging 40 mm out of it towards
-    the cameras, so that the bump hides parts of the plane from some views.  Depth maps are ray-cast in float64 at the
-    pixel centres (0 where a ray misses) and then rounded to fp32.  Optional, all seeded: relative Gaussian noise of
-    standard deviation `noise`, a fraction `holes` of pixels set to 0, and `bad` pixels per view set to NaN, +inf,
-    -inf or a negative depth.
+    K is at the map size (2892.33 px focal length at 1600 px width).  `focal_jitter` (relative) and `centre_jitter`
+    (pixels) give every view its own fx, fy and principal point, drawn uniformly from +-jitter by a generator of their
+    own (so that the default scene does not change); each view's depth map is ray-cast with its own K.  The surface is
+    the plane z = 650 + tilt[0] x + tilt[1] y with a sphere of radius `bump_radius` (0: none) bulging 40 mm out of it
+    towards the cameras, so that the bump hides parts of the plane from some views.  Depth maps are ray-cast in
+    float64 at the pixel centres (0 where a ray misses) and then rounded to fp32.  Optional, all seeded: relative
+    Gaussian noise of standard deviation `noise`, a fraction `holes` of pixels set to 0, and `bad` pixels per view set
+    to NaN, +inf, -inf or a negative depth.
     -> {"depth": float32 [V,H,W], "cams": float64 [V,2,4,4] (the library's camera layout, depth range in row
     [1,3]), "images": uint8 RGB [V,H,W,3]}"""
     import numpy as np
     rng = np.random.default_rng(seed)
     target = np.array([0.0, 0.0, 650.0])
     f = 2892.33 * width / 1600.0
-    K = np.array([[f, 0.0, width / 2.0], [0.0, f, height / 2.0], [0.0, 0.0, 1.0]])
+    jit = np.random.default_rng([seed, 1])
     normal = np.array([-tilt[0], -tilt[1], 1.0])  # plane: normal . P = 650
     centre = np.array([20.0, -10.0, 650.0 - 40.0 + bump_radius])
     ys, xs = np.meshgrid(np.arange(height) + 0.5, np.arange(width) + 0.5, indexing="ij")
@@ -147,6 +153,10 @@ def make_fusion_scene(views, height, width, seed=0, noise=0.0, holes=0.0, bad=0,
         x = np.cross([0.0, -1.0, 0.0], z)
         x /= np.linalg.norm(x)
         R = np.stack([x, np.cross(z, x), z])
+        K = np.array([[f, 0.0, width / 2.0], [0.0, f, height / 2.0], [0.0, 0.0, 1.0]])
+        if focal_jitter > 0 or centre_jitter > 0:
+            K[[0, 1], [0, 1]] *= 1.0 + focal_jitter * jit.uniform(-1.0, 1.0, 2)
+            K[[0, 1], [2, 2]] += centre_jitter * jit.uniform(-1.0, 1.0, 2)
         cams[v, 0, :3, :3] = R
         cams[v, 0, :3, 3] = -R @ c
         cams[v, 0, 3, 3] = 1.0
