@@ -267,6 +267,46 @@ int pmvs_volume_conv(const float* x, const pmvs_volume_weights* weights, int tra
 int pmvs_coarse_depth(const float* filtered, const float* cams, int B, int V, int D, int H, int W, float* depth_out,
                       float* prob_out, pmvs_stream_t stream);
 
+/* Outputs of pmvs_volume_conv_backward, PyTorch layouts, overwritten (not accumulated), like pmvs_flow_grads. */
+typedef struct pmvs_volume_grads {
+  float* weight[11]; /* Conv3d [Cout, Cin, 3, 3, 3]; ConvTranspose3d (l = 7, 8, 9) [Cin, Cout, 3, 3, 3] */
+  float* gamma[10];
+  float* beta[10];
+} pmvs_volume_grads;
+
+/* Bytes of device workspace pmvs_volume_conv_backward needs; 0 (with pmvs_last_error) for a shape the forward does not
+ * take.  With V_k = D*H*W / 8^k the voxels of level k, layer l reading Cin_l channels at V_in,l voxels and writing
+ * Cout_l at V_out,l, w_l = 27 Cin_l Cout_l and up(n) = n rounded up to a multiple of 256:
+ *   sum_l up(4 w_l)                                             packed data-gradient weights
+ * + sum_{l < 10} up(4 B Cout_l V_out,l) + up(16 Cout_l)          G_l (the pre-BatchNorm gradient) and its constants
+ * + sum_{l != conv1_0} up(4 B Cin_l V_in,l)                      data gradients (conv0_1's: its share of grad_x)
+ * + up(max_{l < 10} 16 Cout_l B ceil(V_out,l / 4096))            BatchNorm-backward partials
+ * + up(max_l 8 w_l B n_l)                                        weight-gradient partials,
+ * n_l = max(1, min(ceil(4224 / (3 Cin_l (Cout_l / c_l) B)), ceil(P_l / 1024))), c_l = 8 (1 for conv6_2), P_l = V_in,l
+ * for the transposed layers and V_out,l otherwise.  For (64, 8) that is about 4 B D H W (64 + 3 * 8 + 12) bytes. */
+size_t pmvs_volume_conv_backward_workspace_bytes(int B, int in_channels, int base_channels, int D, int H, int W);
+/* Gradients of one pmvs_volume_conv call given grad_out [B, 1, D, H, W]: grad_x [B, Cin, D, H, W] (NULL: skipped, with
+ * the two largest launches) and, in grads, every weight, gamma and beta.  fwd_workspace is the workspace of a
+ * pmvs_volume_conv call with the same shapes, weights and train flag, not modified since; it is only read, so the call
+ * can be repeated.  batch_sums is that call's output and is required in train mode (the batch statistics are
+ * recomputed from it); eval mode reads the running statistics in weights.  The ReLU masks are the forward's own
+ * activations (no gradient at exactly 0, as PyTorch); padding gets no gradient.  Train mode: dgamma = sum dz xhat,
+ * dbeta = sum dz, G = gamma invstd (dz - dbeta / n - xhat dgamma / n); eval: G = gamma invstd dz.  Every argument is
+ * checked before any launch.  fp32 products; per-CTA and final sums in a fixed order (fp64 across threads and CTAs), no
+ * floating-point atomics, so two calls give the same bits.  No allocation, no synchronisation.  workspace:
+ * pmvs_volume_conv_backward_workspace_bytes(...) bytes, 256-byte aligned, device memory (as is fwd_workspace). */
+int pmvs_volume_conv_backward(const float* x, const pmvs_volume_weights* weights, int train,
+                              const void* fwd_workspace, const double* batch_sums, const float* grad_out,
+                              float* grad_x /* NULL: skip */, const pmvs_volume_grads* grads, void* workspace,
+                              size_t workspace_bytes, int B, int in_channels, int base_channels, int D, int H, int W,
+                              pmvs_stream_t stream);
+/* Backward of pmvs_coarse_depth with respect to filtered: grad_filtered[b, d] = g p_d (depth - z_d), with g =
+ * grad_depth [B, H, W], p = softmax(-filtered) and the planes z_d as the forward computes them, and depth the forward's
+ * fp64 expectation before rounding (exactly 0 for D = 1).  The cameras and the probability map get no gradient.  One
+ * launch, every element of grad_filtered [B, D, H, W] written. */
+int pmvs_coarse_depth_backward(const float* filtered, const float* cams, const float* grad_depth,
+                               float* grad_filtered, int B, int V, int D, int H, int W, pmvs_stream_t stream);
+
 /* ---- layout helpers used by the module-level API --------------------------------- */
 /* batched 2-D transpose: in [batch, R, C] -> out [batch, C, R] */
 int pmvs_transpose(const float* in, float* out, int batch, int R, int C, pmvs_stream_t stream);

@@ -5,6 +5,7 @@ over the [B,V,C,D*h*w] tensor (503 MB at 640x512, V=4, D=96).  This is the row i
 PointFlow path (SURVEY.md section 8f-1); the reference model calls it once per forward.  ``coarse_depth`` is the
 regression that follows VolumeConv (model.py:117-130)."""
 import torch
+from torch.autograd.function import once_differentiable
 
 from ._lib import lib, check, stream_ptr, ptr, require_cuda, f32c
 
@@ -67,6 +68,47 @@ def build_cost_volume(feature_list, cam_params_list, is_test=True):
     return _forward(feats, cams, D, is_test)
 
 
+class _CoarseDepthFn(torch.autograd.Function):
+    """coarse_depth under autograd: coarse_depth_map is differentiable in filtered_cost (pmvs_coarse_depth_backward);
+    coarse_prob_map is not (the reference computes it under no_grad, functions.py:141-175), and the cameras get no
+    gradient (the reference's torch.linspace planes carry none)."""
+
+    @staticmethod
+    def forward(ctx, filtered_cost, cams):
+        vol = _volume_of(filtered_cost).contiguous()
+        depth, prob = _coarse_forward(vol, cams)
+        ctx.save_for_backward(vol, cams)
+        ctx.in_shape = filtered_cost.shape
+        ctx.mark_non_differentiable(prob)
+        return depth, prob
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_depth, grad_prob):
+        vol, cams = ctx.saved_tensors
+        B, D, H, W = vol.shape
+        g = torch.zeros(B, 1, H, W, device=vol.device, dtype=torch.float32) if grad_depth is None else f32c(grad_depth)
+        grad = torch.empty_like(vol)
+        with torch.cuda.device(vol.device):
+            check(lib.pmvs_coarse_depth_backward(ptr(vol), ptr(cams), ptr(g), ptr(grad), B, cams.shape[1], D, H, W,
+                                                 stream_ptr()))
+        return grad.view(ctx.in_shape), None
+
+
+def _volume_of(filtered_cost):
+    return filtered_cost.squeeze(1) if filtered_cost.dim() == 5 else filtered_cost
+
+
+def _coarse_forward(vol, cams):
+    B, D, H, W = vol.shape
+    depth = torch.empty(B, 1, H, W, device=vol.device, dtype=torch.float32)
+    prob = torch.empty(B, 1, H, W, device=vol.device, dtype=torch.float32)
+    with torch.cuda.device(vol.device):
+        check(lib.pmvs_coarse_depth(ptr(vol), ptr(cams), B, cams.shape[1], D, H, W, ptr(depth), ptr(prob),
+                                    stream_ptr()))
+    return depth, prob
+
+
 def coarse_depth(filtered_cost, cam_params_list):
     """The coarse depth regression (model.py:117-130) in one sm_90a kernel (``pmvs_coarse_depth``).
 
@@ -77,20 +119,24 @@ def coarse_depth(filtered_cost, cam_params_list):
       cam_params_list[:, 0, 1, 3, 0:2], read on the device: no host synchronisation);
       coarse_prob_map = p at floor(t) plus p at ceil(t), t = (depth - start) / interval, both clamped to [0, D-1]
       (``get_propability_map``).
-    The [B,D,h,w] probability volume is never written.  Forward-only: raises ``NotImplementedError`` with grad
-    enabled and an input requiring grad."""
-    if torch.is_grad_enabled() and (filtered_cost.requires_grad or cam_params_list.requires_grad):
-        raise NotImplementedError("pointmvsnet_b200 coarse_depth is forward-only; wrap the call in torch.no_grad()")
+    The [B,D,h,w] probability volume is never written.  With grad enabled and an input requiring grad it raises
+    ``NotImplementedError`` unless ``networks.enable_volume_backward()`` is on; then coarse_depth_map is
+    differentiable in ``filtered_cost`` (``pmvs_coarse_depth_backward``: g p_d (depth - depth_d), the gradient in
+    ``filtered_cost``'s shape), coarse_prob_map is marked non-differentiable and ``cam_params_list`` gets no
+    gradient."""
+    from . import networks
+    grad = torch.is_grad_enabled() and (filtered_cost.requires_grad or cam_params_list.requires_grad)
+    if grad and not networks.volume_backward_enabled():
+        raise NotImplementedError("pointmvsnet_b200 coarse_depth is forward-only; wrap the call in torch.no_grad() "
+                                  "or call pointmvsnet_b200.networks.enable_volume_backward()")
     if filtered_cost.dim() == 5:
         if filtered_cost.shape[1] != 1:
             raise RuntimeError("coarse_depth: a 5-D filtered_cost must be [B,1,D,h,w], got %s"
                                % (tuple(filtered_cost.shape),))
-        vol = filtered_cost.squeeze(1)
-    elif filtered_cost.dim() == 4:
-        vol = filtered_cost
-    else:
+    elif filtered_cost.dim() != 4:
         raise RuntimeError("coarse_depth: filtered_cost must be [B,1,D,h,w] or [B,D,h,w], got %s"
                            % (tuple(filtered_cost.shape),))
+    vol = _volume_of(filtered_cost)
     if vol.dtype != torch.float32 or cam_params_list.dtype != torch.float32:
         raise RuntimeError("coarse_depth: filtered_cost and cam_params_list must be float32")
     B, D, H, W = vol.shape
@@ -102,11 +148,7 @@ def coarse_depth(filtered_cost, cam_params_list):
     require_cuda(vol, cam_params_list)
     if cam_params_list.device != vol.device:
         raise RuntimeError("coarse_depth: filtered_cost and cam_params_list must be on the same device")
-    vol = vol.contiguous()
-    cams = cam_params_list.contiguous()
-    depth = torch.empty(B, 1, H, W, device=vol.device, dtype=torch.float32)
-    prob = torch.empty(B, 1, H, W, device=vol.device, dtype=torch.float32)
-    with torch.cuda.device(vol.device):
-        check(lib.pmvs_coarse_depth(ptr(vol), ptr(cams), B, cams.shape[1], D, H, W, ptr(depth), ptr(prob),
-                                    stream_ptr()))
-    return depth, prob
+    cams = cam_params_list.detach().contiguous()
+    if grad and filtered_cost.requires_grad:
+        return _CoarseDepthFn.apply(filtered_cost, cams)
+    return _coarse_forward(vol.detach().contiguous(), cams)

@@ -13,11 +13,12 @@ import torch
 import torch.nn as nn
 from torch.autograd.function import once_differentiable
 
-from ._lib import lib, check, stream_ptr, ptr, require_cuda, f32c, VolumeWeights
+from ._lib import lib, check, stream_ptr, ptr, require_cuda, f32c, VolumeWeights, VolumeGrads
 from .nn.conv import Conv2d, Conv3d, Deconv3d
 
 _SUPPORTED_COUT = (16, 32, 64, 128)
 _backward_enabled = False
+_volume_backward_enabled = False
 
 
 def enable_backward(enabled=True):
@@ -35,6 +36,28 @@ def enable_backward(enabled=True):
     prev = _backward_enabled
     _backward_enabled = bool(enabled)
     return prev
+
+
+def enable_volume_backward(enabled=True):
+    """Process-wide switch for the coarse stage: while on, ``VolumeConv`` and ``cost_volume.coarse_depth`` called with
+    grad enabled (and an input or parameter that requires grad) run through autograd Functions whose backwards are the
+    fused, deterministic CUDA backwards (``pmvs_volume_conv_backward``, ``pmvs_coarse_depth_backward``); while off (the
+    default) such calls raise ``NotImplementedError``.  Returns the previous setting.  ``enable_backward()`` does not
+    cover these two.
+
+    It is opt-in because a grad-enabled ``VolumeConv`` forward keeps its whole workspace
+    (``pmvs_volume_conv_workspace_bytes``: every layer's pre-BatchNorm output, about 23 MB per batch element at
+    [B,64,48,64,80]) and its input alive until backward runs; the backward then allocates its own workspace
+    (``pmvs_volume_conv_backward_workspace_bytes``, about 100 MB per batch element at that shape) for the duration of
+    the call.  Under ``torch.no_grad()`` the switch has no effect."""
+    global _volume_backward_enabled
+    prev = _volume_backward_enabled
+    _volume_backward_enabled = bool(enabled)
+    return prev
+
+
+def volume_backward_enabled():
+    return _volume_backward_enabled
 
 
 def _edge_layer(mod, feature, knn_inds, concat_central):
@@ -276,8 +299,12 @@ class VolumeConv(nn.Module):
     running statistics in eval mode.  ``momentum=None`` gives BatchNorm's cumulative average.
 
     Supported: (in_channels, base_channels) = (64, 8), the shipped configuration; D, h, w multiples of 8 (the
-    reference fails at its skip additions otherwise).  Forward-only: with grad enabled and the input or a parameter
-    requiring grad it raises ``NotImplementedError``; wrap inference in ``torch.no_grad()``."""
+    reference fails at its skip additions otherwise).  With grad enabled and the input or a parameter requiring grad it
+    raises ``NotImplementedError`` unless ``enable_volume_backward()`` is on; then the call runs through an autograd
+    Function whose backward is the fused, deterministic ``pmvs_volume_conv_backward`` (DESIGN 3.13), filling the
+    parameters' ``.grad`` and, when the input requires grad, its gradient.  Its forward output is bit-identical to the
+    ``no_grad`` forward, and the running statistics update once, in the forward.  Wrap inference in
+    ``torch.no_grad()``."""
 
     def __init__(self, in_channels, base_channels):
         super().__init__()
@@ -302,8 +329,21 @@ class VolumeConv(nn.Module):
 
     def forward(self, x):
         if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters())):
-            raise NotImplementedError("pointmvsnet_b200 VolumeConv is forward-only; wrap the call in torch.no_grad() "
-                                      "(its backward is not implemented)")
+            if not _volume_backward_enabled:
+                raise NotImplementedError("pointmvsnet_b200 VolumeConv is forward-only; wrap the call in "
+                                          "torch.no_grad() or call pointmvsnet_b200.networks.enable_volume_backward()")
+            self._check_input(x)
+            return _VolumeConvFn.apply(x, *self._volume_params(), self)
+        self._check_input(x)
+        return _volume_forward(self, x, None)
+
+    def _volume_params(self):
+        """the 31 parameters in the order of pmvs_volume_weights: 11 conv weights, 10 gammas, 10 betas"""
+        ws = [getattr(self, n).weight if n == "conv6_2" else getattr(self, n).conv.weight for n in _VOLUME_LAYERS]
+        bns = self._bns()
+        return ws + [bn.weight for bn in bns] + [bn.bias for bn in bns]
+
+    def _check_input(self, x):
         if x.dim() != 5 or x.dtype != torch.float32:
             raise RuntimeError("VolumeConv: input must be a float32 [B, C, D, h, w] tensor, got %s %s"
                                % (x.dtype, tuple(x.shape)))
@@ -315,18 +355,95 @@ class VolumeConv(nn.Module):
             raise RuntimeError("VolumeConv: input has %d channels, the module expects %d" % (C, self.in_channels))
         if B < 1 or min(D, H, W) < 8 or D % 8 or H % 8 or W % 8:
             raise RuntimeError("VolumeConv: D, h, w = %d, %d, %d must be positive multiples of 8" % (D, H, W))
-        bns = self._bns()
-        modes = set(bn.training or not bn.track_running_stats for bn in bns)
-        if len(modes) != 1:
-            raise RuntimeError("VolumeConv: its BatchNorm layers must all be in train mode or all in eval mode")
-        train = modes.pop()
-        if train and B * (D // 8) * (H // 8) * (W // 8) < 2:
+        if self._train_mode() and B * (D // 8) * (H // 8) * (W // 8) < 2:
             raise RuntimeError("VolumeConv: in train mode the coarsest level needs more than 1 value per channel "
                                "(B*D*h*w/512 = %d)" % (B * (D // 8) * (H // 8) * (W // 8)))
         require_cuda(x, *self.parameters())
         dev = x.device
         if any(t.device != dev for t in list(self.parameters()) + list(self.buffers())):
             raise RuntimeError("VolumeConv: the module's parameters and buffers must be on the input's device")
+
+    def _train_mode(self):
+        modes = set(bn.training or not bn.track_running_stats for bn in self._bns())
+        if len(modes) != 1:
+            raise RuntimeError("VolumeConv: its BatchNorm layers must all be in train mode or all in eval mode")
+        return modes.pop()
+
+
+def _volume_weights(mod, train, keep):
+    """pmvs_volume_weights of `mod`: fp32 contiguous copies (or the tensors themselves) appended to `keep`"""
+    def p32(t):
+        t = f32c(t.detach())
+        keep.append(t)
+        return t.data_ptr()
+
+    wt = VolumeWeights()
+    for l, name in enumerate(_VOLUME_LAYERS):
+        m = getattr(mod, name)
+        wt.weight[l] = p32(m.weight if name == "conv6_2" else m.conv.weight)
+    for l, bn in enumerate(mod._bns()):
+        wt.gamma[l], wt.beta[l], wt.eps[l] = p32(bn.weight), p32(bn.bias), float(bn.eps)
+        if not train:
+            wt.running_mean[l], wt.running_var[l] = p32(bn.running_mean), p32(bn.running_var)
+    return wt
+
+
+def _volume_forward(mod, x, ctx):
+    """pmvs_volume_conv on `x` (checked by VolumeConv._check_input); with `ctx` (an autograd context) the call gets its
+    own workspace, which is saved on it with what the backward needs."""
+    B, C, D, H, W = x.shape
+    train = mod._train_mode()
+    bns = mod._bns()
+    dev = x.device
+    keep = []
+    wt = _volume_weights(mod, train, keep)
+    xin = x.contiguous()
+    out = torch.empty(B, 1, D, H, W, device=dev, dtype=torch.float32)
+    couts = [bn.num_features for bn in bns]
+    sums = torch.empty(2 * sum(couts), device=dev, dtype=torch.float64) if train else None
+    with torch.cuda.device(dev):
+        nbytes = int(lib.pmvs_volume_conv_workspace_bytes(B, C, mod.base_channels, D, H, W))
+        if nbytes == 0:
+            check(1)
+        ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)  # the caching allocator aligns to 512 bytes
+        check(lib.pmvs_volume_conv(ptr(xin), ctypes.byref(wt), 1 if train else 0, ptr(out), ptr(sums),
+                                   ptr(ws), nbytes, B, C, mod.base_channels, D, H, W, stream_ptr()))
+    if ctx is not None:
+        ctx.x, ctx.ws, ctx.sums, ctx.train = xin, ws, sums, train
+        # eval mode normalised with the running statistics: keep copies of what the forward read
+        ctx.running = None if train else [(bn.running_mean.detach().float().clone(),
+                                           bn.running_var.detach().float().clone()) for bn in bns]
+        ctx.eps = [float(bn.eps) for bn in bns]
+    if train:
+        key = (B, D, H, W, str(dev))
+        if getattr(mod, "_pmvs_counts", (None,))[0] != key:  # one small upload per shape, not per call
+            n = torch.cat([torch.full((c,), float(B * (D >> l) * (H >> l) * (W >> l)), dtype=torch.float64)
+                           for c, l in zip(couts, _LEVEL)]).to(dev)
+            object.__setattr__(mod, "_pmvs_counts", (key, n))
+        _update_running_3d(bns, sums, couts, mod._pmvs_counts[1])
+    return out
+
+
+class _VolumeConvFn(torch.autograd.Function):
+    """VolumeConv with the fused backward (pmvs_volume_conv_backward).  Inputs are x and the module's 31 parameters
+    (11 conv weights, 10 gammas, 10 betas), so their .grad fills; the running statistics update once, in the forward."""
+
+    @staticmethod
+    def forward(ctx, x, *args):
+        params, mod = args[:-1], args[-1]
+        ctx.base_channels = mod.base_channels
+        out = _volume_forward(mod, x, ctx)
+        # x (as the kernels read it) and the parameters: an in-place change before backward trips the version check
+        ctx.save_for_backward(ctx.x, *params)
+        del ctx.x
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_out):
+        x, *params = ctx.saved_tensors
+        B, C, D, H, W = x.shape
+        dev = x.device
         keep = []
 
         def p32(t):
@@ -335,32 +452,33 @@ class VolumeConv(nn.Module):
             return t.data_ptr()
 
         wt = VolumeWeights()
-        for l, name in enumerate(_VOLUME_LAYERS):
-            m = getattr(self, name)
-            wt.weight[l] = p32(m.weight if name == "conv6_2" else m.conv.weight)
-        for l, bn in enumerate(bns):
-            wt.gamma[l], wt.beta[l], wt.eps[l] = p32(bn.weight), p32(bn.bias), float(bn.eps)
-            if not train:
-                wt.running_mean[l], wt.running_var[l] = p32(bn.running_mean), p32(bn.running_var)
-        xin = x.contiguous()
-        out = torch.empty(B, 1, D, H, W, device=dev, dtype=torch.float32)
-        couts = [bn.num_features for bn in bns]
-        sums = torch.empty(2 * sum(couts), device=dev, dtype=torch.float64) if train else None
+        for l in range(11):
+            wt.weight[l] = p32(params[l])
+        for l in range(10):
+            wt.gamma[l], wt.beta[l], wt.eps[l] = p32(params[11 + l]), p32(params[21 + l]), ctx.eps[l]
+            if not ctx.train:
+                wt.running_mean[l], wt.running_var[l] = p32(ctx.running[l][0]), p32(ctx.running[l][1])
+        need_dx = ctx.needs_input_grad[0]
+        grads = [torch.empty(p.shape, device=dev, dtype=torch.float32) for p in params]
+        g = VolumeGrads()
+        for l in range(11):
+            g.weight[l] = grads[l].data_ptr()
+        for l in range(10):
+            g.gamma[l], g.beta[l] = grads[11 + l].data_ptr(), grads[21 + l].data_ptr()
+        dy = f32c(grad_out)
         with torch.cuda.device(dev):
-            nbytes = int(lib.pmvs_volume_conv_workspace_bytes(B, C, self.base_channels, D, H, W))
+            dx = torch.empty(B, C, D, H, W, device=dev, dtype=torch.float32) if need_dx else None
+            nbytes = int(lib.pmvs_volume_conv_backward_workspace_bytes(B, C, ctx.base_channels, D, H, W))
             if nbytes == 0:
                 check(1)
-            ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)  # the caching allocator aligns to 512 bytes
-            check(lib.pmvs_volume_conv(ptr(xin), ctypes.byref(wt), 1 if train else 0, ptr(out), ptr(sums),
-                                       ptr(ws), nbytes, B, C, self.base_channels, D, H, W, stream_ptr()))
-        if train:
-            key = (B, D, H, W, str(dev))
-            if getattr(self, "_pmvs_counts", (None,))[0] != key:  # one small upload per shape, not per call
-                n = torch.cat([torch.full((c,), float(B * (D >> l) * (H >> l) * (W >> l)), dtype=torch.float64)
-                               for c, l in zip(couts, _LEVEL)]).to(dev)
-                object.__setattr__(self, "_pmvs_counts", (key, n))
-            _update_running_3d(bns, sums, couts, self._pmvs_counts[1])
-        return out
+            ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+            check(lib.pmvs_volume_conv_backward(ptr(x), ctypes.byref(wt), 1 if ctx.train else 0, ptr(ctx.ws),
+                                                ptr(ctx.sums), ptr(dy), ptr(dx), ctypes.byref(g), ptr(ws), nbytes, B,
+                                                C, ctx.base_channels, D, H, W, stream_ptr()))
+        res = [dx]
+        for i, p in enumerate(params):
+            res.append(grads[i].to(p.dtype) if ctx.needs_input_grad[1 + i] else None)
+        return tuple(res) + (None,)
 
 
 # output level of each BatchNorm layer of VolumeConv (each level halves D, h and w)
