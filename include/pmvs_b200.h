@@ -267,6 +267,47 @@ int pmvs_volume_conv(const float* x, const pmvs_volume_weights* weights, int tra
 int pmvs_coarse_depth(const float* filtered, const float* cams, int B, int V, int D, int H, int W, float* depth_out,
                       float* prob_out, pmvs_stream_t stream);
 
+/* ---- image towers: ImageConv for every view in one call (DESIGN 3.14; networks.py:84-124, model.py:71-77,133-148) */
+/* The 11 layers in module order: conv0.0, conv0.1, conv1.0, conv1.1, conv1.2, conv2.0, conv2.1, conv2.2, conv3.0,
+ * conv3.1, conv3.2.  weight[l] is the PyTorch Conv2d tensor as stored, [Cout, Cin, K, K] (K = 5 for the stride-2
+ * layers conv1.0, conv2.0, conv3.0, else 3).  The BatchNorm arrays cover the first ten layers (conv3.2 is a plain
+ * convolution); running_mean / running_var are read in eval mode only and never written. */
+typedef struct pmvs_image_weights {
+  const float* weight[11];
+  const float* gamma[10];
+  const float* beta[10];
+  const float* running_mean[10];
+  const float* running_var[10];
+  float eps[10];
+} pmvs_image_weights;
+
+/* Bytes of device workspace pmvs_image_conv needs; 0 (with pmvs_last_error) for a shape it does not serve.  With
+ * N = B*V images, level sizes h_0 = H, h_k = ceil(h_(k-1) / 2) (w alike), layer l writing C_l channels at level k_l,
+ * nb_l = ceil(h_(k_l) * ceil(w_(k_l) / px_l) / 128) CTAs per image (px_l = 8 for conv0.1, else 4) and up(n) = n
+ * rounded up to a multiple of 256:
+ *   sum_l up(4 K_l^2 Cin_l C_l)                         packed weights
+ * + 2 up(max_{l < 10} 4 N h_(k_l) w_(k_l) C_l)          two ping-pong pre-BatchNorm activations (NHWC)
+ * + up(max_{l < 10} 16 V C_l B nb_l)                    per-CTA BatchNorm partials of one layer
+ * + 2 up(512 V)                                         two ping-pong per-view scale / shift sets.
+ * The activation term is conv0's, 32 N H W bytes, so the total is about 64 B V H W bytes.  Supported:
+ * base_channels = 8, B, V >= 1, B*V <= 65535, 1 <= H, W <= 32768, H*W <= 2^28. */
+size_t pmvs_image_conv_workspace_bytes(int B, int V, int H, int W, int base_channels);
+/* img [B, V, 3, H, W] fp32 -> the feature pyramid of every view, as ImageConv run on each view img[:, v]: level_out[k]
+ * (k = 0..3 for conv0 .. conv3; NULL = not written) receives [B, V, h_k, w_k, C_k] (channels_last != 0) or
+ * [B, V, C_k, h_k, w_k] (channels_last == 0), C = 8, 16, 32, 64.  conv0 .. conv2 are ReLU(BN(.)) of their stage's last
+ * layer, conv3 the plain conv3.2.  BatchNorm uses each view's own batch statistics over (B, h, w) (train != 0; biased
+ * variance for normalising) or the running statistics (train == 0); train mode needs B*h_3*w_3 >= 2.  In train mode
+ * batch_sums (fp64 device memory, may be NULL) receives, per view v and per BatchNorm layer in the order above, the
+ * sums and then the sums of squares of that layer's convolution output over (B, h, w): row v is [sum[C_l],
+ * sumsq[C_l]] for l = 0..9, 576 doubles per view; the caller updates its running statistics from them, view by view.
+ * Zero padding applies to the activated tensor.  fp32 FMA arithmetic; reductions in a fixed order (no floating-point
+ * atomics), so two calls give the same bits.  Every argument is checked before any launch.  No allocation, no
+ * synchronisation.  workspace: pmvs_image_conv_workspace_bytes(...) bytes, 256-byte aligned, device memory; level
+ * outputs 16-byte aligned. */
+int pmvs_image_conv(const float* img, const pmvs_image_weights* weights, int train, float* const* level_out,
+                    int channels_last, double* batch_sums, void* workspace, size_t workspace_bytes, int B, int V,
+                    int H, int W, int base_channels, pmvs_stream_t stream);
+
 /* Outputs of pmvs_volume_conv_backward, PyTorch layouts, overwritten (not accumulated), like pmvs_flow_grads. */
 typedef struct pmvs_volume_grads {
   float* weight[11]; /* Conv3d [Cout, Cin, 3, 3, 3]; ConvTranspose3d (l = 7, 8, 9) [Cin, Cout, 3, 3, 3] */

@@ -58,6 +58,13 @@ class VolumeWeights(C.Structure):
     ]
 
 
+class ImageWeights(C.Structure):
+    _fields_ = [
+        ("weight", C.c_void_p * 11), ("gamma", C.c_void_p * 10), ("beta", C.c_void_p * 10),
+        ("running_mean", C.c_void_p * 10), ("running_var", C.c_void_p * 10), ("eps", C.c_float * 10),
+    ]
+
+
 class VolumeGrads(C.Structure):
     _fields_ = [("weight", C.c_void_p * 11), ("gamma", C.c_void_p * 10), ("beta", C.c_void_p * 10)]
 
@@ -106,6 +113,9 @@ _sig("pmvs_volume_conv_backward_workspace_bytes", C.c_size_t, [I, I, I, I, I, I]
 _sig("pmvs_volume_conv_backward", I, [P, C.POINTER(VolumeWeights), I, P, P, P, P, C.POINTER(VolumeGrads), P,
                                       C.c_size_t, I, I, I, I, I, I, P])
 _sig("pmvs_coarse_depth_backward", I, [P, P, P, P, I, I, I, I, I, P])
+_sig("pmvs_image_conv_workspace_bytes", C.c_size_t, [I, I, I, I, I])
+_sig("pmvs_image_conv", I, [P, C.POINTER(ImageWeights), I, C.POINTER(C.c_void_p * 4), I, P, P, C.c_size_t, I, I, I,
+                            I, I, P])
 _sig("pmvs_transpose", I, [P, P, I, I, I, P])
 _sig("pmvs_idx64_to_idx32", I, [P, P, LL, P])
 _sig("pmvs_edgeconv_pm", I, [P, I, P, P, P, P, F, I, I, P, I, P, P, I, I, I, I, I, I, P])
@@ -132,6 +142,7 @@ EXPORTED = [
     "pmvs_thin_cloud", "pmvs_nearest_distances_workspace_bytes", "pmvs_nearest_distances", "pmvs_cloud_filter",
     "pmvs_volume_conv_workspace_bytes", "pmvs_volume_conv", "pmvs_coarse_depth",
     "pmvs_volume_conv_backward_workspace_bytes", "pmvs_volume_conv_backward", "pmvs_coarse_depth_backward",
+    "pmvs_image_conv_workspace_bytes", "pmvs_image_conv",
     "pmvs_transpose", "pmvs_idx64_to_idx32", "pmvs_edgeconv_pm", "pmvs_edgeconv_pm_backward_workspace_bytes", "pmvs_edgeconv_pm_backward", "pmvs_linear_pm", "pmvs_point_flow_workspace_bytes",
     "pmvs_point_flow_iter", "pmvs_pyramid_to_channels_last", "pmvs_point_flow_debug_offsets",
     "pmvs_point_flow_debug_feature", "pmvs_point_flow_backward_workspace_bytes", "pmvs_point_flow_backward",

@@ -24,51 +24,6 @@ const char* const VC_NAMES[VC_LAYERS] = {"vc_conv0_1", "vc_conv1_0", "vc_conv2_0
 // dependency order of the forward
 const int VC_ORDER[VC_LAYERS] = {L0_1, L1_0, L1_1, L2_0, L2_1, L3_0, L3_1, L4_0, L5_0, L6_0, L6_2};
 
-// One CTA per channel: the batch statistics from the CTA partials (fixed order), or the running statistics in eval
-// mode, folded with the affine into the scale / shift the consumers apply: BN(y) = y * scale + shift.
-__global__ void __launch_bounds__(VC_FIN_THREADS)
-    vc_bn_finalize_kernel(const double* __restrict__ part, int nparts, int Cout, double count,
-                          const float* __restrict__ gamma, const float* __restrict__ beta,
-                          const float* __restrict__ rmean, const float* __restrict__ rvar, float eps,
-                          float* __restrict__ scale, float* __restrict__ shift, double* __restrict__ sums) {
-  const int c = blockIdx.x;
-  double mean, var;
-  if (part != nullptr) {
-    __shared__ double rs[VC_FIN_THREADS], rq[VC_FIN_THREADS];
-    double s = 0.0, q = 0.0;
-    for (int i = threadIdx.x; i < nparts; i += VC_FIN_THREADS) {
-      s += part[(long long)c * nparts + i];
-      q += part[(long long)(Cout + c) * nparts + i];
-    }
-    rs[threadIdx.x] = s;
-    rq[threadIdx.x] = q;
-    __syncthreads();
-    for (int o = VC_FIN_THREADS / 2; o > 0; o >>= 1) {
-      if (threadIdx.x < o) {
-        rs[threadIdx.x] += rs[threadIdx.x + o];
-        rq[threadIdx.x] += rq[threadIdx.x + o];
-      }
-      __syncthreads();
-    }
-    if (threadIdx.x != 0) return;
-    s = rs[0];
-    q = rq[0];
-    if (sums != nullptr) {
-      sums[c] = s;
-      sums[Cout + c] = q;
-    }
-    mean = s / count;
-    var = fmax(q / count - mean * mean, 0.0);  // biased, for normalising (as nn.BatchNorm3d in train mode)
-  } else {
-    if (threadIdx.x != 0) return;
-    mean = (double)rmean[c];
-    var = (double)rvar[c];
-  }
-  const double sc = (double)gamma[c] / sqrt(var + (double)eps);
-  scale[c] = (float)sc;
-  shift[c] = (float)((double)beta[c] - mean * sc);
-}
-
 // PyTorch layouts -> [Cin][27][Cout] for every layer in one launch
 struct VcPack {
   const float* src[VC_LAYERS];
@@ -233,7 +188,7 @@ extern "C" int pmvs_volume_conv(const float* x, const pmvs_volume_weights* wt, i
     prof_begin("vc_bn_finalize", st);
     vc_bn_finalize_kernel<<<q.cout, VC_FIN_THREADS, 0, st>>>(
         a.part, (int)q.nparts, q.cout, count, wt->gamma[l], wt->beta[l], wt->running_mean[l], wt->running_var[l],
-        wt->eps[l], scale, scale + q.cout, (train && batch_sums) ? batch_sums + sums_at[l] : nullptr);
+        wt->eps[l], scale, scale + q.cout, (train && batch_sums) ? batch_sums + sums_at[l] : nullptr, 0);
     PMVS_TRY(check_launch("vc_bn_finalize_kernel", st));
   }
   return PMVS_OK;

@@ -195,6 +195,58 @@ __device__ __forceinline__ float linspace_at(float start, float end, float step,
   return __fmaf_rn(-step, (float)(D - 1 - i), end);
 }
 
+// One CTA per (channel, view = blockIdx.y): the batch statistics from the CTA partials (fixed order), or the running
+// statistics in eval mode, folded with the affine into the scale / shift the consumers apply: BN(y) = y * scale +
+// shift.  View v reads part + v * 2 * Cout * nparts and writes scale / shift + v * Cout and sums + v * sums_stride;
+// VolumeConv launches one view, ImageConv one per view (each view's BatchNorm has its own batch statistics).
+__global__ void __launch_bounds__(VC_FIN_THREADS)
+    vc_bn_finalize_kernel(const double* __restrict__ part, int nparts, int Cout, double count,
+                          const float* __restrict__ gamma, const float* __restrict__ beta,
+                          const float* __restrict__ rmean, const float* __restrict__ rvar, float eps,
+                          float* __restrict__ scale, float* __restrict__ shift, double* __restrict__ sums,
+                          long long sums_stride) {
+  const int c = blockIdx.x, v = blockIdx.y;
+  scale += (long long)v * Cout;
+  shift += (long long)v * Cout;
+  if (sums != nullptr) sums += (long long)v * sums_stride;
+  double mean, var;
+  if (part != nullptr) {
+    __shared__ double rs[VC_FIN_THREADS], rq[VC_FIN_THREADS];
+    double s = 0.0, q = 0.0;
+    part += (long long)v * 2 * Cout * nparts;
+    for (int i = threadIdx.x; i < nparts; i += VC_FIN_THREADS) {
+      s += part[(long long)c * nparts + i];
+      q += part[(long long)(Cout + c) * nparts + i];
+    }
+    rs[threadIdx.x] = s;
+    rq[threadIdx.x] = q;
+    __syncthreads();
+    for (int o = VC_FIN_THREADS / 2; o > 0; o >>= 1) {
+      if (threadIdx.x < o) {
+        rs[threadIdx.x] += rs[threadIdx.x + o];
+        rq[threadIdx.x] += rq[threadIdx.x + o];
+      }
+      __syncthreads();
+    }
+    if (threadIdx.x != 0) return;
+    s = rs[0];
+    q = rq[0];
+    if (sums != nullptr) {
+      sums[c] = s;
+      sums[Cout + c] = q;
+    }
+    mean = s / count;
+    var = fmax(q / count - mean * mean, 0.0);  // biased, for normalising (as nn.BatchNorm3d in train mode)
+  } else {
+    if (threadIdx.x != 0) return;
+    mean = (double)rmean[c];
+    var = (double)rvar[c];
+  }
+  const double sc = (double)gamma[c] / sqrt(var + (double)eps);
+  scale[c] = (float)sc;
+  shift[c] = (float)((double)beta[c] - mean * sc);
+}
+
 inline size_t up256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 struct VcLayerPlan {

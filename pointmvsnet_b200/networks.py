@@ -13,7 +13,7 @@ import torch
 import torch.nn as nn
 from torch.autograd.function import once_differentiable
 
-from ._lib import lib, check, stream_ptr, ptr, require_cuda, f32c, VolumeWeights, VolumeGrads
+from ._lib import lib, check, stream_ptr, ptr, require_cuda, f32c, ImageWeights, VolumeWeights, VolumeGrads
 from .nn.conv import Conv2d, Conv3d, Deconv3d
 
 _SUPPORTED_COUT = (16, 32, 64, 128)
@@ -238,7 +238,10 @@ class ImageConv(nn.Module):
     once to NHWC, every layer runs in that format, and ``conv1 / conv2 / conv3`` come out as [B,C,h,w] tensors whose
     memory is [B,h,w,C] - the layout the fetch kernels read.  ``stack_views_channels_last`` then replaces the
     ``torch.stack(dim=1)`` of model.py:144-145 with a copy into one [B,V,h,w,C] buffer per level (the same bytes the
-    stack moves), and ``PointFlow`` consumes the result zero-copy: the three ``transpose`` launches per pass vanish."""
+    stack moves), and ``PointFlow`` consumes the result zero-copy: the three ``transpose`` launches per pass vanish.
+
+    ``forward_views`` runs every view at once on the library's own kernels (``pmvs_image_conv``, DESIGN 3.14) and
+    returns the stacked pyramids directly; it is forward-only, so ``forward`` stays the path under autograd."""
 
     def __init__(self, base_channels, channels_last=True):
         super().__init__()
@@ -262,6 +265,94 @@ class ImageConv(nn.Module):
             out[name] = x
         return out
 
+    def forward_views(self, img_list, keys=("conv1", "conv2", "conv3"), out=None):
+        """Every view's pyramid in one ``pmvs_image_conv`` call (fp32 direct convolutions on sm_90a, DESIGN 3.14):
+        img_list [B, V, 3, H, W] -> {key: [B, V, C, h, w]} for the requested levels (any of ``conv0`` .. ``conv3``).
+
+        Equivalent to ``self(img_list[:, v])`` for each view, stacked along dim 1, side effects included: in train
+        mode each view's BatchNorm uses that view's batch statistics over (B, h, w), and the running statistics and
+        ``num_batches_tracked`` get V sequential updates in view order, each layer with its own momentum and eps
+        (``momentum=None``: the cumulative average); in eval mode the running statistics are used and left alone.
+        The memory layout follows ``channels_last``: [B, V, h, w, C] (what ``stack_views_channels_last`` produces and
+        ``PointFlow.pyramids_to_channels_last`` passes through) or contiguous [B, V, C, h, w] (what
+        ``cost_volume.build_cost_volume`` reads).  ``out`` ({key: buffer in that layout}) lets a caller reuse the
+        buffers across passes.  No host synchronisation once a shape has been seen.
+
+        Supported: base_channels = 8, any H, W >= 1 (stride-2 layers give ceil(n / 2)).  Forward only: with grad
+        enabled and the input or a parameter requiring grad it raises ``NotImplementedError``; ``forward`` (one view
+        at a time, stock convolutions) is the path under autograd."""
+        if torch.is_grad_enabled() and (img_list.requires_grad or any(p.requires_grad for p in self.parameters())):
+            raise NotImplementedError("ImageConv.forward_views is forward-only; wrap the call in torch.no_grad() or "
+                                      "run the per-view ImageConv.forward under autograd")
+        if self.base_channels != 8:
+            raise RuntimeError("ImageConv.forward_views: base_channels = %d is not supported; the fused kernels "
+                               "serve 8" % self.base_channels)
+        if img_list.dim() != 5 or img_list.shape[2] != 3 or img_list.dtype != torch.float32:
+            raise RuntimeError("ImageConv.forward_views: img_list must be a float32 [B, V, 3, H, W] tensor, got %s %s"
+                               % (img_list.dtype, tuple(img_list.shape)))
+        keys = tuple(keys)
+        if not set(keys) <= set(_IMAGE_LEVELS):
+            raise RuntimeError("ImageConv.forward_views: keys %s must be among %s" % (keys, _IMAGE_LEVELS))
+        B, V, _, H, W = img_list.shape
+        if min(B, V, H, W) < 1:
+            raise RuntimeError("ImageConv.forward_views: empty input %s" % (tuple(img_list.shape),))
+        convs, bns = self._image_layers()
+        train = _bn_train_mode(bns, "ImageConv")
+        hs, ws = [H], [W]
+        for _ in range(3):
+            hs.append((hs[-1] + 1) // 2)
+            ws.append((ws[-1] + 1) // 2)
+        if train and B * hs[3] * ws[3] < 2:
+            raise RuntimeError("ImageConv.forward_views: in train mode the coarsest level needs more than 1 value per "
+                               "channel (B*h3*w3 = %d)" % (B * hs[3] * ws[3]))
+        require_cuda(img_list, *self.parameters())
+        dev = img_list.device
+        if any(t.device != dev for t in list(self.parameters()) + list(self.buffers())):
+            raise RuntimeError("ImageConv.forward_views: the module's parameters and buffers must be on the input's "
+                               "device")
+        res, bufs = {}, [None] * 4
+        for k in keys:
+            lev = _IMAGE_LEVELS.index(k)
+            C, h, w = 8 << lev, hs[lev], ws[lev]
+            shape = (B, V, h, w, C) if self.channels_last else (B, V, C, h, w)
+            if out is not None and k in out:
+                buf = out[k]
+                if (tuple(buf.shape) != shape or buf.dtype != torch.float32 or buf.device != dev
+                        or not buf.is_contiguous()):
+                    raise RuntimeError("ImageConv.forward_views: out[%r] must be a contiguous float32 %s tensor on %s"
+                                       % (k, shape, dev))
+            else:
+                buf = torch.empty(shape, device=dev, dtype=torch.float32)
+            bufs[lev] = buf
+            res[k] = buf.permute(0, 1, 4, 2, 3) if self.channels_last else buf
+        keep = []
+        wt = _conv_bn_weights(ImageWeights(), [c.weight for c in convs], bns, train, keep)
+        img = img_list.contiguous()
+        couts = [bn.num_features for bn in bns]
+        sums = torch.empty(V, 2 * sum(couts), device=dev, dtype=torch.float64) if train else None
+        levels = (ctypes.c_void_p * 4)(*[ptr(b) for b in bufs])
+        with torch.cuda.device(dev):
+            nbytes = int(lib.pmvs_image_conv_workspace_bytes(B, V, H, W, self.base_channels))
+            if nbytes == 0:
+                check(1)
+            wsp = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+            check(lib.pmvs_image_conv(ptr(img), ctypes.byref(wt), 1 if train else 0, ctypes.byref(levels),
+                                      1 if self.channels_last else 0, ptr(sums), ptr(wsp), nbytes, B, V, H, W,
+                                      self.base_channels, stream_ptr()))
+        if train:
+            key = (B, H, W, str(dev))
+            if getattr(self, "_pmvs_counts", (None,))[0] != key:  # one small upload per shape, not per call
+                n = torch.cat([torch.full((c,), float(B * hs[l] * ws[l]), dtype=torch.float64)
+                               for c, l in zip(couts, _IMAGE_LEVEL)]).to(dev)
+                object.__setattr__(self, "_pmvs_counts", (key, n))
+            _update_running_rows(bns, sums, couts, self._pmvs_counts[1])
+        return res
+
+    def _image_layers(self):
+        """the 11 convolutions in the order of pmvs_image_weights and the 10 BatchNorm layers"""
+        mods = list(self.conv0) + list(self.conv1) + list(self.conv2) + list(self.conv3)
+        return [m if isinstance(m, nn.Conv2d) else m.conv for m in mods], [m.bn for m in mods[:10]]
+
 
 def stack_views_channels_last(per_view, keys=("conv1", "conv2", "conv3"), out=None):
     """model.py:137-145 (``torch.stack`` of the per-view pyramids along dim 1) for a channels-last producer.
@@ -279,6 +370,20 @@ def stack_views_channels_last(per_view, keys=("conv1", "conv2", "conv3"), out=No
             buf[:, v].copy_(d[k].permute(0, 2, 3, 1))  # NHWC -> NHWC: a plain contiguous copy for a channels-last source
         res[k] = buf.permute(0, 1, 4, 2, 3)
     return res
+
+
+# the pyramid levels ImageConv hands out and the level (each halves h and w) of each of its BatchNorm layers
+_IMAGE_LEVELS = ("conv0", "conv1", "conv2", "conv3")
+_IMAGE_LEVEL = (0, 0, 1, 1, 1, 2, 2, 2, 3, 3)
+
+
+def _bn_train_mode(bns, what):
+    """True for batch statistics (train mode, or no running statistics), False for the running statistics; the
+    layers must agree."""
+    modes = set(bn.training or not bn.track_running_stats for bn in bns)
+    if len(modes) != 1:
+        raise RuntimeError("%s: its BatchNorm layers must all be in train mode or all in eval mode" % what)
+    return modes.pop()
 
 
 # the layers of VolumeConv in the order of pmvs_volume_weights (include/pmvs_b200.h)
@@ -364,28 +469,30 @@ class VolumeConv(nn.Module):
             raise RuntimeError("VolumeConv: the module's parameters and buffers must be on the input's device")
 
     def _train_mode(self):
-        modes = set(bn.training or not bn.track_running_stats for bn in self._bns())
-        if len(modes) != 1:
-            raise RuntimeError("VolumeConv: its BatchNorm layers must all be in train mode or all in eval mode")
-        return modes.pop()
+        return _bn_train_mode(self._bns(), "VolumeConv")
 
 
-def _volume_weights(mod, train, keep):
-    """pmvs_volume_weights of `mod`: fp32 contiguous copies (or the tensors themselves) appended to `keep`"""
+def _conv_bn_weights(wt, weights, bns, train, keep):
+    """fill `wt` (pmvs_volume_weights or pmvs_image_weights) from the conv weights and BatchNorm layers: fp32
+    contiguous copies (or the tensors themselves) appended to `keep`"""
     def p32(t):
         t = f32c(t.detach())
         keep.append(t)
         return t.data_ptr()
 
-    wt = VolumeWeights()
-    for l, name in enumerate(_VOLUME_LAYERS):
-        m = getattr(mod, name)
-        wt.weight[l] = p32(m.weight if name == "conv6_2" else m.conv.weight)
-    for l, bn in enumerate(mod._bns()):
+    for l, w in enumerate(weights):
+        wt.weight[l] = p32(w)
+    for l, bn in enumerate(bns):
         wt.gamma[l], wt.beta[l], wt.eps[l] = p32(bn.weight), p32(bn.bias), float(bn.eps)
         if not train:
             wt.running_mean[l], wt.running_var[l] = p32(bn.running_mean), p32(bn.running_var)
     return wt
+
+
+def _volume_weights(mod, train, keep):
+    """pmvs_volume_weights of `mod`"""
+    weights = [getattr(mod, n).weight if n == "conv6_2" else getattr(mod, n).conv.weight for n in _VOLUME_LAYERS]
+    return _conv_bn_weights(VolumeWeights(), weights, mod._bns(), train, keep)
 
 
 def _volume_forward(mod, x, ctx):
@@ -420,7 +527,7 @@ def _volume_forward(mod, x, ctx):
             n = torch.cat([torch.full((c,), float(B * (D >> l) * (H >> l) * (W >> l)), dtype=torch.float64)
                            for c, l in zip(couts, _LEVEL)]).to(dev)
             object.__setattr__(mod, "_pmvs_counts", (key, n))
-        _update_running_3d(bns, sums, couts, mod._pmvs_counts[1])
+        _update_running_rows(bns, sums, couts, mod._pmvs_counts[1])
     return out
 
 
@@ -485,27 +592,30 @@ class _VolumeConvFn(torch.autograd.Function):
 _LEVEL = (0, 1, 2, 3, 1, 2, 3, 2, 1, 0)
 
 
-def _update_running_3d(bns, sums, couts, n):
-    """nn.BatchNorm3d's train-mode side effect for every layer, from the fp64 batch sums [sum; sumsq] per layer and
-    the per-channel value counts n (device); without a host read (momentum=None: the cumulative average
-    1 / num_batches_tracked)."""
-    s = torch.cat([sums[2 * o:2 * o + 2 * c].view(2, c) for o, c in zip(_offsets(couts), couts)], dim=1)
-    mean = s[0] / n
-    var = ((s[1] / n - mean * mean).clamp_(min=0) * (n / (n - 1.0))).float()
+def _update_running_rows(bns, sums, couts, n):
+    """BatchNorm's train-mode side effect for every layer, from the fp64 batch sums [sum; sumsq] per layer and the
+    per-channel value counts n (device); without a host read (momentum=None: the cumulative average
+    1 / num_batches_tracked).  sums is one row [2 * sum(couts)] (VolumeConv) or one row per view [V, 2 * sum(couts)]
+    (ImageConv.forward_views); each row is one update, in row order, as V separate calls make them."""
+    rows = sums.view(-1, sums.shape[-1])
+    s = torch.cat([rows[:, 2 * o:2 * o + 2 * c].view(-1, 2, c) for o, c in zip(_offsets(couts), couts)], dim=2)
+    mean = s[:, 0] / n
+    var = ((s[:, 1] / n - mean * mean).clamp_(min=0) * (n / (n - 1.0))).float()
     mean = mean.float()
-    off = 0
-    for bn, c in zip(bns, couts):
-        if bn.track_running_stats and bn.running_mean is not None:
-            bn.num_batches_tracked.add_(1)
-            m, v = mean[off:off + c], var[off:off + c]
-            if bn.momentum is None:
-                f = 1.0 / bn.num_batches_tracked.float()
-                bn.running_mean.add_((m - bn.running_mean) * f)
-                bn.running_var.add_((v - bn.running_var) * f)
-            else:
-                bn.running_mean.mul_(1 - bn.momentum).add_(m, alpha=bn.momentum)
-                bn.running_var.mul_(1 - bn.momentum).add_(v, alpha=bn.momentum)
-        off += c
+    for r in range(rows.shape[0]):
+        off = 0
+        for bn, c in zip(bns, couts):
+            if bn.track_running_stats and bn.running_mean is not None:
+                bn.num_batches_tracked.add_(1)
+                m, v = mean[r, off:off + c], var[r, off:off + c]
+                if bn.momentum is None:
+                    f = 1.0 / bn.num_batches_tracked.float()
+                    bn.running_mean.add_((m - bn.running_mean) * f)
+                    bn.running_var.add_((v - bn.running_var) * f)
+                else:
+                    bn.running_mean.mul_(1 - bn.momentum).add_(m, alpha=bn.momentum)
+                    bn.running_var.mul_(1 - bn.momentum).add_(v, alpha=bn.momentum)
+            off += c
 
 
 def _offsets(couts):
