@@ -308,6 +308,58 @@ int pmvs_image_conv(const float* img, const pmvs_image_weights* weights, int tra
                     int channels_last, double* batch_sums, void* workspace, size_t workspace_bytes, int B, int V,
                     int H, int W, int base_channels, pmvs_stream_t stream);
 
+/* The forward of a training step (DESIGN 3.15): pmvs_image_conv with the same arguments, the same launches on the same
+ * plan and bit-identical level outputs and batch sums, but a workspace that keeps what pmvs_image_conv_backward reads:
+ * every BatchNorm layer's pre-BatchNorm output (NHWC) and per-view scale / shift at its own offset and, in eval mode,
+ * a copy of the running statistics it normalised with (one more launch).  Bytes, with the notation above and
+ * P_l = h_(k_l) w_(k_l):
+ *   sum_l up(4 K_l^2 Cin_l C_l)                          packed weights (as pmvs_image_conv)
+ * + sum_{l < 10} [up(4 N P_l C_l) + up(8 V C_l)]          each layer's pre-BatchNorm output and scale / shift
+ * + up(max_{l < 10} 16 V C_l B nb_l)                     per-CTA BatchNorm partials of one layer
+ * + up(2304)                                             the running statistics of eval mode (576 floats).
+ * The activation term is (64 + 48 + 24 + 8) N H W, about 144 B V H W bytes: 566 MB at B = 4, V = 3, 512 x 640. */
+size_t pmvs_image_conv_keep_workspace_bytes(int B, int V, int H, int W, int base_channels);
+int pmvs_image_conv_keep(const float* img, const pmvs_image_weights* weights, int train, float* const* level_out,
+                         int channels_last, double* batch_sums, void* workspace, size_t workspace_bytes, int B, int V,
+                         int H, int W, int base_channels, pmvs_stream_t stream);
+
+/* Outputs of pmvs_image_conv_backward, PyTorch layouts, overwritten (not accumulated), like pmvs_volume_grads. */
+typedef struct pmvs_image_grads {
+  float* weight[11]; /* Conv2d [Cout, Cin, K, K] */
+  float* gamma[10];
+  float* beta[10];
+} pmvs_image_grads;
+
+/* Bytes of device workspace pmvs_image_conv_backward needs; 0 (with pmvs_last_error) for a shape the forward does not
+ * take.  With the notation above, E_l = K_l^2 Cin_l C_l the weights of layer l, and
+ * n_l = max(1, min(ceil(4224 / (K_l q_l (C_l / 8) N)), ceil(P_l / 1024))) the weight-gradient chunks per image, where
+ * q_l = 1 for conv0.0 and Cin_l / 4 otherwise (chunks of c_l = ceil(P_l / n_l) output pixels, ceil(P_l / c_l) of them):
+ *   sum_{l >= 1} up(4 E_l)                               packed data-gradient weights
+ * + 2 up(max_l 4 N P_l C_l)                              two gradient buffers, conv0's 32 N H W bytes each
+ * + up(max_{l < 10} 16 V C_l B ceil(P_l / max(1, 16384 / C_l)))   BatchNorm-backward partials
+ * + up(1024 V)                                           per-view constants of G
+ * + up(max_l 8 E_l N ceil(P_l / c_l))                    weight-gradient partials.
+ * About 64 B V H W bytes plus the partials: 262 MB at B = 4, V = 3, 512 x 640. */
+size_t pmvs_image_conv_backward_workspace_bytes(int B, int V, int H, int W, int base_channels);
+/* Gradients of one pmvs_image_conv_keep call.  grad_level[k] (k = 0..3) is the gradient of level k in the layout the
+ * forward wrote it ([B, V, h_k, w_k, C_k] with channels_last != 0, else [B, V, C_k, h_k, w_k]), 16-byte aligned; NULL
+ * means zero.  Every gradient in grads is written: a layer that no given level depends on (above the coarsest level
+ * with a gradient) gets zeros, and its kernels are not launched.  The images get no gradient.  fwd_workspace is that
+ * call's workspace, with the same shapes, weights and train flag, not modified since; it is only read, so the call can
+ * be repeated.  The ReLU masks and the scale of eval mode are the forward's own kept scale / shift; batch_sums (that
+ * call's output, required in train mode) gives each view's batch statistics, and eval mode uses the forward's kept
+ * copy of the running statistics: weights->running_mean / running_var are not read, so an update of the module's
+ * buffers between forward and backward changes nothing.  Padding gets no gradient.  Per view v, train mode:
+ * G = gamma invstd_v (dz - sum dz / n - xhat sum dz xhat / n), eval: G = scale dz; dgamma = sum_v sum dz xhat and
+ * dbeta = sum_v sum dz, added in view order.  Every argument is checked before any launch.  fp32 FMA products; per-CTA
+ * and final sums in a fixed order (fp64 across threads and CTAs), no floating-point atomics, so two calls give the same
+ * bits.  No allocation, no synchronisation.  workspace: pmvs_image_conv_backward_workspace_bytes(...) bytes, 256-byte
+ * aligned, device memory (as is fwd_workspace). */
+int pmvs_image_conv_backward(const float* img, const pmvs_image_weights* weights, int train, const void* fwd_workspace,
+                             const double* batch_sums, const float* const* grad_level, int channels_last,
+                             const pmvs_image_grads* grads, void* workspace, size_t workspace_bytes, int B, int V,
+                             int H, int W, int base_channels, pmvs_stream_t stream);
+
 /* Outputs of pmvs_volume_conv_backward, PyTorch layouts, overwritten (not accumulated), like pmvs_flow_grads. */
 typedef struct pmvs_volume_grads {
   float* weight[11]; /* Conv3d [Cout, Cin, 3, 3, 3]; ConvTranspose3d (l = 7, 8, 9) [Cin, Cout, 3, 3, 3] */

@@ -69,6 +69,10 @@ class VolumeGrads(C.Structure):
     _fields_ = [("weight", C.c_void_p * 11), ("gamma", C.c_void_p * 10), ("beta", C.c_void_p * 10)]
 
 
+class ImageGrads(C.Structure):
+    _fields_ = [("weight", C.c_void_p * 11), ("gamma", C.c_void_p * 10), ("beta", C.c_void_p * 10)]
+
+
 def _sig(name, restype, argtypes):
     fn = getattr(lib, name)
     fn.restype = restype
@@ -116,6 +120,12 @@ _sig("pmvs_coarse_depth_backward", I, [P, P, P, P, I, I, I, I, I, P])
 _sig("pmvs_image_conv_workspace_bytes", C.c_size_t, [I, I, I, I, I])
 _sig("pmvs_image_conv", I, [P, C.POINTER(ImageWeights), I, C.POINTER(C.c_void_p * 4), I, P, P, C.c_size_t, I, I, I,
                             I, I, P])
+_sig("pmvs_image_conv_keep_workspace_bytes", C.c_size_t, [I, I, I, I, I])
+_sig("pmvs_image_conv_keep", I, [P, C.POINTER(ImageWeights), I, C.POINTER(C.c_void_p * 4), I, P, P, C.c_size_t, I,
+                                 I, I, I, I, P])
+_sig("pmvs_image_conv_backward_workspace_bytes", C.c_size_t, [I, I, I, I, I])
+_sig("pmvs_image_conv_backward", I, [P, C.POINTER(ImageWeights), I, P, P, C.POINTER(C.c_void_p * 4), I,
+                                     C.POINTER(ImageGrads), P, C.c_size_t, I, I, I, I, I, P])
 _sig("pmvs_transpose", I, [P, P, I, I, I, P])
 _sig("pmvs_idx64_to_idx32", I, [P, P, LL, P])
 _sig("pmvs_edgeconv_pm", I, [P, I, P, P, P, P, F, I, I, P, I, P, P, I, I, I, I, I, I, P])
@@ -142,7 +152,8 @@ EXPORTED = [
     "pmvs_thin_cloud", "pmvs_nearest_distances_workspace_bytes", "pmvs_nearest_distances", "pmvs_cloud_filter",
     "pmvs_volume_conv_workspace_bytes", "pmvs_volume_conv", "pmvs_coarse_depth",
     "pmvs_volume_conv_backward_workspace_bytes", "pmvs_volume_conv_backward", "pmvs_coarse_depth_backward",
-    "pmvs_image_conv_workspace_bytes", "pmvs_image_conv",
+    "pmvs_image_conv_workspace_bytes", "pmvs_image_conv", "pmvs_image_conv_keep_workspace_bytes",
+    "pmvs_image_conv_keep", "pmvs_image_conv_backward_workspace_bytes", "pmvs_image_conv_backward",
     "pmvs_transpose", "pmvs_idx64_to_idx32", "pmvs_edgeconv_pm", "pmvs_edgeconv_pm_backward_workspace_bytes", "pmvs_edgeconv_pm_backward", "pmvs_linear_pm", "pmvs_point_flow_workspace_bytes",
     "pmvs_point_flow_iter", "pmvs_pyramid_to_channels_last", "pmvs_point_flow_debug_offsets",
     "pmvs_point_flow_debug_feature", "pmvs_point_flow_backward_workspace_bytes", "pmvs_point_flow_backward",

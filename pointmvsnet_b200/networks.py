@@ -13,12 +13,14 @@ import torch
 import torch.nn as nn
 from torch.autograd.function import once_differentiable
 
-from ._lib import lib, check, stream_ptr, ptr, require_cuda, f32c, ImageWeights, VolumeWeights, VolumeGrads
+from ._lib import (lib, check, stream_ptr, ptr, require_cuda, f32c, ImageGrads, ImageWeights, VolumeWeights,
+                   VolumeGrads)
 from .nn.conv import Conv2d, Conv3d, Deconv3d
 
 _SUPPORTED_COUT = (16, 32, 64, 128)
 _backward_enabled = False
 _volume_backward_enabled = False
+_image_backward_enabled = False
 
 
 def enable_backward(enabled=True):
@@ -58,6 +60,28 @@ def enable_volume_backward(enabled=True):
 
 def volume_backward_enabled():
     return _volume_backward_enabled
+
+
+def enable_image_backward(enabled=True):
+    """Process-wide switch for the image towers: while on, ``ImageConv.forward_views`` called with grad enabled and a
+    parameter requiring grad runs through an autograd Function whose backward is the fused, deterministic CUDA
+    backward (``pmvs_image_conv_backward``, DESIGN 3.15); while off (the default) such calls raise
+    ``NotImplementedError``.  Returns the previous setting.  ``enable_backward()`` and ``enable_volume_backward()`` do
+    not cover it.
+
+    It is opt-in because a grad-enabled ``forward_views`` keeps its whole workspace
+    (``pmvs_image_conv_keep_workspace_bytes``: every BatchNorm layer's pre-BatchNorm output, about 144 * B * V * H * W
+    bytes, 566 MB per tower at B = 4, V = 3, 512 x 640) alive until backward runs; the backward then allocates its own
+    workspace (``pmvs_image_conv_backward_workspace_bytes``, about 64 * B * V * H * W bytes) for the duration of the
+    call.  Under ``torch.no_grad()`` the switch has no effect."""
+    global _image_backward_enabled
+    prev = _image_backward_enabled
+    _image_backward_enabled = bool(enabled)
+    return prev
+
+
+def image_backward_enabled():
+    return _image_backward_enabled
 
 
 def _edge_layer(mod, feature, knn_inds, concat_central):
@@ -241,7 +265,8 @@ class ImageConv(nn.Module):
     stack moves), and ``PointFlow`` consumes the result zero-copy: the three ``transpose`` launches per pass vanish.
 
     ``forward_views`` runs every view at once on the library's own kernels (``pmvs_image_conv``, DESIGN 3.14) and
-    returns the stacked pyramids directly; it is forward-only, so ``forward`` stays the path under autograd."""
+    returns the stacked pyramids directly.  Under autograd it needs ``enable_image_backward()``: then its backward is
+    the library's too (``pmvs_image_conv_backward``, DESIGN 3.15), and the towers train without the per-view path."""
 
     def __init__(self, base_channels, channels_last=True):
         super().__init__()
@@ -278,12 +303,34 @@ class ImageConv(nn.Module):
         ``cost_volume.build_cost_volume`` reads).  ``out`` ({key: buffer in that layout}) lets a caller reuse the
         buffers across passes.  No host synchronisation once a shape has been seen.
 
-        Supported: base_channels = 8, any H, W >= 1 (stride-2 layers give ceil(n / 2)).  Forward only: with grad
-        enabled and the input or a parameter requiring grad it raises ``NotImplementedError``; ``forward`` (one view
-        at a time, stock convolutions) is the path under autograd."""
-        if torch.is_grad_enabled() and (img_list.requires_grad or any(p.requires_grad for p in self.parameters())):
-            raise NotImplementedError("ImageConv.forward_views is forward-only; wrap the call in torch.no_grad() or "
-                                      "run the per-view ImageConv.forward under autograd")
+        Supported: base_channels = 8, any H, W >= 1 (stride-2 layers give ceil(n / 2)).  With grad enabled and the
+        input or a parameter requiring grad it raises ``NotImplementedError`` unless ``enable_image_backward()`` is
+        on.  While it is on, a parameter requiring grad makes the call run through an autograd Function whose
+        backward is the fused, deterministic ``pmvs_image_conv_backward`` (DESIGN 3.15): the outputs are the same
+        bits as the ``no_grad`` call's, the running statistics update once, in the forward, and ``backward`` fills
+        the ``.grad`` of every parameter a level with a gradient depends on (the others keep ``None``, as the stock
+        graph leaves them).  The images get no gradient: ``img_list`` requiring grad, and ``out=``, are refused
+        there with ``RuntimeError``.  ``forward`` (one view at a time, stock convolutions) also runs under
+        autograd."""
+        grad = torch.is_grad_enabled() and (img_list.requires_grad or any(p.requires_grad for p in self.parameters()))
+        if grad:
+            if not _image_backward_enabled:
+                raise NotImplementedError("ImageConv.forward_views is forward-only; wrap the call in torch.no_grad() "
+                                          "or run the per-view ImageConv.forward under autograd")
+            if img_list.requires_grad:
+                raise RuntimeError("ImageConv.forward_views: the images get no gradient; pass img_list without "
+                                   "requires_grad")
+            if out is not None:
+                raise RuntimeError("ImageConv.forward_views: out= is not supported with grad enabled (the outputs "
+                                   "are autograd's)")
+        keys = self._check_views(img_list, keys)
+        if grad:
+            bufs = _ImageConvFn.apply(img_list, self, keys, *self._image_params())
+            return {k: b.permute(0, 1, 4, 2, 3) if self.channels_last else b for k, b in zip(keys, bufs)}
+        return _image_forward(self, img_list, keys, out, None)
+
+    def _check_views(self, img_list, keys):
+        """the argument checks of forward_views (before any launch); returns keys as a tuple"""
         if self.base_channels != 8:
             raise RuntimeError("ImageConv.forward_views: base_channels = %d is not supported; the fused kernels "
                                "serve 8" % self.base_channels)
@@ -296,57 +343,23 @@ class ImageConv(nn.Module):
         B, V, _, H, W = img_list.shape
         if min(B, V, H, W) < 1:
             raise RuntimeError("ImageConv.forward_views: empty input %s" % (tuple(img_list.shape),))
-        convs, bns = self._image_layers()
+        _, bns = self._image_layers()
         train = _bn_train_mode(bns, "ImageConv")
-        hs, ws = [H], [W]
-        for _ in range(3):
-            hs.append((hs[-1] + 1) // 2)
-            ws.append((ws[-1] + 1) // 2)
-        if train and B * hs[3] * ws[3] < 2:
+        h3, w3 = _level_sizes(H, W)[3]
+        if train and B * h3 * w3 < 2:
             raise RuntimeError("ImageConv.forward_views: in train mode the coarsest level needs more than 1 value per "
-                               "channel (B*h3*w3 = %d)" % (B * hs[3] * ws[3]))
+                               "channel (B*h3*w3 = %d)" % (B * h3 * w3))
         require_cuda(img_list, *self.parameters())
         dev = img_list.device
         if any(t.device != dev for t in list(self.parameters()) + list(self.buffers())):
             raise RuntimeError("ImageConv.forward_views: the module's parameters and buffers must be on the input's "
                                "device")
-        res, bufs = {}, [None] * 4
-        for k in keys:
-            lev = _IMAGE_LEVELS.index(k)
-            C, h, w = 8 << lev, hs[lev], ws[lev]
-            shape = (B, V, h, w, C) if self.channels_last else (B, V, C, h, w)
-            if out is not None and k in out:
-                buf = out[k]
-                if (tuple(buf.shape) != shape or buf.dtype != torch.float32 or buf.device != dev
-                        or not buf.is_contiguous()):
-                    raise RuntimeError("ImageConv.forward_views: out[%r] must be a contiguous float32 %s tensor on %s"
-                                       % (k, shape, dev))
-            else:
-                buf = torch.empty(shape, device=dev, dtype=torch.float32)
-            bufs[lev] = buf
-            res[k] = buf.permute(0, 1, 4, 2, 3) if self.channels_last else buf
-        keep = []
-        wt = _conv_bn_weights(ImageWeights(), [c.weight for c in convs], bns, train, keep)
-        img = img_list.contiguous()
-        couts = [bn.num_features for bn in bns]
-        sums = torch.empty(V, 2 * sum(couts), device=dev, dtype=torch.float64) if train else None
-        levels = (ctypes.c_void_p * 4)(*[ptr(b) for b in bufs])
-        with torch.cuda.device(dev):
-            nbytes = int(lib.pmvs_image_conv_workspace_bytes(B, V, H, W, self.base_channels))
-            if nbytes == 0:
-                check(1)
-            wsp = torch.empty(nbytes, device=dev, dtype=torch.uint8)
-            check(lib.pmvs_image_conv(ptr(img), ctypes.byref(wt), 1 if train else 0, ctypes.byref(levels),
-                                      1 if self.channels_last else 0, ptr(sums), ptr(wsp), nbytes, B, V, H, W,
-                                      self.base_channels, stream_ptr()))
-        if train:
-            key = (B, H, W, str(dev))
-            if getattr(self, "_pmvs_counts", (None,))[0] != key:  # one small upload per shape, not per call
-                n = torch.cat([torch.full((c,), float(B * hs[l] * ws[l]), dtype=torch.float64)
-                               for c, l in zip(couts, _IMAGE_LEVEL)]).to(dev)
-                object.__setattr__(self, "_pmvs_counts", (key, n))
-            _update_running_rows(bns, sums, couts, self._pmvs_counts[1])
-        return res
+        return keys
+
+    def _image_params(self):
+        """the 31 parameters in the order of pmvs_image_weights: 11 conv weights, 10 gammas, 10 betas"""
+        convs, bns = self._image_layers()
+        return [c.weight for c in convs] + [bn.weight for bn in bns] + [bn.bias for bn in bns]
 
     def _image_layers(self):
         """the 11 convolutions in the order of pmvs_image_weights and the 10 BatchNorm layers"""
@@ -375,6 +388,135 @@ def stack_views_channels_last(per_view, keys=("conv1", "conv2", "conv3"), out=No
 # the pyramid levels ImageConv hands out and the level (each halves h and w) of each of its BatchNorm layers
 _IMAGE_LEVELS = ("conv0", "conv1", "conv2", "conv3")
 _IMAGE_LEVEL = (0, 0, 1, 1, 1, 2, 2, 2, 3, 3)
+
+
+def _level_sizes(H, W):
+    """(h, w) of the four pyramid levels: each 5x5 stride-2 layer gives ceil(n / 2)"""
+    res = [(H, W)]
+    for _ in range(3):
+        res.append(((res[-1][0] + 1) // 2, (res[-1][1] + 1) // 2))
+    return res
+
+
+def _image_forward(mod, img_list, keys, out, ctx):
+    """pmvs_image_conv on `img_list` (checked by ImageConv._check_views) -> {key: level}; with `ctx` (an autograd
+    context) pmvs_image_conv_keep, whose workspace is saved on it with what the backward needs, and the list of the
+    level buffers in `keys` order."""
+    B, V, _, H, W = img_list.shape
+    convs, bns = mod._image_layers()
+    train = _bn_train_mode(bns, "ImageConv")
+    sizes = _level_sizes(H, W)
+    dev = img_list.device
+    res, bufs = {}, [None] * 4
+    for k in keys:
+        lev = _IMAGE_LEVELS.index(k)
+        (h, w), C = sizes[lev], 8 << lev
+        shape = (B, V, h, w, C) if mod.channels_last else (B, V, C, h, w)
+        if out is not None and k in out:
+            buf = out[k]
+            if (tuple(buf.shape) != shape or buf.dtype != torch.float32 or buf.device != dev
+                    or not buf.is_contiguous()):
+                raise RuntimeError("ImageConv.forward_views: out[%r] must be a contiguous float32 %s tensor on %s"
+                                   % (k, shape, dev))
+        else:
+            buf = torch.empty(shape, device=dev, dtype=torch.float32)
+        bufs[lev] = buf
+        res[k] = buf.permute(0, 1, 4, 2, 3) if mod.channels_last else buf
+    keep = []
+    wt = _conv_bn_weights(ImageWeights(), [c.weight for c in convs], bns, train, keep)
+    img = img_list.contiguous()
+    couts = [bn.num_features for bn in bns]
+    sums = torch.empty(V, 2 * sum(couts), device=dev, dtype=torch.float64) if train else None
+    levels = (ctypes.c_void_p * 4)(*[ptr(b) for b in bufs])
+    size_fn, call = ((lib.pmvs_image_conv_workspace_bytes, lib.pmvs_image_conv) if ctx is None else
+                     (lib.pmvs_image_conv_keep_workspace_bytes, lib.pmvs_image_conv_keep))
+    with torch.cuda.device(dev):
+        nbytes = int(size_fn(B, V, H, W, mod.base_channels))
+        if nbytes == 0:
+            check(1)
+        wsp = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+        check(call(ptr(img), ctypes.byref(wt), 1 if train else 0, ctypes.byref(levels), 1 if mod.channels_last else 0,
+                   ptr(sums), ptr(wsp), nbytes, B, V, H, W, mod.base_channels, stream_ptr()))
+    if ctx is not None:
+        ctx.img, ctx.ws, ctx.sums, ctx.train = img, wsp, sums, train
+        ctx.eps = [float(bn.eps) for bn in bns]
+        ctx.shape = (B, V, H, W, mod.base_channels)
+        ctx.channels_last = mod.channels_last
+        ctx.levels = [_IMAGE_LEVELS.index(k) for k in keys]
+    if train:
+        key = (B, H, W, str(dev))
+        if getattr(mod, "_pmvs_counts", (None,))[0] != key:  # one small upload per shape, not per call
+            n = torch.cat([torch.full((c,), float(B * sizes[l][0] * sizes[l][1]), dtype=torch.float64)
+                           for c, l in zip(couts, _IMAGE_LEVEL)]).to(dev)
+            object.__setattr__(mod, "_pmvs_counts", (key, n))
+        _update_running_rows(bns, sums, couts, mod._pmvs_counts[1])
+    return res if ctx is None else [bufs[_IMAGE_LEVELS.index(k)] for k in keys]
+
+
+# the conv layer that produces each pyramid level (pmvs_image_weights order)
+_IMAGE_LEVEL_LAYER = (1, 4, 7, 10)
+
+
+class _ImageConvFn(torch.autograd.Function):
+    """ImageConv.forward_views with the fused backward (pmvs_image_conv_backward).  Inputs are the images (data: no
+    gradient) and the module's 31 parameters (11 conv weights, 10 gammas, 10 betas), so their .grad fills; outputs
+    are the level buffers of `keys` in the forward's layout.  The running statistics update once, in the forward."""
+
+    @staticmethod
+    def forward(ctx, img_list, mod, keys, *params):
+        ctx.set_materialize_grads(False)
+        bufs = _image_forward(mod, img_list, keys, None, ctx)
+        # the images as the kernels read them and the parameters: an in-place change before backward trips the
+        # version check
+        ctx.save_for_backward(ctx.img, *params)
+        del ctx.img
+        return tuple(bufs)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, *grad_levels):
+        img, *params = ctx.saved_tensors
+        B, V, H, W, base = ctx.shape
+        dev = img.device
+        levels = [None] * 4
+        for lev, g in zip(ctx.levels, grad_levels):
+            if g is not None:
+                levels[lev] = f32c(g)
+        top = max([_IMAGE_LEVEL_LAYER[k] for k in range(4) if levels[k] is not None], default=-1)
+        res = [None, None, None]
+        if top < 0:
+            return tuple(res + [None] * len(params))
+        keep = []
+
+        def p32(t):
+            t = f32c(t.detach())
+            keep.append(t)
+            return t.data_ptr()
+
+        wt = ImageWeights()
+        for l in range(11):
+            wt.weight[l] = p32(params[l])
+        for l in range(10):
+            wt.gamma[l], wt.beta[l], wt.eps[l] = p32(params[11 + l]), p32(params[21 + l]), ctx.eps[l]
+        grads = [torch.empty(p.shape, device=dev, dtype=torch.float32) for p in params]
+        g = ImageGrads()
+        for l in range(11):
+            g.weight[l] = grads[l].data_ptr()
+        for l in range(10):
+            g.gamma[l], g.beta[l] = grads[11 + l].data_ptr(), grads[21 + l].data_ptr()
+        lv = (ctypes.c_void_p * 4)(*[ptr(t) for t in levels])
+        with torch.cuda.device(dev):
+            nbytes = int(lib.pmvs_image_conv_backward_workspace_bytes(B, V, H, W, base))
+            if nbytes == 0:
+                check(1)
+            ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+            check(lib.pmvs_image_conv_backward(ptr(img), ctypes.byref(wt), 1 if ctx.train else 0, ptr(ctx.ws),
+                                               ptr(ctx.sums), ctypes.byref(lv), 1 if ctx.channels_last else 0,
+                                               ctypes.byref(g), ptr(ws), nbytes, B, V, H, W, base, stream_ptr()))
+        for i, p in enumerate(params):
+            layer = i if i < 11 else (i - 11) % 10
+            res.append(grads[i].to(p.dtype) if ctx.needs_input_grad[3 + i] and layer <= top else None)
+        return tuple(res)
 
 
 def _bn_train_mode(bns, what):
