@@ -576,6 +576,36 @@ int pmvs_point_flow_backward(const pmvs_flow_shape* shape, const pmvs_flow_weigh
                              const float* grad_prob_out, const pmvs_flow_grads* grads, void* workspace,
                              size_t workspace_bytes, pmvs_stream_t stream);
 
+/* ---- training loss and metrics (DESIGN 3.16; model.py:308-420, networks.py:170-181 MAELoss) ------------------- */
+/* The T predicted depth maps a step is scored on: T = 1 (coarse_depth_map, isFlow false) or T = 3 (coarse_depth_map,
+ * flow1, flow2).  pred[t] is [B, 1, h[t], w[t]] fp32 device memory.  Where h[t - 1] == h[t], w[t - 1] must equal w[t]
+ * (model.py:362 resizes the previous map only when its height differs). */
+typedef struct pmvs_depth_terms {
+  const float* pred[3];
+  int h[3], w[3];
+  int T;
+} pmvs_depth_terms;
+
+/* Replaces PointMVSNetLoss.forward and PointMVSNetMetric.forward (model.py:314-339, 382-420).  gt [B, 1, Hg, Wg] and
+ * cams [B, V, 2, 4, 4] fp32 device memory.  Term t reads the ground truth at F.interpolate(gt, (h[t], w[t])) (mode
+ * nearest, source index min(floor(dst * (float)in / out), in - 1) in fp32), gathered on the fly, and the interval
+ * iv_t[b] = s_t * cams[b, 0, 1, 3, 1] in fp32 with s = (1, 0.75, 0.375).  m = (g != 0).
+ *   loss_out[t]         = (1 / T) sum_b (sum_p m |p - g| / iv_t[b]) / (sum_p m + 1e-7)          (MAELoss / T)
+ *   metric_out[2t + k]  = sum_{b,p} mv [|p - g| / iv_t <= thr_k] / (sum_{b,p} mv + 1e-7), thr = (1, 3) (batch-wide)
+ * with mv = m for the coarse term and mv = m [|q - g| / iv_t < valid_threshold] for a flow term, q the previous term
+ * (nearest-resized to the term's grid when its height differs).  Divisions are IEEE fp32, so the counts equal an fp32
+ * restatement's; sums are fp64 in a fixed order.  stats [T, B, 5] fp64 (written): per (t, b) sum m |p - g|, sum m,
+ * sum mv and the two threshold counts, read by the backward.  Two launches, no allocation, no synchronisation, no
+ * floating-point atomics. */
+int pmvs_depth_loss(const pmvs_depth_terms* terms, const float* gt, int Hg, int Wg, const float* cams, int B, int V,
+                    float valid_threshold, float* loss_out, float* metric_out, double* stats, pmvs_stream_t stream);
+/* Gradient of the T losses of pmvs_depth_loss with respect to the predictions (the backward of model.py:320-334):
+ * grad_pred[t] [B, 1, h[t], w[t]] = grad_loss[t] m sign(p - g) / (T iv_t[b] (sum m + 1e-7)), sign(0) = 0.  grad_loss
+ * [T] fp32 and stats (the forward's) are read on the device; every grad_pred[t] is overwritten.  One launch. */
+int pmvs_depth_loss_backward(const pmvs_depth_terms* terms, const float* gt, int Hg, int Wg, const float* cams, int B,
+                             int V, const double* stats, const float* grad_loss, float* const grad_pred[3],
+                             pmvs_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

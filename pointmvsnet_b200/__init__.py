@@ -9,13 +9,14 @@ Mirrors the reference's import surface (pointmvsnet/model.py:8-12):
     pointmvsnet_b200.nn.mlp / nn.conv    SharedMLP, Conv1d
     pointmvsnet_b200.utils.io / utils.eval_file_logger   PFM / camera files, per-view outputs (test.py:76)
 plus the new ``PointFlow`` module that replaces the ``point_flow`` closure
-(pointmvsnet/model.py:150-295).  ``install_as_pointmvsnet()`` aliases these modules
+(pointmvsnet/model.py:150-295), and ``pointmvsnet_b200.model``, the whole model with its loss and metrics
+(pointmvsnet/model.py:15-438).  ``install_as_pointmvsnet()`` aliases these modules
 under the reference's own names so an unchanged ``pointmvsnet/model.py`` imports them.
 """
 __version__ = "0.1.0"
 
 
-def install_as_pointmvsnet(reference_root=None):
+def install_as_pointmvsnet(reference_root=None, model=False):
     """Make ``import pointmvsnet.<hot-path module>`` resolve to this package.
 
     With ``reference_root`` (a checkout of callmeray/PointMVSNet) the rest of the
@@ -23,7 +24,9 @@ def install_as_pointmvsnet(reference_root=None):
     the hot-path modules are replaced, so the unchanged ``pointmvsnet/model.py`` runs on
     the sm_90a kernels.  Without it, stub parent packages are created and every module
     this package mirrors is aliased (enough for ``from pointmvsnet.utils.torch_utils
-    import get_knn_3d`` style imports).  See INTEGRATION.md."""
+    import get_knn_3d`` style imports).  With ``model=True`` ``pointmvsnet.model`` is aliased to
+    ``pointmvsnet_b200.model`` as well, so an unchanged train.py / test.py builds the whole model on the library
+    (``from pointmvsnet.model import build_pointmvsnet``).  See INTEGRATION.md."""
     import importlib
     import sys
     import types
@@ -36,6 +39,8 @@ def install_as_pointmvsnet(reference_root=None):
         "pointmvsnet.utils.io": "pointmvsnet_b200.utils.io",
         "pointmvsnet.utils.eval_file_logger": "pointmvsnet_b200.utils.eval_file_logger",
     }
+    if model:
+        hot["pointmvsnet.model"] = "pointmvsnet_b200.model"
     extra = {
         "pointmvsnet.functions.functions": "pointmvsnet_b200.functions.functions",
         "pointmvsnet.networks": "pointmvsnet_b200.networks",

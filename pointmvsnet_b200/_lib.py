@@ -73,6 +73,10 @@ class ImageGrads(C.Structure):
     _fields_ = [("weight", C.c_void_p * 11), ("gamma", C.c_void_p * 10), ("beta", C.c_void_p * 10)]
 
 
+class DepthTerms(C.Structure):
+    _fields_ = [("pred", C.c_void_p * 3), ("h", C.c_int * 3), ("w", C.c_int * 3), ("T", C.c_int)]
+
+
 def _sig(name, restype, argtypes):
     fn = getattr(lib, name)
     fn.restype = restype
@@ -142,6 +146,8 @@ _sig("pmvs_point_flow_debug_feature", I, [C.POINTER(FlowShape), P, P, P])
 _sig("pmvs_point_flow_backward_workspace_bytes", C.c_size_t, [C.POINTER(FlowShape)])
 _sig("pmvs_point_flow_backward", I, [C.POINTER(FlowShape), C.POINTER(FlowWeights), C.POINTER(C.c_void_p * 3),
                                      P, P, P, P, P, P, P, P, C.POINTER(FlowGrads), P, C.c_size_t, P])
+_sig("pmvs_depth_loss", I, [C.POINTER(DepthTerms), P, I, I, P, I, I, F, P, P, P, P])
+_sig("pmvs_depth_loss_backward", I, [C.POINTER(DepthTerms), P, I, I, P, I, I, P, P, C.POINTER(C.c_void_p * 3), P])
 
 EXPORTED = [
     "pmvs_version", "pmvs_last_error", "pmvs_launch_count", "pmvs_set_option", "pmvs_get_option", "pmvs_profile_enable", "pmvs_profile_collect", "pmvs_set_gemm_mode", "pmvs_get_gemm_mode", "pmvs_gather_knn_forward",
@@ -157,6 +163,7 @@ EXPORTED = [
     "pmvs_transpose", "pmvs_idx64_to_idx32", "pmvs_edgeconv_pm", "pmvs_edgeconv_pm_backward_workspace_bytes", "pmvs_edgeconv_pm_backward", "pmvs_linear_pm", "pmvs_point_flow_workspace_bytes",
     "pmvs_point_flow_iter", "pmvs_pyramid_to_channels_last", "pmvs_point_flow_debug_offsets",
     "pmvs_point_flow_debug_feature", "pmvs_point_flow_backward_workspace_bytes", "pmvs_point_flow_backward",
+    "pmvs_depth_loss", "pmvs_depth_loss_backward",
 ]
 
 

@@ -60,9 +60,14 @@ def build_cost_volume(feature_list, cam_params_list, is_test=True):
     require_cuda(feature_list, cam_params_list)
     if feature_list.dim() != 5 or cam_params_list.dim() != 5:
         raise RuntimeError("build_cost_volume: feature_list [B,V,C,h,w], cam_params_list [B,V,2,4,4]")
+    D = int(cam_params_list[0, 0, 1, 3, 2].item())  # model.py:65 (the reference syncs here too)
+    return _build_cost_volume(feature_list, cam_params_list, D, is_test)
+
+
+def _build_cost_volume(feature_list, cam_params_list, D, is_test):
+    """build_cost_volume with D already read on the host (model.PointMVSNet reads it once, before any launch)"""
     feats = f32c(feature_list)
     cams = f32c(cam_params_list)
-    D = int(cams[0, 0, 1, 3, 2].item())  # model.py:65 (the reference syncs here too)
     if torch.is_grad_enabled() and feature_list.requires_grad:
         return _CostVolumeFn.apply(feats, cams.detach(), D, bool(is_test))
     return _forward(feats, cams, D, is_test)
