@@ -233,18 +233,29 @@ int pmvs_cloud_filter(const float* xyz, int n, const float* bb, float margin, co
                       pmvs_stream_t stream);
 
 /* ---- coarse stage: VolumeConv and the depth regression (DESIGN 3.12; networks.py:127-167, model.py:115-130) ---- */
-/* The 11 layers in the reference's attribute order: conv0_1, conv1_0, conv2_0, conv3_0, conv1_1, conv2_1, conv3_1,
- * conv4_0, conv5_0, conv6_0, conv6_2.  weight[l] is the PyTorch tensor as stored: Conv3d [Cout, Cin, 3, 3, 3] (l != 7,
- * 8, 9), ConvTranspose3d [Cin, Cout, 3, 3, 3] (l = 7, 8, 9).  The BatchNorm arrays cover the first ten layers (conv6_2
- * has none); running_mean / running_var are read in eval mode only and never written. */
-typedef struct pmvs_volume_weights {
+/* The parameters of a conv-BatchNorm tower of 11 convolutions, the first ten followed by BatchNorm (VolumeConv,
+ * ImageConv).  weight[l] is the PyTorch tensor as stored; running_mean / running_var are read in eval mode only and
+ * never written. */
+typedef struct pmvs_conv_bn_weights {
   const float* weight[11];
   const float* gamma[10];
   const float* beta[10];
   const float* running_mean[10];
   const float* running_var[10];
   float eps[10];
-} pmvs_volume_weights;
+} pmvs_conv_bn_weights;
+
+/* Gradients of a conv-BatchNorm tower in the PyTorch layouts, overwritten (not accumulated), like pmvs_flow_grads. */
+typedef struct pmvs_conv_bn_grads {
+  float* weight[11];
+  float* gamma[10];
+  float* beta[10];
+} pmvs_conv_bn_grads;
+
+/* The 11 layers in the reference's attribute order: conv0_1, conv1_0, conv2_0, conv3_0, conv1_1, conv2_1, conv3_1,
+ * conv4_0, conv5_0, conv6_0, conv6_2.  weight[l] is Conv3d [Cout, Cin, 3, 3, 3] (l != 7, 8, 9), ConvTranspose3d [Cin,
+ * Cout, 3, 3, 3] (l = 7, 8, 9).  The BatchNorm arrays cover the first ten layers (conv6_2 has none). */
+typedef pmvs_conv_bn_weights pmvs_volume_weights;
 
 /* x [B, Cin, D, H, W] fp32 (the layout of the cost volume) -> out [B, 1, D, H, W]: the forward of VolumeConv with
  * BatchNorm on batch statistics (train != 0; biased variance for normalising) or on the running statistics (train ==
@@ -269,17 +280,9 @@ int pmvs_coarse_depth(const float* filtered, const float* cams, int B, int V, in
 
 /* ---- image towers: ImageConv for every view in one call (DESIGN 3.14; networks.py:84-124, model.py:71-77,133-148) */
 /* The 11 layers in module order: conv0.0, conv0.1, conv1.0, conv1.1, conv1.2, conv2.0, conv2.1, conv2.2, conv3.0,
- * conv3.1, conv3.2.  weight[l] is the PyTorch Conv2d tensor as stored, [Cout, Cin, K, K] (K = 5 for the stride-2
- * layers conv1.0, conv2.0, conv3.0, else 3).  The BatchNorm arrays cover the first ten layers (conv3.2 is a plain
- * convolution); running_mean / running_var are read in eval mode only and never written. */
-typedef struct pmvs_image_weights {
-  const float* weight[11];
-  const float* gamma[10];
-  const float* beta[10];
-  const float* running_mean[10];
-  const float* running_var[10];
-  float eps[10];
-} pmvs_image_weights;
+ * conv3.1, conv3.2.  weight[l] is the PyTorch Conv2d tensor, [Cout, Cin, K, K] (K = 5 for the stride-2 layers conv1.0,
+ * conv2.0, conv3.0, else 3).  The BatchNorm arrays cover the first ten layers (conv3.2 is a plain convolution). */
+typedef pmvs_conv_bn_weights pmvs_image_weights;
 
 /* Bytes of device workspace pmvs_image_conv needs; 0 (with pmvs_last_error) for a shape it does not serve.  With
  * N = B*V images, level sizes h_0 = H, h_k = ceil(h_(k-1) / 2) (w alike), layer l writing C_l channels at level k_l,
@@ -323,12 +326,8 @@ int pmvs_image_conv_keep(const float* img, const pmvs_image_weights* weights, in
                          int channels_last, double* batch_sums, void* workspace, size_t workspace_bytes, int B, int V,
                          int H, int W, int base_channels, pmvs_stream_t stream);
 
-/* Outputs of pmvs_image_conv_backward, PyTorch layouts, overwritten (not accumulated), like pmvs_volume_grads. */
-typedef struct pmvs_image_grads {
-  float* weight[11]; /* Conv2d [Cout, Cin, K, K] */
-  float* gamma[10];
-  float* beta[10];
-} pmvs_image_grads;
+/* Outputs of pmvs_image_conv_backward: weight[l] Conv2d [Cout, Cin, K, K]. */
+typedef pmvs_conv_bn_grads pmvs_image_grads;
 
 /* Bytes of device workspace pmvs_image_conv_backward needs; 0 (with pmvs_last_error) for a shape the forward does not
  * take.  With the notation above, E_l = K_l^2 Cin_l C_l the weights of layer l, and
@@ -360,12 +359,9 @@ int pmvs_image_conv_backward(const float* img, const pmvs_image_weights* weights
                              const pmvs_image_grads* grads, void* workspace, size_t workspace_bytes, int B, int V,
                              int H, int W, int base_channels, pmvs_stream_t stream);
 
-/* Outputs of pmvs_volume_conv_backward, PyTorch layouts, overwritten (not accumulated), like pmvs_flow_grads. */
-typedef struct pmvs_volume_grads {
-  float* weight[11]; /* Conv3d [Cout, Cin, 3, 3, 3]; ConvTranspose3d (l = 7, 8, 9) [Cin, Cout, 3, 3, 3] */
-  float* gamma[10];
-  float* beta[10];
-} pmvs_volume_grads;
+/* Outputs of pmvs_volume_conv_backward: weight[l] Conv3d [Cout, Cin, 3, 3, 3]; ConvTranspose3d (l = 7, 8, 9)
+ * [Cin, Cout, 3, 3, 3]. */
+typedef pmvs_conv_bn_grads pmvs_volume_grads;
 
 /* Bytes of device workspace pmvs_volume_conv_backward needs; 0 (with pmvs_last_error) for a shape the forward does not
  * take.  With V_k = D*H*W / 8^k the voxels of level k, layer l reading Cin_l channels at V_in,l voxels and writing

@@ -51,26 +51,22 @@ class FlowGrads(C.Structure):
     ]
 
 
-class VolumeWeights(C.Structure):
+class ConvBnWeights(C.Structure):
+    """pmvs_conv_bn_weights (pmvs_volume_weights, pmvs_image_weights)"""
     _fields_ = [
         ("weight", C.c_void_p * 11), ("gamma", C.c_void_p * 10), ("beta", C.c_void_p * 10),
         ("running_mean", C.c_void_p * 10), ("running_var", C.c_void_p * 10), ("eps", C.c_float * 10),
     ]
 
 
-class ImageWeights(C.Structure):
-    _fields_ = [
-        ("weight", C.c_void_p * 11), ("gamma", C.c_void_p * 10), ("beta", C.c_void_p * 10),
-        ("running_mean", C.c_void_p * 10), ("running_var", C.c_void_p * 10), ("eps", C.c_float * 10),
-    ]
-
-
-class VolumeGrads(C.Structure):
+class ConvBnGrads(C.Structure):
+    """pmvs_conv_bn_grads (pmvs_volume_grads, pmvs_image_grads)"""
     _fields_ = [("weight", C.c_void_p * 11), ("gamma", C.c_void_p * 10), ("beta", C.c_void_p * 10)]
 
 
-class ImageGrads(C.Structure):
-    _fields_ = [("weight", C.c_void_p * 11), ("gamma", C.c_void_p * 10), ("beta", C.c_void_p * 10)]
+# the per-tower names, kept for existing callers as the C header keeps its typedefs
+VolumeWeights = ImageWeights = ConvBnWeights
+VolumeGrads = ImageGrads = ConvBnGrads
 
 
 class DepthTerms(C.Structure):
@@ -115,21 +111,21 @@ _sig("pmvs_nearest_distances_workspace_bytes", C.c_size_t, [I])
 _sig("pmvs_nearest_distances", I, [P, I, P, I, F, F, P, P, C.c_size_t, P])
 _sig("pmvs_cloud_filter", I, [P, I, P, F, P, P, F, P, P, P])
 _sig("pmvs_volume_conv_workspace_bytes", C.c_size_t, [I, I, I, I, I, I])
-_sig("pmvs_volume_conv", I, [P, C.POINTER(VolumeWeights), I, P, P, P, C.c_size_t, I, I, I, I, I, I, P])
+_sig("pmvs_volume_conv", I, [P, C.POINTER(ConvBnWeights), I, P, P, P, C.c_size_t, I, I, I, I, I, I, P])
 _sig("pmvs_coarse_depth", I, [P, P, I, I, I, I, I, P, P, P])
 _sig("pmvs_volume_conv_backward_workspace_bytes", C.c_size_t, [I, I, I, I, I, I])
-_sig("pmvs_volume_conv_backward", I, [P, C.POINTER(VolumeWeights), I, P, P, P, P, C.POINTER(VolumeGrads), P,
+_sig("pmvs_volume_conv_backward", I, [P, C.POINTER(ConvBnWeights), I, P, P, P, P, C.POINTER(ConvBnGrads), P,
                                       C.c_size_t, I, I, I, I, I, I, P])
 _sig("pmvs_coarse_depth_backward", I, [P, P, P, P, I, I, I, I, I, P])
 _sig("pmvs_image_conv_workspace_bytes", C.c_size_t, [I, I, I, I, I])
-_sig("pmvs_image_conv", I, [P, C.POINTER(ImageWeights), I, C.POINTER(C.c_void_p * 4), I, P, P, C.c_size_t, I, I, I,
+_sig("pmvs_image_conv", I, [P, C.POINTER(ConvBnWeights), I, C.POINTER(C.c_void_p * 4), I, P, P, C.c_size_t, I, I, I,
                             I, I, P])
 _sig("pmvs_image_conv_keep_workspace_bytes", C.c_size_t, [I, I, I, I, I])
-_sig("pmvs_image_conv_keep", I, [P, C.POINTER(ImageWeights), I, C.POINTER(C.c_void_p * 4), I, P, P, C.c_size_t, I,
+_sig("pmvs_image_conv_keep", I, [P, C.POINTER(ConvBnWeights), I, C.POINTER(C.c_void_p * 4), I, P, P, C.c_size_t, I,
                                  I, I, I, I, P])
 _sig("pmvs_image_conv_backward_workspace_bytes", C.c_size_t, [I, I, I, I, I])
-_sig("pmvs_image_conv_backward", I, [P, C.POINTER(ImageWeights), I, P, P, C.POINTER(C.c_void_p * 4), I,
-                                     C.POINTER(ImageGrads), P, C.c_size_t, I, I, I, I, I, P])
+_sig("pmvs_image_conv_backward", I, [P, C.POINTER(ConvBnWeights), I, P, P, C.POINTER(C.c_void_p * 4), I,
+                                     C.POINTER(ConvBnGrads), P, C.c_size_t, I, I, I, I, I, P])
 _sig("pmvs_transpose", I, [P, P, I, I, I, P])
 _sig("pmvs_idx64_to_idx32", I, [P, P, LL, P])
 _sig("pmvs_edgeconv_pm", I, [P, I, P, P, P, P, F, I, I, P, I, P, P, I, I, I, I, I, I, P])
@@ -193,6 +189,14 @@ def f32c(t):
     if t.dtype != torch.float32:
         t = t.float()
     return t.contiguous()
+
+
+def workspace(nbytes, device):
+    """a device workspace of `nbytes` bytes, a library size function's result (0: the library's error is raised).
+    The caching allocator aligns blocks to 512 bytes, more than the 256 the library needs."""
+    if nbytes == 0:
+        check(1)
+    return torch.empty(nbytes, device=device, dtype=torch.uint8)
 
 
 def launch_count():

@@ -7,7 +7,7 @@ regression that follows VolumeConv (model.py:117-130)."""
 import torch
 from torch.autograd.function import once_differentiable
 
-from ._lib import lib, check, stream_ptr, ptr, require_cuda, f32c
+from ._lib import lib, check, stream_ptr, ptr, require_cuda, f32c, workspace
 
 
 def _forward(feats, cams, D, is_test):
@@ -37,9 +37,7 @@ class _CostVolumeFn(torch.autograd.Function):
         g = f32c(grad_cost)
         grad = torch.empty_like(feats)
         nbytes = int(lib.pmvs_cost_volume_backward_workspace_bytes(B, V, Cc, h, w, ctx.D))
-        if nbytes == 0:
-            check(1)
-        ws = torch.empty(nbytes, device=feats.device, dtype=torch.uint8)  # the caching allocator aligns to 512 bytes
+        ws = workspace(nbytes, feats.device)
         with torch.cuda.device(feats.device):
             check(lib.pmvs_cost_volume_backward(ptr(feats), ptr(cams), ptr(g), ptr(grad), ptr(ws), nbytes, B, V, Cc,
                                                 h, w, ctx.D, 1 if ctx.is_test else 0, stream_ptr()))

@@ -132,8 +132,6 @@ __global__ void __launch_bounds__(256)
 // ---------------------------------------------------------------------------------------
 // PointFlow iteration: workspace plan
 // ---------------------------------------------------------------------------------------
-static inline size_t align_up(size_t x) { return (x + 255) & ~(size_t)255; }
-
 struct FlowPlan {
   int S, hs, ws, N;  // S = sub-clouds PROCESSED by this call (all ratio^2 unless sharded)
   int sub_begin;
@@ -173,17 +171,17 @@ static int make_plan(const pmvs_flow_shape* s, FlowPlan& p) {
   p.R = (size_t)p.S * s->B * p.N;
   PMVS_REQUIRE(p.R * 224 < (size_t)1 << 40, "point_flow: problem too large");
   size_t o = 0;
-  p.cam = o; o += align_up(cam_block_bytes(s->B, s->V));
-  p.feature = o; o += align_up(p.R * PMVS_FEAT_CH * 4);
-  p.xyz = o; o += align_up(p.R * 3 * 4);
-  p.idx = o; o += align_up(p.R * PMVS_KNN * 4);
-  p.le = o; o += align_up(p.R * 128 * 4);
-  p.ecat = o; o += align_up(p.R * 224 * 4);
-  p.h0 = o; o += align_up(p.R * 64 * 4);
-  p.h1 = o; o += align_up(p.R * 64 * 4);
-  p.h2 = o; o += align_up(p.R * 16 * 4);
-  p.warp_src = o; o += align_up(warp_source_bytes(s->B, s->V, s->flow_h, s->flow_w));
-  p.cand = o; o += align_up(p.R * PMVS_KNN * 2);
+  p.cam = o; o += up256(cam_block_bytes(s->B, s->V));
+  p.feature = o; o += up256(p.R * PMVS_FEAT_CH * 4);
+  p.xyz = o; o += up256(p.R * 3 * 4);
+  p.idx = o; o += up256(p.R * PMVS_KNN * 4);
+  p.le = o; o += up256(p.R * 128 * 4);
+  p.ecat = o; o += up256(p.R * 224 * 4);
+  p.h0 = o; o += up256(p.R * 64 * 4);
+  p.h1 = o; o += up256(p.R * 64 * 4);
+  p.h2 = o; o += up256(p.R * 16 * 4);
+  p.warp_src = o; o += up256(warp_source_bytes(s->B, s->V, s->flow_h, s->flow_w));
+  p.cand = o; o += up256(p.R * PMVS_KNN * 2);
   size_t d = 0;
   const int ec_cout[3] = {32, 32, 64};
   const int mlp_cout[3] = {64, 64, 16};
@@ -194,8 +192,8 @@ static int make_plan(const pmvs_flow_shape* s, FlowPlan& p) {
   for (int l = 0; l < 3; ++l) { p.st_mlp[l] = d; d += (size_t)p.S * 2 * mlp_cout[l]; }
   p.st_ticket = d; d += (3 * (size_t)p.S + 1) / 2 + 1;
   p.stats_doubles = d;
-  p.stats = o; o += align_up(d * 8);
-  p.coef = o; o += align_up(3 * (size_t)p.S * 6 * 64 * sizeof(float));
+  p.stats = o; o += up256(d * 8);
+  p.coef = o; o += up256(3 * (size_t)p.S * 6 * 64 * sizeof(float));
   p.total = o;
   return PMVS_OK;
 }
@@ -302,11 +300,7 @@ extern "C" int pmvs_gather_knn_backward(const float* grad_output, const int64_t*
   if ((long long)B * C * N == 0) return PMVS_OK;
   PMVS_REQUIRE(grad_output && index && grad_input, "gather_knn_backward: NULL pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  if ((long long)B * C * N > 0 &&
-      cudaMemsetAsync(grad_input, 0, (size_t)B * C * N * sizeof(float), st) != cudaSuccess) {
-    set_error("gather_knn_backward: memset failed");
-    return PMVS_ERR_CUDA;
-  }
+  PMVS_TRY(memset_async("gather_knn_backward", grad_input, (size_t)B * C * N * sizeof(float), st));
   const long long total = (long long)B * C * N * K;
   if (total == 0) return PMVS_OK;
   const int grid = (int)std::min<long long>(cdiv(total, 256), sm_count() * 16);
@@ -321,10 +315,7 @@ extern "C" int pmvs_edgeconv_pm(const float* x, int ldx, const int32_t* idx32, c
   PMVS_REQUIRE(x && idx32 && w12 && gamma && beta && out && le_scratch && stats_scratch, "edgeconv: NULL pointer");
   PMVS_REQUIRE(groups > 0 && rows_per_group > 0 && N > 0 && K > 0, "edgeconv: bad sizes");
   cudaStream_t st = (cudaStream_t)stream;
-  if (bn_train && cudaMemsetAsync(stats_scratch, 0, (size_t)groups * 4 * cout * sizeof(double), st) != cudaSuccess) {
-    set_error("edgeconv: memset failed");
-    return PMVS_ERR_CUDA;
-  }
+  if (bn_train) PMVS_TRY(memset_async("edgeconv", stats_scratch, (size_t)groups * 4 * cout * sizeof(double), st));
   GemmArgs g{};
   g.x = x; g.ldx = ldx; g.w = w12; g.y = le_scratch; g.ldy = 2 * cout;
   g.groups = groups; g.rows_per_group = rows_per_group; g.cin = cin; g.cout = 2 * cout; g.eps = eps;
@@ -385,11 +376,7 @@ extern "C" int pmvs_point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flo
   PMVS_TRY(make_plan(shape, p));
   PMVS_REQUIRE(wts && pyramids_cl && depth_prev && cam_params && interval && mean && stdv && depth_out && workspace,
                "point_flow: NULL pointer");
-  if (workspace_bytes < p.total) {
-    set_error("point_flow: workspace %zu bytes < required %zu", workspace_bytes, p.total);
-    return PMVS_ERR_WORKSPACE;
-  }
-  PMVS_REQUIRE(((uintptr_t)workspace & 255) == 0, "point_flow: workspace must be 256-byte aligned");
+  PMVS_TRY(check_workspace("point_flow", workspace, workspace_bytes, p.total));
   cudaStream_t st = (cudaStream_t)stream;
   char* ws = (char*)workspace;
   float* cam = (float*)(ws + p.cam);
@@ -405,10 +392,7 @@ extern "C" int pmvs_point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flo
   const int B = shape->B, S = p.S;
   const int rows_per_group = B * p.N;
 
-  if (cudaMemsetAsync(stats, 0, p.stats_doubles * sizeof(double), st) != cudaSuccess) {
-    set_error("point_flow: memset failed");
-    return PMVS_ERR_CUDA;
-  }
+  PMVS_TRY(memset_async("point_flow", stats, p.stats_doubles * sizeof(double), st));
   // model.py:159-163: K rows 0,1 scaled by image_scale (test) or 4*image_scale (train)
   const float kscale = shape->is_test ? shape->image_scale : (float)(4.0 * (double)shape->image_scale);
   PMVS_TRY(launch_cam_setup(cam_params, interval, mean, stdv, cam, B, shape->V, kscale, shape->interval_scale, st));

@@ -251,8 +251,6 @@ float sqrt_limit(float max_dist) {
   return L;
 }
 
-inline size_t up256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 struct GridPlan {
   size_t key, inv, rec, rank, total;
 };
@@ -278,25 +276,6 @@ int check_cell(const char* what, float cell) {
   int e = 0;
   PMVS_REQUIRE(cell > 0.f && cell <= FLT_MAX && frexpf(cell, &e) == 0.5f && e >= -59 && e <= 61,
                "%s: cell = %g (must be a power of two in [2^-60, 2^60])", what, (double)cell);
-  return PMVS_OK;
-}
-
-int check_workspace(const char* what, const void* ws, size_t bytes, size_t need) {
-  PMVS_REQUIRE(ws != nullptr && ((uintptr_t)ws & 255) == 0, "%s: workspace must be non-NULL and 256-byte aligned",
-               what);
-  if (bytes < need) {
-    set_error("%s: workspace %zu bytes < required %zu", what, bytes, need);
-    return PMVS_ERR_WORKSPACE;
-  }
-  return PMVS_OK;
-}
-
-int memset_async(const char* what, void* p, size_t bytes, cudaStream_t st) {
-  if (bytes != 0 && cudaMemsetAsync(p, 0, bytes, st) != cudaSuccess) {
-    cudaGetLastError();
-    set_error("%s: cudaMemsetAsync failed", what);
-    return PMVS_ERR_CUDA;
-  }
   return PMVS_OK;
 }
 

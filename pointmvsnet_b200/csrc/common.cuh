@@ -1,6 +1,7 @@
 // Shared helpers for libpmvs_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
+#include <float.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
@@ -45,6 +46,36 @@ inline int check_launch(const char* what, cudaStream_t st = nullptr) {
   } while (0)
 
 static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
+
+// workspace regions start at multiples of 256 bytes
+inline size_t up256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+inline bool finite_nonneg(float t) { return t >= 0.f && t <= FLT_MAX; }
+
+// the workspace an entry point takes: at least `need` bytes (PMVS_ERR_WORKSPACE) ...
+inline int check_workspace_size(const char* what, size_t bytes, size_t need) {
+  if (bytes < need) {
+    set_error("%s: workspace %zu bytes < required %zu", what, bytes, need);
+    return PMVS_ERR_WORKSPACE;
+  }
+  return PMVS_OK;
+}
+// ... and, checked first, non-NULL and 256-byte aligned (PMVS_ERR_ARG)
+inline int check_workspace(const char* what, const void* ws, size_t bytes, size_t need) {
+  PMVS_REQUIRE(ws != nullptr && ((uintptr_t)ws & 255) == 0, "%s: workspace must be non-NULL and 256-byte aligned",
+               what);
+  return check_workspace_size(what, bytes, need);
+}
+
+// cudaMemsetAsync(p, 0, bytes); a failure is cleared, so the next check_launch does not report it against a kernel
+inline int memset_async(const char* what, void* p, size_t bytes, cudaStream_t st) {
+  if (bytes != 0 && cudaMemsetAsync(p, 0, bytes, st) != cudaSuccess) {
+    cudaGetLastError();
+    set_error("%s: cudaMemsetAsync failed", what);
+    return PMVS_ERR_CUDA;
+  }
+  return PMVS_OK;
+}
 
 // SMs of the current device, for grid sizing (132 on an H100; the devices of one process are alike)
 inline int sm_count() {

@@ -124,8 +124,6 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-inline size_t up256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 struct CvBwdPlan {
   long long N, S;  // plane points and source rows (point, view >= 1) of a batch element
   size_t cam, df0, dfv, rec_idx, rec_w, lists, tex, total;
@@ -170,11 +168,7 @@ extern "C" int pmvs_cost_volume_backward(const float* features, const float* cam
   PMVS_REQUIRE(features && cam_params && grad_cost && grad_features && workspace, "cost_volume_backward: NULL pointer");
   CvBwdPlan p;
   PMVS_TRY(cv_bwd_plan(B, V, C, h, w, D, p));
-  PMVS_REQUIRE(((uintptr_t)workspace & 255) == 0, "cost_volume_backward: workspace must be 256-byte aligned");
-  if (workspace_bytes < p.total) {
-    set_error("cost_volume_backward: workspace %zu bytes < required %zu", workspace_bytes, p.total);
-    return PMVS_ERR_WORKSPACE;
-  }
+  PMVS_TRY(check_workspace("cost_volume_backward", workspace, workspace_bytes, p.total));
   cudaStream_t st = (cudaStream_t)stream;
   char* ws = (char*)workspace;
   auto F = [&](size_t off) { return (float*)(ws + off); };

@@ -132,8 +132,6 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-inline size_t up256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 struct FusePlan {
   size_t used, bits, total;
 };
@@ -148,8 +146,6 @@ int fuse_plan(int V, int H, int W, FusePlan& p) {
   p.total = p.bits + up256((size_t)cdiv(V, FUSE_CHUNK) * HW * 4);
   return PMVS_OK;
 }
-
-bool finite_nonneg(float t) { return t >= 0.f && t <= FLT_MAX; }
 
 }  // namespace
 
@@ -174,21 +170,13 @@ extern "C" int pmvs_fuse_depth_maps(const float* depth, const float* cam_block, 
   PMVS_REQUIRE(finite_nonneg(depth_thresh) && finite_nonneg(reproj_thresh),
                "fuse_depth_maps: thresholds must be finite and >= 0 (depth %g, reproj %g)", (double)depth_thresh,
                (double)reproj_thresh);
-  PMVS_REQUIRE(((uintptr_t)workspace & 255) == 0, "fuse_depth_maps: workspace must be 256-byte aligned");
-  if (workspace_bytes < p.total) {
-    set_error("fuse_depth_maps: workspace %zu bytes < required %zu", workspace_bytes, p.total);
-    return PMVS_ERR_WORKSPACE;
-  }
+  PMVS_TRY(check_workspace("fuse_depth_maps", workspace, workspace_bytes, p.total));
   cudaStream_t st = (cudaStream_t)stream;
   char* ws = (char*)workspace;
   unsigned char* used = (unsigned char*)(ws + p.used);
   unsigned* bits = (unsigned*)(ws + p.bits);
   const size_t VHW = (size_t)V * H * W;
-  if (cudaMemsetAsync(used, 0, VHW, st) != cudaSuccess) {
-    cudaGetLastError();
-    set_error("fuse_depth_maps: cudaMemsetAsync failed");
-    return PMVS_ERR_CUDA;
-  }
+  PMVS_TRY(memset_async("fuse_depth_maps", used, VHW, st));
   const int HW = H * W;
   for (int r = 0; r < V; ++r) {
     prof_begin("fuse_view", st);

@@ -683,13 +683,8 @@ extern "C" int pmvs_edgeconv_pm_backward(const float* x, int ldx, const int32_t*
                "edgeconv_backward: row strides must cover the row and be multiples of 4 floats");
   PMVS_REQUIRE(x && idx32 && idx64 && w12 && gamma && beta && le && stats && dy && dw12 && dgamma && dbeta,
                "edgeconv_backward: NULL pointer");
-  PMVS_REQUIRE(workspace != nullptr && ((uintptr_t)workspace & 255) == 0,
-               "edgeconv_backward: workspace must be 256-byte aligned");
   const BwdPlan p = bwd_plan(B, N, K, cin, cout);
-  if (workspace_bytes < p.total) {
-    set_error("edgeconv_backward: workspace %zu bytes < required %zu", workspace_bytes, p.total);
-    return PMVS_ERR_WORKSPACE;
-  }
+  PMVS_TRY(check_workspace("edgeconv_backward", workspace, workspace_bytes, p.total));
   cudaStream_t st = (cudaStream_t)stream;
   char* ws = (char*)workspace;
   EdgeLayerBwd L{};

@@ -1033,10 +1033,7 @@ extern "C" int pmvs_feature_fetch_backward(const float* grad_out, const float* p
   PMVS_REQUIRE(B > 0 && V > 0 && C > 0 && H > 1 && W > 1 && N >= 0, "feature_fetch_backward: bad shape");
   PMVS_REQUIRE((long long)B * V <= 65535, "feature_fetch_backward: B*V too large");
   cudaStream_t st = (cudaStream_t)stream;
-  if (cudaMemsetAsync(grad_maps, 0, (size_t)B * V * C * H * W * sizeof(float), st) != cudaSuccess) {
-    set_error("feature_fetch_backward: memset failed");
-    return PMVS_ERR_CUDA;
-  }
+  PMVS_TRY(memset_async("feature_fetch_backward", grad_maps, (size_t)B * V * C * H * W * sizeof(float), st));
   if (N == 0) return PMVS_OK;
   dim3 grid(cdiv(N, 256), B * V);
   feature_fetch_kernel<true><<<grid, 256, 0, st>>>(nullptr, pts, intrinsics, extrinsics, const_cast<float*>(grad_out),
@@ -1050,10 +1047,7 @@ extern "C" int pmvs_cost_volume(const float* features, const float* cam_params, 
   using namespace pmvs;
   PMVS_REQUIRE(features && cam_params && cost && workspace, "cost_volume: NULL pointer");
   PMVS_TRY(cost_volume_check_shape("cost_volume", B, V, C, h, w, D));
-  if (workspace_bytes < cam_block_bytes(B, V)) {
-    set_error("cost_volume: workspace %zu bytes < required %zu", workspace_bytes, cam_block_bytes(B, V));
-    return PMVS_ERR_WORKSPACE;
-  }
+  PMVS_TRY(check_workspace_size("cost_volume", workspace_bytes, cam_block_bytes(B, V)));
   cudaStream_t st = (cudaStream_t)stream;
   // model.py:58-61: K rows 0,1 divided by 2, and by 4 more at test time
   PMVS_TRY(launch_cam_setup(cam_params, nullptr, nullptr, nullptr, (float*)workspace, B, V, is_test ? 0.125f : 0.5f, 1.f,

@@ -102,8 +102,6 @@ __global__ void __launch_bounds__(256)
     if (j < nc) out[(size_t)j * HW] = acc[j];
 }
 
-inline size_t up256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 struct FdPlan {
   int rows;  // record rows per (b, v): max(N, H W)
   size_t rec_idx, rec_w, lists, total;
@@ -160,11 +158,7 @@ extern "C" int pmvs_feature_fetch_backward_det(const float* grad_out, const floa
                "feature_fetch_backward_det: NULL pointer");
   FdPlan p;
   PMVS_TRY(fd_plan(B, V, C, H, W, N, p));
-  PMVS_REQUIRE(((uintptr_t)workspace & 255) == 0, "feature_fetch_backward_det: workspace must be 256-byte aligned");
-  if (workspace_bytes < p.total) {
-    set_error("feature_fetch_backward_det: workspace %zu bytes < required %zu", workspace_bytes, p.total);
-    return PMVS_ERR_WORKSPACE;
-  }
+  PMVS_TRY(check_workspace("feature_fetch_backward_det", workspace, workspace_bytes, p.total));
   cudaStream_t st = (cudaStream_t)stream;
   char* ws = (char*)workspace;
   int64_t* rec_idx = (int64_t*)(ws + p.rec_idx);

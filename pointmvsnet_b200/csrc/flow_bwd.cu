@@ -286,8 +286,6 @@ __global__ void __launch_bounds__(256) nearest_bwd_kernel(const float* __restric
   dprev[e] = acc;
 }
 
-inline size_t up256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 struct BwdFlowPlan {
   size_t R, npix, nrec;
   int N, head_ctas, mlp_ctas;
@@ -412,12 +410,8 @@ extern "C" int pmvs_point_flow_backward(const pmvs_flow_shape* shape, const pmvs
                      grads->mlp_dgamma[l] && grads->mlp_dbeta[l] && pyramids_cl[l],
                  "point_flow_backward: NULL pointer");
   PMVS_REQUIRE(grads->mlp_dw[3] != nullptr, "point_flow_backward: NULL pointer");
-  PMVS_REQUIRE(((uintptr_t)workspace & 255) == 0 && ((uintptr_t)fwd_workspace & 255) == 0,
-               "point_flow_backward: workspaces must be 256-byte aligned");
-  if (workspace_bytes < p.total) {
-    set_error("point_flow_backward: workspace %zu bytes < required %zu", workspace_bytes, p.total);
-    return PMVS_ERR_WORKSPACE;
-  }
+  PMVS_REQUIRE(((uintptr_t)fwd_workspace & 255) == 0, "point_flow_backward: fwd_workspace must be 256-byte aligned");
+  PMVS_TRY(check_workspace("point_flow_backward", workspace, workspace_bytes, p.total));
   (void)cam_params; (void)mean; (void)stdv;  // the forward's camera blocks already hold them
   FlowRegions fr;
   PMVS_TRY(flow_regions(shape, fr));

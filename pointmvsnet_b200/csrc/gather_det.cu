@@ -172,10 +172,7 @@ int build_inv_lists(const int64_t* idx, int B, int N, int K, void* workspace, co
   int* list = (int*)(ws + p.list);
   *off_out = off;
   *list_out = list;
-  if (cudaMemsetAsync(cnt, 0, p.off - p.cnt, st) != cudaSuccess) {  // cnt and cur are adjacent
-    set_error("gather_knn_backward_det: memset failed");
-    return PMVS_ERR_CUDA;
-  }
+  PMVS_TRY(memset_async("build_inv_lists", cnt, p.off - p.cnt, st));  // cnt and cur are adjacent
   cudaStream_t pst = prof_name ? st : nullptr;  // check_launch closes the profiling record on this stream
   const long long NK = (long long)N * K, entries = (long long)B * NK, rows = (long long)B * N;
   auto blocks = [](long long n) { return (int)std::min<long long>(std::max<long long>(cdiv(n, GD_THREADS), 1), sm_count() * 16); };
@@ -256,12 +253,7 @@ extern "C" int pmvs_gather_knn_backward_det(const float* grad_output, const int6
   PMVS_REQUIRE(grad_input && (index || (long long)N * K == 0), "gather_knn_backward_det: NULL pointer");
   PMVS_REQUIRE((long long)B * N * K < (1ll << 31) && (long long)B * (N + 1) < (1ll << 31),
                "gather_knn_backward_det: B*N*K must be below 2^31");
-  const size_t need = inv_lists_bytes(B, N, K);
-  PMVS_REQUIRE(workspace != nullptr && ((uintptr_t)workspace & 255) == 0, "gather_knn_backward_det: workspace must be 256-byte aligned");
-  if (workspace_bytes < need) {
-    set_error("gather_knn_backward_det: workspace %zu bytes < required %zu", workspace_bytes, need);
-    return PMVS_ERR_WORKSPACE;
-  }
+  PMVS_TRY(check_workspace("gather_knn_backward_det", workspace, workspace_bytes, inv_lists_bytes(B, N, K)));
   cudaStream_t st = (cudaStream_t)stream;
   const int* off = nullptr;
   const int* list = nullptr;

@@ -39,25 +39,6 @@ __global__ void __launch_bounds__(256)
   out[i] = act(__ldg(y + src), __ldg(ss + v * C + c), __ldg(ss + (V + v) * C + c));
 }
 
-// PyTorch Conv2d weights [Cout, Cin, K, K] -> [K*K][Cin][Cout] for every layer in one launch
-struct IcPack {
-  const float* src[IC_LAYERS];
-  long long end[IC_LAYERS];  // running sum of the layers' element counts
-  long long dst_off[IC_LAYERS];
-  int cin[IC_LAYERS], cout[IC_LAYERS], taps[IC_LAYERS];
-};
-
-__global__ void ic_pack_kernel(const IcPack p, float* __restrict__ dst, long long total) {
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    int l = 0;
-    while (i >= p.end[l]) ++l;
-    const long long e = i - (l > 0 ? p.end[l - 1] : 0);
-    const int cout = p.cout[l], cin = p.cin[l], taps = p.taps[l];
-    const int co = (int)(e % cout), ci = (int)((e / cout) % cin), tap = (int)(e / ((long long)cout * cin));
-    dst[p.dst_off[l] + e] = __ldg(p.src[l] + ((long long)co * cin + ci) * taps + tap);
-  }
-}
-
 template <int K, int S, int CIN, int COUT, int CO, int PX>
 int launch_ic(const IcArgs& a, const IcLayerPlan& q, int N, const char* name, cudaStream_t st) {
   dim3 grid((unsigned)q.pix_blocks, (unsigned)q.groups, (unsigned)N);
@@ -108,37 +89,26 @@ int ic_forward(const float* img, const pmvs_image_weights* wt, int train, float*
     PMVS_REQUIRE(wt->gamma[l] && wt->beta[l], "image_conv: NULL BatchNorm affine of layer %d", l);
     PMVS_REQUIRE(train || (wt->running_mean[l] && wt->running_var[l]),
                  "image_conv: eval mode needs the running statistics of layer %d", l);
-    PMVS_REQUIRE(ic_finite_nonneg(wt->eps[l]), "image_conv: eps of layer %d = %g (finite, >= 0)", l,
+    PMVS_REQUIRE(finite_nonneg(wt->eps[l]), "image_conv: eps of layer %d = %g (finite, >= 0)", l,
                  (double)wt->eps[l]);
   }
   PMVS_REQUIRE(!train || (long long)B * p.h[3] * p.w[3] >= 2,
                "image_conv: train mode needs more than 1 value per channel at the coarsest level (B*h3*w3 = %lld)",
                (long long)B * p.h[3] * p.w[3]);
-  PMVS_REQUIRE(((uintptr_t)workspace & 255) == 0, "image_conv: workspace must be 256-byte aligned");
   for (int k = 0; k < 4; ++k)
     PMVS_REQUIRE(((uintptr_t)level_out[k] & 15) == 0, "image_conv: level output %d must be 16-byte aligned", k);
-  if (workspace_bytes < p.total) {
-    set_error("image_conv: workspace %zu bytes < required %zu", workspace_bytes, p.total);
-    return PMVS_ERR_WORKSPACE;
-  }
+  PMVS_TRY(check_workspace("image_conv", workspace, workspace_bytes, p.total));
   char* ws = (char*)workspace;
   const int N = B * V;
 
-  IcPack pk;
-  long long run = 0;
+  // PyTorch Conv2d weights [Cout, Cin, K, K] -> [K*K][Cin][Cout]
+  PackTable pk;
   for (int l = 0; l < IC_LAYERS; ++l) {
     const IcLayerPlan& q = p.L[l];
-    pk.src[l] = wt->weight[l];
-    run += (long long)q.k * q.k * q.cin * q.cout;
-    pk.end[l] = run;
-    pk.dst_off[l] = (long long)(q.w / 4);
-    pk.cin[l] = q.cin;
-    pk.cout[l] = q.cout;
-    pk.taps[l] = q.k * q.k;
+    const int taps = q.k * q.k;
+    pk.L[l] = {wt->weight[l], (long long)(q.w / 4), {taps, q.cin, q.cout}, 0, {1, taps, q.cin * taps}};
   }
-  prof_begin("ic_pack", st);
-  ic_pack_kernel<<<cdiv(p.wtotal, 256), 256, 0, st>>>(pk, (float*)ws, p.wtotal);
-  PMVS_TRY(check_launch("ic_pack_kernel", st));
+  PMVS_TRY(launch_pack(pk, IC_LAYERS, (float*)ws, "ic_pack", st));
   if (keep && !train) {
     IcRunning r;
     r.at[0] = 0;

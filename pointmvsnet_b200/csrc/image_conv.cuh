@@ -203,7 +203,6 @@ struct IcLayerPlan {
 struct IcPlan {
   IcLayerPlan L[IC_LAYERS];
   int h[4], w[4];  // level sizes
-  long long wtotal;
   int keep;
   size_t y[IC_BN], ss[IC_BN];  // workspace offsets of each BatchNorm layer's pre-BatchNorm output and scale / shift
   size_t part, rs, total;
@@ -232,7 +231,6 @@ int ic_plan(int B, int V, int H, int W, int base, int keep, IcPlan& p) {
                                   {3, 1, 8 * b, 8 * b, 16, 4}};
   const long long N = (long long)B * V;
   size_t off = 0, ymax = 0, partmax = 0;
-  p.wtotal = 0;
   p.keep = keep;
   for (int l = 0; l < IC_LAYERS; ++l) {
     IcLayerPlan& q = p.L[l];
@@ -247,7 +245,6 @@ int ic_plan(int B, int V, int H, int W, int base, int keep, IcPlan& p) {
     const long long wn = (long long)q.k * q.k * q.cin * q.cout;
     q.w = off;
     off += up256(wn * 4);
-    p.wtotal += wn;
     if (l < IC_BN) {
       ymax = std::max(ymax, (size_t)N * q.Ho * q.Wo * q.cout * 4);
       partmax = std::max(partmax, (size_t)V * 2 * q.cout * (size_t)q.nparts * 8);
@@ -284,8 +281,6 @@ int ic_plan(int B, int V, int H, int W, int base, int keep, IcPlan& p) {
   p.total = off;
   return PMVS_OK;
 }
-
-bool ic_finite_nonneg(float t) { return t >= 0.f && t <= 3.402823466e38f; }
 
 }  // namespace
 

@@ -38,19 +38,6 @@ const char* const IB_WGRAD[IC_LAYERS] = {"icb_wgrad0_0", "icb_wgrad0_1", "icb_wg
                                          "icb_wgrad1_2", "icb_wgrad2_0", "icb_wgrad2_1", "icb_wgrad2_2",
                                          "icb_wgrad3_0", "icb_wgrad3_1", "icb_wgrad3_2"};
 
-// fixed-order tree sum of one value per thread over a block of IB_THREADS; the result is valid in thread 0
-__device__ __forceinline__ double ib_block_sum(double v, double* red) {
-  red[threadIdx.x] = v;
-  __syncthreads();
-  for (int o = IB_THREADS / 2; o > 0; o >>= 1) {
-    if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
-    __syncthreads();
-  }
-  const double r = red[0];
-  __syncthreads();
-  return r;
-}
-
 // The data gradient of a stride-1 layer: the forward's convolution on G without the BatchNorm prologue.
 template <int K, int CIN, int COUT, int CO, int PX>
 __global__ void __launch_bounds__(IC_THREADS) ic_dgrad_kernel(const IcArgs a) {
@@ -128,27 +115,6 @@ __global__ void __launch_bounds__(IC_THREADS) ic_dgrad_s2_kernel(const IcArgs a)
 #pragma unroll
     for (int c = 0; c < CO; c += 4)
       *reinterpret_cast<float4*>(yp + c) = make_float4(acc[p][c], acc[p][c + 1], acc[p][c + 2], acc[p][c + 3]);
-  }
-}
-
-// PyTorch Conv2d weights [Cout, Cin, K, K] -> [K*K][Cout][Cin], the packing of the data-gradient convolutions (input
-// G with Cout channels, output Cin channels); stride-1 layers with the taps flipped (tap -> K*K - 1 - tap).
-struct IcPackB {
-  const float* src[IC_LAYERS];
-  long long end[IC_LAYERS];  // running sum of the layers' element counts (layer 0 has none)
-  long long dst_off[IC_LAYERS];
-  int cin[IC_LAYERS], cout[IC_LAYERS], taps[IC_LAYERS], flip[IC_LAYERS];
-};
-
-__global__ void ic_pack_bwd_kernel(const IcPackB p, float* __restrict__ dst, long long total) {
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    int l = 0;
-    while (i >= p.end[l]) ++l;
-    const long long e = i - (l > 0 ? p.end[l - 1] : 0);
-    const int cout = p.cout[l], cin = p.cin[l], taps = p.taps[l];
-    const int ci = (int)(e % cin), co = (int)((e / cin) % cout), tap = (int)(e / ((long long)cout * cin));
-    const int st = p.flip[l] ? taps - 1 - tap : tap;
-    dst[p.dst_off[l] + e] = __ldg(p.src[l] + ((long long)co * cin + ci) * taps + st);
   }
 }
 
@@ -256,8 +222,8 @@ __global__ void __launch_bounds__(IB_THREADS)
       s += pv[(long long)c * nparts + i];
       t += pv[(long long)(C + c) * nparts + i];
     }
-    s = ib_block_sum(s, red);
-    t = ib_block_sum(t, red);
+    s = block_sum<IB_THREADS>(s, red);
+    t = block_sum<IB_THREADS>(t, red);
     if (threadIdx.x == 0) {
       double mean, var;
       if (sums != nullptr) {
@@ -446,7 +412,6 @@ struct IbPlan {
   size_t wb[IC_LAYERS];        // packed data-gradient weights (layers 1 .. 10)
   size_t buf[2];               // ping-pong gradient buffers: dA_l, overwritten by G_l; the data gradient goes to the other
   size_t bn_part, kc, w_part, total;
-  long long wtotal;
   int bn_chunk[IC_BN], bn_nch[IC_BN];  // BatchNorm backward: pixels per CTA, CTAs per image
   int w_chunk[IC_LAYERS], w_nch[IC_LAYERS];  // weight gradients: output pixels per CTA, CTAs per image
 };
@@ -455,14 +420,12 @@ int ib_plan(int B, int V, int H, int W, int base, IbPlan& p) {
   PMVS_TRY(ic_plan(B, V, H, W, base, 1, p.f));
   const long long N = (long long)B * V;
   size_t off = 0, bufmax = 0, bn_part = 0, w_part = 0;
-  p.wtotal = 0;
   p.wb[0] = 0;
   for (int l = 1; l < IC_LAYERS; ++l) {
     const IcLayerPlan& q = p.f.L[l];
     const long long wn = (long long)q.k * q.k * q.cin * q.cout;
     p.wb[l] = off;
     off += up256(wn * 4);
-    p.wtotal += wn;
   }
   for (int l = 0; l < IC_LAYERS; ++l) {
     const IcLayerPlan& q = p.f.L[l];
@@ -550,15 +513,6 @@ int ib_launch_wgrad(int l, const IcWgArgs& a, int N, cudaStream_t st) {
   }
 }
 
-int ib_zero(float* p, size_t n, cudaStream_t st) {
-  if (cudaMemsetAsync(p, 0, n * sizeof(float), st) != cudaSuccess) {
-    cudaGetLastError();
-    set_error("image_conv_backward: cudaMemsetAsync failed");
-    return PMVS_ERR_CUDA;
-  }
-  return PMVS_OK;
-}
-
 }  // namespace
 
 }  // namespace pmvs
@@ -587,22 +541,18 @@ extern "C" int pmvs_image_conv_backward(const float* img, const pmvs_image_weigh
   for (int l = 0; l < IC_BN; ++l) {
     PMVS_REQUIRE(wt->gamma[l] && wt->beta[l], "image_conv_backward: NULL BatchNorm affine of layer %d", l);
     PMVS_REQUIRE(grads->gamma[l] && grads->beta[l], "image_conv_backward: NULL BatchNorm gradient of layer %d", l);
-    PMVS_REQUIRE(ic_finite_nonneg(wt->eps[l]), "image_conv_backward: eps of layer %d = %g (finite, >= 0)", l,
+    PMVS_REQUIRE(finite_nonneg(wt->eps[l]), "image_conv_backward: eps of layer %d = %g (finite, >= 0)", l,
                  (double)wt->eps[l]);
   }
   PMVS_REQUIRE(!train || (long long)B * p.f.h[3] * p.f.w[3] >= 2,
                "image_conv_backward: train mode needs more than 1 value per channel at the coarsest level "
                "(B*h3*w3 = %lld)", (long long)B * p.f.h[3] * p.f.w[3]);
   PMVS_REQUIRE(!train || batch_sums, "image_conv_backward: train mode needs the forward's batch_sums");
-  PMVS_REQUIRE(((uintptr_t)workspace & 255) == 0 && ((uintptr_t)fwd_workspace & 255) == 0,
-               "image_conv_backward: workspace and fwd_workspace must be 256-byte aligned");
+  PMVS_REQUIRE(((uintptr_t)fwd_workspace & 255) == 0, "image_conv_backward: fwd_workspace must be 256-byte aligned");
   for (int k = 0; k < 4; ++k)
     PMVS_REQUIRE(((uintptr_t)grad_level[k] & 15) == 0, "image_conv_backward: grad_level[%d] must be 16-byte aligned",
                  k);
-  if (workspace_bytes < p.total) {
-    set_error("image_conv_backward: workspace %zu bytes < required %zu", workspace_bytes, p.total);
-    return PMVS_ERR_WORKSPACE;
-  }
+  PMVS_TRY(check_workspace("image_conv_backward", workspace, workspace_bytes, p.total));
   cudaStream_t st = (cudaStream_t)stream;
   const char* fw = (const char*)fwd_workspace;
   char* ws = (char*)workspace;
@@ -615,32 +565,27 @@ extern "C" int pmvs_image_conv_backward(const float* img, const pmvs_image_weigh
     if (grad_level[k] != nullptr) top = IC_LEVEL_LAYER[k];
   for (int l = top + 1; l < IC_LAYERS; ++l) {
     const IcLayerPlan& q = F[l];
-    PMVS_TRY(ib_zero(grads->weight[l], (size_t)q.k * q.k * q.cin * q.cout, st));
+    const char* what = "image_conv_backward";
+    PMVS_TRY(memset_async(what, grads->weight[l], (size_t)q.k * q.k * q.cin * q.cout * sizeof(float), st));
     if (l < IC_BN) {
-      PMVS_TRY(ib_zero(grads->gamma[l], q.cout, st));
-      PMVS_TRY(ib_zero(grads->beta[l], q.cout, st));
+      PMVS_TRY(memset_async(what, grads->gamma[l], q.cout * sizeof(float), st));
+      PMVS_TRY(memset_async(what, grads->beta[l], q.cout * sizeof(float), st));
     }
   }
   if (top < 0) return PMVS_OK;
 
   if (top >= 1) {
-    IcPackB pk;
-    memset(&pk, 0, sizeof(pk));
-    long long run = 0;
+    // PyTorch Conv2d weights [Cout, Cin, K, K] -> [K*K][Cout][Cin], the packing of the data-gradient convolutions
+    // (input G with Cout channels, output Cin channels) of layers 1 .. top; stride-1 layers with the taps flipped
+    // (tap -> K*K - 1 - tap)
+    PackTable pk;
     for (int l = 1; l <= top; ++l) {
       const IcLayerPlan& q = F[l];
-      pk.src[l] = wt->weight[l];
-      run += (long long)q.k * q.k * q.cin * q.cout;
-      pk.end[l] = run;
-      pk.dst_off[l] = (long long)(p.wb[l] / 4);
-      pk.cin[l] = q.cin;
-      pk.cout[l] = q.cout;
-      pk.taps[l] = q.k * q.k;
-      pk.flip[l] = q.s == 1;
+      const int taps = q.k * q.k, flip = q.s == 1;
+      pk.L[l - 1] = {wt->weight[l], (long long)(p.wb[l] / 4), {taps, q.cout, q.cin}, flip ? taps - 1 : 0,
+                     {flip ? -1 : 1, q.cin * taps, taps}};
     }
-    prof_begin("icb_pack", st);
-    ic_pack_bwd_kernel<<<cdiv(run, 256), 256, 0, st>>>(pk, (float*)ws, run);
-    PMVS_TRY(check_launch("ic_pack_bwd_kernel", st));
+    PMVS_TRY(launch_pack(pk, top, (float*)ws, "icb_pack", st));
   }
 
   size_t sums_at[IC_BN], sums_stride = 0;

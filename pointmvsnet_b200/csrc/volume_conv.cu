@@ -24,27 +24,6 @@ const char* const VC_NAMES[VC_LAYERS] = {"vc_conv0_1", "vc_conv1_0", "vc_conv2_0
 // dependency order of the forward
 const int VC_ORDER[VC_LAYERS] = {L0_1, L1_0, L1_1, L2_0, L2_1, L3_0, L3_1, L4_0, L5_0, L6_0, L6_2};
 
-// PyTorch layouts -> [Cin][27][Cout] for every layer in one launch
-struct VcPack {
-  const float* src[VC_LAYERS];
-  long long end[VC_LAYERS];  // running sum of the layers' element counts
-  long long dst_off[VC_LAYERS];
-  int cin[VC_LAYERS], cout[VC_LAYERS], transposed[VC_LAYERS];
-};
-
-__global__ void vc_pack_kernel(const VcPack p, float* __restrict__ dst, long long total) {
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    int l = 0;
-    while (i >= p.end[l]) ++l;
-    const long long e = i - (l > 0 ? p.end[l - 1] : 0);
-    const int cout = p.cout[l], cin = p.cin[l];
-    const int co = (int)(e % cout), tap = (int)((e / cout) % VC_TAPS), ci = (int)(e / ((long long)cout * VC_TAPS));
-    const long long s = p.transposed[l] ? ((long long)ci * cout + co) * VC_TAPS + tap   // ConvTranspose3d [Cin,Cout,.]
-                                        : ((long long)co * cin + ci) * VC_TAPS + tap;  // Conv3d [Cout,Cin,.]
-    dst[p.dst_off[l] + e] = __ldg(p.src[l] + s);
-  }
-}
-
 // ---- depth regression: softmax(-x) over D, expectation against torch.linspace's planes, probability map ----------
 
 __global__ void __launch_bounds__(256)
@@ -100,8 +79,6 @@ int launch_layer(int l, const VcArgs& a, const VcLayerPlan& q, int B, cudaStream
   }
 }
 
-bool finite_nonneg(float t) { return t >= 0.f && t <= FLT_MAX; }
-
 }  // namespace
 
 }  // namespace pmvs
@@ -127,28 +104,19 @@ extern "C" int pmvs_volume_conv(const float* x, const pmvs_volume_weights* wt, i
                  "volume_conv: eval mode needs the running statistics of layer %d", l);
     PMVS_REQUIRE(finite_nonneg(wt->eps[l]), "volume_conv: eps of layer %d = %g (finite, >= 0)", l, (double)wt->eps[l]);
   }
-  PMVS_REQUIRE(((uintptr_t)workspace & 255) == 0, "volume_conv: workspace must be 256-byte aligned");
-  if (workspace_bytes < p.total) {
-    set_error("volume_conv: workspace %zu bytes < required %zu", workspace_bytes, p.total);
-    return PMVS_ERR_WORKSPACE;
-  }
+  PMVS_TRY(check_workspace("volume_conv", workspace, workspace_bytes, p.total));
   cudaStream_t st = (cudaStream_t)stream;
   char* ws = (char*)workspace;
 
-  VcPack pk;
-  long long run = 0;
+  // PyTorch layouts -> [Cin][27][Cout]: Conv3d [Cout, Cin, 27], ConvTranspose3d [Cin, Cout, 27]
+  PackTable pk;
   for (int l = 0; l < VC_LAYERS; ++l) {
-    pk.src[l] = wt->weight[l];
-    run += (long long)p.L[l].cin * VC_TAPS * p.L[l].cout;
-    pk.end[l] = run;
-    pk.dst_off[l] = (long long)(p.L[l].w / 4);
-    pk.cin[l] = p.L[l].cin;
-    pk.cout[l] = p.L[l].cout;
-    pk.transposed[l] = p.L[l].mode == VC_T2;
+    const VcLayerPlan& q = p.L[l];
+    const bool t = q.mode == VC_T2;
+    pk.L[l] = {wt->weight[l], (long long)(q.w / 4), {q.cin, VC_TAPS, q.cout}, 0,
+               {t ? q.cout * VC_TAPS : VC_TAPS, 1, t ? VC_TAPS : q.cin * VC_TAPS}};
   }
-  prof_begin("vc_pack", st);
-  vc_pack_kernel<<<cdiv(p.wtotal, 256), 256, 0, st>>>(pk, (float*)ws, p.wtotal);
-  PMVS_TRY(check_launch("vc_pack_kernel", st));
+  PMVS_TRY(launch_pack(pk, VC_LAYERS, (float*)ws, "vc_pack", st));
 
   size_t sums_off = 0;
   size_t sums_at[VC_BN];

@@ -247,7 +247,57 @@ __global__ void __launch_bounds__(VC_FIN_THREADS)
   shift[c] = (float)((double)beta[c] - mean * sc);
 }
 
-inline size_t up256(size_t x) { return (x + 255) & ~(size_t)255; }
+// fixed-order tree sum of one value per thread over a block of THREADS; `red` is free again when it returns
+template <int THREADS>
+__device__ __forceinline__ double block_sum(double v, double* red) {
+  red[threadIdx.x] = v;
+  __syncthreads();
+  for (int o = THREADS / 2; o > 0; o >>= 1) {
+    if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
+    __syncthreads();
+  }
+  const double r = red[0];
+  __syncthreads();
+  return r;
+}
+
+// The weight repacking of the conv towers (VolumeConv, ImageConv; forward and backward), every layer in one launch:
+// dst[dst_off + (i0 * n1 + i1) * n2 + i2] = src[base + i0 * s0 + i1 * s1 + i2 * s2] for i < n.  A negative stride
+// with base at the far end walks that axis backwards (the flipped taps of the stride-1 data gradients).
+constexpr int PACK_MAX_LAYERS = 11;
+struct PackLayer {
+  const float* src;
+  long long dst_off;
+  int n[3];
+  long long base, s[3];
+};
+struct PackTable {
+  PackLayer L[PACK_MAX_LAYERS];
+  long long end[PACK_MAX_LAYERS];  // running sum of the layers' element counts
+};
+
+__global__ void pack_kernel(const PackTable t, float* __restrict__ dst, long long total) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    int l = 0;
+    while (i >= t.end[l]) ++l;
+    const PackLayer& L = t.L[l];
+    const long long e = i - (l > 0 ? t.end[l - 1] : 0);
+    const int i2 = (int)(e % L.n[2]), i1 = (int)((e / L.n[2]) % L.n[1]), i0 = (int)(e / ((long long)L.n[1] * L.n[2]));
+    dst[L.dst_off + e] = __ldg(L.src + L.base + i0 * L.s[0] + i1 * L.s[1] + i2 * L.s[2]);
+  }
+}
+
+// the first n layers of t (end is filled here)
+int launch_pack(PackTable& t, int n, float* dst, const char* name, cudaStream_t st) {
+  long long total = 0;
+  for (int l = 0; l < n; ++l) {
+    total += (long long)t.L[l].n[0] * t.L[l].n[1] * t.L[l].n[2];
+    t.end[l] = total;
+  }
+  prof_begin(name, st);
+  pack_kernel<<<cdiv(total, 256), 256, 0, st>>>(t, dst, total);
+  return check_launch(name, st);
+}
 
 struct VcLayerPlan {
   int mode, cin, cout, co, vd, src;
@@ -259,7 +309,6 @@ struct VcLayerPlan {
 
 struct VcPlan {
   VcLayerPlan L[VC_LAYERS];
-  long long wtotal;
   size_t total;
 };
 
@@ -280,7 +329,6 @@ int vc_plan(int B, int Cin, int base, int D, int H, int W, VcPlan& p) {
       {VC_T2, 4 * b, 2 * b, 2, 1, 8, 4, 2},  {VC_T2, 2 * b, b, 1, 0, 8, 4, 2},
       {VC_S1, b, 1, 0, 0, 1, 8, 2}};
   size_t off = 0;
-  p.wtotal = 0;
   for (int l = 0; l < VC_LAYERS; ++l) {
     VcLayerPlan& q = p.L[l];
     q.mode = spec[l][0]; q.cin = spec[l][1]; q.cout = spec[l][2];
@@ -297,7 +345,6 @@ int vc_plan(int B, int Cin, int base, int D, int H, int W, VcPlan& p) {
     const long long wn = (long long)q.cin * VC_TAPS * q.cout;
     q.w = off;
     off += up256(wn * 4);
-    p.wtotal += wn;
   }
   for (int l = 0; l < VC_BN; ++l) {
     VcLayerPlan& q = p.L[l];

@@ -34,17 +34,6 @@ const char* const VB_WGRAD[VC_LAYERS] = {"vcb_wgrad0_1", "vcb_wgrad1_0", "vcb_wg
 // reverse dependency order of the forward
 const int VB_ORDER[VC_LAYERS] = {L6_2, L6_0, L5_0, L4_0, L3_1, L3_0, L2_1, L2_0, L1_1, L1_0, L0_1};
 
-// fixed-order tree sum of one value per thread over a block of VB_THREADS; the result is valid in thread 0
-__device__ __forceinline__ double block_sum(double v, double* red) {
-  red[threadIdx.x] = v;
-  __syncthreads();
-  for (int o = VB_THREADS / 2; o > 0; o >>= 1) {
-    if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
-    __syncthreads();
-  }
-  return red[0];
-}
-
 __device__ __forceinline__ float relu_grad(float y, float sc, float sh, const float* da, const float* db, long long i) {
   float g = __ldg(da + i);
   if (db != nullptr) g += __ldg(db + i);  // two consumers: their data gradients added in a fixed order
@@ -72,10 +61,9 @@ __global__ void __launch_bounds__(VB_THREADS)
     t += (double)dz * ((double)yv - mean);
   }
   const long long nparts = (long long)gridDim.x * gridDim.z, at = (long long)b * gridDim.x + blockIdx.x;
-  s = block_sum(s, red);
+  s = block_sum<VB_THREADS>(s, red);
   if (threadIdx.x == 0) part[(long long)c * nparts + at] = s;
-  __syncthreads();
-  t = block_sum(t, red);
+  t = block_sum<VB_THREADS>(t, red);
   if (threadIdx.x == 0) part[(long long)(C + c) * nparts + at] = t;
 }
 
@@ -94,9 +82,8 @@ __global__ void __launch_bounds__(VB_THREADS)
     s += part[(long long)c * nparts + i];
     t += part[(long long)(C + c) * nparts + i];
   }
-  s = block_sum(s, red);
-  __syncthreads();
-  t = block_sum(t, red);
+  s = block_sum<VB_THREADS>(s, red);
+  t = block_sum<VB_THREADS>(t, red);
   if (threadIdx.x != 0) return;
   double mean, var;
   if (sums != nullptr) {  // the forward's statistics, recomputed from its sums exactly as vc_bn_finalize_kernel does
@@ -252,30 +239,6 @@ __global__ void vc_wgrad_finalize_kernel(const double* __restrict__ part, int np
   dw[transposed ? (ci * Cout + co) * VC_TAPS + tap : (co * Cin + ci) * VC_TAPS + tap] = (float)s;
 }
 
-// PyTorch layouts -> [Cout][27][Cin], the packing of the data-gradient convolutions (input G, output Cin channels):
-// stride-1 layers with the taps of all three axes flipped (tap -> 26 - tap).
-struct VcPackB {
-  const float* src[VC_LAYERS];
-  long long end[VC_LAYERS];  // running sum of the layers' element counts
-  long long dst_off[VC_LAYERS];
-  int cin[VC_LAYERS], cout[VC_LAYERS], mode[VC_LAYERS];
-};
-
-__global__ void vc_pack_bwd_kernel(const VcPackB p, float* __restrict__ dst, long long total) {
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    int l = 0;
-    while (i >= p.end[l]) ++l;
-    const long long e = i - (l > 0 ? p.end[l - 1] : 0);
-    const int cout = p.cout[l], cin = p.cin[l];
-    const int ci = (int)(e % cin), tap = (int)((e / cin) % VC_TAPS), co = (int)(e / ((long long)cin * VC_TAPS));
-    long long s;
-    if (p.mode[l] == VC_T2) s = ((long long)ci * cout + co) * VC_TAPS + tap;            // ConvTranspose3d [Cin,Cout,.]
-    else if (p.mode[l] == VC_S2) s = ((long long)co * cin + ci) * VC_TAPS + tap;        // Conv3d [Cout,Cin,.]
-    else s = ((long long)co * cin + ci) * VC_TAPS + (VC_TAPS - 1 - tap);                // flipped
-    dst[p.dst_off[l] + e] = __ldg(p.src[l] + s);
-  }
-}
-
 __global__ void vc_add_kernel(float4* __restrict__ dst, const float4* __restrict__ src, long long n4) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
     float4 a = dst[i];
@@ -329,21 +292,18 @@ struct VbLayer {
 struct VbPlan {
   VcPlan f;
   VbLayer L[VC_LAYERS];
-  long long wtotal;
   size_t bn_part, w_part, total;
 };
 
 int vb_plan(int B, int Cin, int base, int D, int H, int W, VbPlan& p) {
   PMVS_TRY(vc_plan(B, Cin, base, D, H, W, p.f));
   size_t off = 0, bn_part = 0, w_part = 0;
-  p.wtotal = 0;
   for (int l = 0; l < VC_LAYERS; ++l) {
     const VcLayerPlan& q = p.f.L[l];
     VbLayer& r = p.L[l];
     const long long wn = (long long)q.cin * VC_TAPS * q.cout;
     r.wb = off;
     off += up256(wn * 4);
-    p.wtotal += wn;
     r.co = l == L6_2 ? 1 : 8;
     if (q.mode == VC_T2) { r.pd = q.Di; r.ph = q.Hi; r.pw = q.Wi; }
     else { r.pd = q.Do; r.ph = q.Ho; r.pw = q.Wo; }
@@ -424,8 +384,6 @@ int launch_wgrad_layer(int l, const VcWgArgs& a, int B, cudaStream_t st) {
   }
 }
 
-bool finite_nonneg(float t) { return t >= 0.f && t <= FLT_MAX; }
-
 }  // namespace
 
 }  // namespace pmvs
@@ -460,31 +418,24 @@ extern "C" int pmvs_volume_conv_backward(const float* x, const pmvs_volume_weigh
                  (double)wt->eps[l]);
   }
   PMVS_REQUIRE(!train || batch_sums, "volume_conv_backward: train mode needs the forward's batch_sums");
-  PMVS_REQUIRE(((uintptr_t)workspace & 255) == 0 && ((uintptr_t)fwd_workspace & 255) == 0,
-               "volume_conv_backward: workspace and fwd_workspace must be 256-byte aligned");
-  if (workspace_bytes < p.total) {
-    set_error("volume_conv_backward: workspace %zu bytes < required %zu", workspace_bytes, p.total);
-    return PMVS_ERR_WORKSPACE;
-  }
+  PMVS_REQUIRE(((uintptr_t)fwd_workspace & 255) == 0, "volume_conv_backward: fwd_workspace must be 256-byte aligned");
+  PMVS_TRY(check_workspace("volume_conv_backward", workspace, workspace_bytes, p.total));
   cudaStream_t st = (cudaStream_t)stream;
   const char* fw = (const char*)fwd_workspace;
   char* ws = (char*)workspace;
   const VcLayerPlan* F = p.f.L;
 
-  VcPackB pk;
-  long long run = 0;
+  // PyTorch layouts -> [Cout][27][Cin], the packing of the data-gradient convolutions (input G, output Cin channels):
+  // ConvTranspose3d [Cin, Cout, 27], Conv3d [Cout, Cin, 27], stride-1 layers with the taps of all three axes flipped
+  // (tap -> 26 - tap)
+  PackTable pk;
   for (int l = 0; l < VC_LAYERS; ++l) {
-    pk.src[l] = wt->weight[l];
-    run += (long long)F[l].cin * VC_TAPS * F[l].cout;
-    pk.end[l] = run;
-    pk.dst_off[l] = (long long)(p.L[l].wb / 4);
-    pk.cin[l] = F[l].cin;
-    pk.cout[l] = F[l].cout;
-    pk.mode[l] = F[l].mode;
+    const VcLayerPlan& q = F[l];
+    const bool t = q.mode == VC_T2, s1 = q.mode == VC_S1;
+    pk.L[l] = {wt->weight[l], (long long)(p.L[l].wb / 4), {q.cout, VC_TAPS, q.cin}, s1 ? VC_TAPS - 1 : 0,
+               {t ? VC_TAPS : q.cin * VC_TAPS, s1 ? -1 : 1, t ? q.cout * VC_TAPS : VC_TAPS}};
   }
-  prof_begin("vcb_pack", st);
-  vc_pack_bwd_kernel<<<cdiv(p.wtotal, 256), 256, 0, st>>>(pk, (float*)ws, p.wtotal);
-  PMVS_TRY(check_launch("vc_pack_bwd_kernel", st));
+  PMVS_TRY(launch_pack(pk, VC_LAYERS, (float*)ws, "vcb_pack", st));
 
   size_t sums_at[VC_BN], sums_off = 0;
   for (int l = 0; l < VC_BN; ++l) {

@@ -42,7 +42,7 @@ def enable_training(enabled=True):
 
 def training_enabled():
     """the triple of the three switches, in enable_training's order"""
-    return (networks._backward_enabled, networks.volume_backward_enabled(), networks.image_backward_enabled())
+    return (networks.backward_enabled(), networks.volume_backward_enabled(), networks.image_backward_enabled())
 
 
 class PointMVSNet(nn.Module):

@@ -13,14 +13,19 @@ import torch
 import torch.nn as nn
 from torch.autograd.function import once_differentiable
 
-from ._lib import (lib, check, stream_ptr, ptr, require_cuda, f32c, ImageGrads, ImageWeights, VolumeWeights,
-                   VolumeGrads)
+from ._lib import lib, check, stream_ptr, ptr, require_cuda, f32c, workspace, ConvBnGrads, ConvBnWeights
 from .nn.conv import Conv2d, Conv3d, Deconv3d
 
 _SUPPORTED_COUT = (16, 32, 64, 128)
-_backward_enabled = False
-_volume_backward_enabled = False
-_image_backward_enabled = False
+# the process-wide training switches: "edge" (EdgeConv, EdgeConvNoC, PointFlow), "volume" (VolumeConv, coarse_depth)
+# and "image" (ImageConv.forward_views)
+_backward = {"edge": False, "volume": False, "image": False}
+
+
+def _enable(which, enabled):
+    prev = _backward[which]
+    _backward[which] = bool(enabled)
+    return prev
 
 
 def enable_backward(enabled=True):
@@ -34,10 +39,11 @@ def enable_backward(enabled=True):
     for ``PointFlow`` the iteration's whole workspace (``pmvs_point_flow_workspace_bytes``).  ``PointFlow`` takes one
     cloud per call under autograd (the train branch, or the test branch at scale 0.125).  Under ``torch.no_grad()``
     the switch has no effect."""
-    global _backward_enabled
-    prev = _backward_enabled
-    _backward_enabled = bool(enabled)
-    return prev
+    return _enable("edge", enabled)
+
+
+def backward_enabled():
+    return _backward["edge"]
 
 
 def enable_volume_backward(enabled=True):
@@ -52,14 +58,11 @@ def enable_volume_backward(enabled=True):
     [B,64,48,64,80]) and its input alive until backward runs; the backward then allocates its own workspace
     (``pmvs_volume_conv_backward_workspace_bytes``, about 100 MB per batch element at that shape) for the duration of
     the call.  Under ``torch.no_grad()`` the switch has no effect."""
-    global _volume_backward_enabled
-    prev = _volume_backward_enabled
-    _volume_backward_enabled = bool(enabled)
-    return prev
+    return _enable("volume", enabled)
 
 
 def volume_backward_enabled():
-    return _volume_backward_enabled
+    return _backward["volume"]
 
 
 def enable_image_backward(enabled=True):
@@ -74,14 +77,11 @@ def enable_image_backward(enabled=True):
     bytes, 566 MB per tower at B = 4, V = 3, 512 x 640) alive until backward runs; the backward then allocates its own
     workspace (``pmvs_image_conv_backward_workspace_bytes``, about 64 * B * V * H * W bytes) for the duration of the
     call.  Under ``torch.no_grad()`` the switch has no effect."""
-    global _image_backward_enabled
-    prev = _image_backward_enabled
-    _image_backward_enabled = bool(enabled)
-    return prev
+    return _enable("image", enabled)
 
 
 def image_backward_enabled():
-    return _image_backward_enabled
+    return _backward["image"]
 
 
 def _edge_layer(mod, feature, knn_inds, concat_central):
@@ -89,7 +89,7 @@ def _edge_layer(mod, feature, knn_inds, concat_central):
     if feature.dim() != 3 or knn_inds.dim() != 3:
         raise RuntimeError("EdgeConv: feature must be [B,C,N] and knn_inds [B,N,K]")
     if torch.is_grad_enabled() and (feature.requires_grad or any(p.requires_grad for p in mod.parameters())):
-        if not _backward_enabled:
+        if not _backward["edge"]:
             # inference under torch.no_grad() is the supported mode (test.py:62); training needs enable_backward()
             raise NotImplementedError("pointmvsnet_b200 EdgeConv is forward-only; wrap the call in torch.no_grad() "
                                       "or call pointmvsnet_b200.networks.enable_backward()")
@@ -177,7 +177,7 @@ class _EdgeConvFn(torch.autograd.Function):
             dgamma = torch.empty_like(gamma)
             dbeta = torch.empty_like(beta)
             nbytes = lib.pmvs_edgeconv_pm_backward_workspace_bytes(B, N, K, cin, cout)
-            ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+            ws = workspace(nbytes, dev)
             check(lib.pmvs_edgeconv_pm_backward(ptr(x_pm), cin, ptr(idx32), ptr(ind), ptr(w12), ptr(gamma), ptr(beta),
                                                 eps, 1 if concat_central else 0, 1 if train else 0, ptr(le), ptr(stats),
                                                 ptr(dy_pm), ctot, ptr(dx_pm), cin, ptr(dw12), ptr(dgamma), ptr(dbeta),
@@ -314,7 +314,7 @@ class ImageConv(nn.Module):
         autograd."""
         grad = torch.is_grad_enabled() and (img_list.requires_grad or any(p.requires_grad for p in self.parameters()))
         if grad:
-            if not _image_backward_enabled:
+            if not _backward["image"]:
                 raise NotImplementedError("ImageConv.forward_views is forward-only; wrap the call in torch.no_grad() "
                                           "or run the per-view ImageConv.forward under autograd")
             if img_list.requires_grad:
@@ -343,17 +343,9 @@ class ImageConv(nn.Module):
         B, V, _, H, W = img_list.shape
         if min(B, V, H, W) < 1:
             raise RuntimeError("ImageConv.forward_views: empty input %s" % (tuple(img_list.shape),))
-        _, bns = self._image_layers()
-        train = _bn_train_mode(bns, "ImageConv")
         h3, w3 = _level_sizes(H, W)[3]
-        if train and B * h3 * w3 < 2:
-            raise RuntimeError("ImageConv.forward_views: in train mode the coarsest level needs more than 1 value per "
-                               "channel (B*h3*w3 = %d)" % (B * h3 * w3))
-        require_cuda(img_list, *self.parameters())
-        dev = img_list.device
-        if any(t.device != dev for t in list(self.parameters()) + list(self.buffers())):
-            raise RuntimeError("ImageConv.forward_views: the module's parameters and buffers must be on the input's "
-                               "device")
+        _check_tail(self, img_list, _bn_train_mode(self._image_layers()[1], "ImageConv"), "ImageConv.forward_views",
+                    B * h3 * w3, "B*h3*w3")
         return keys
 
     def _image_params(self):
@@ -403,7 +395,7 @@ def _image_forward(mod, img_list, keys, out, ctx):
     context) pmvs_image_conv_keep, whose workspace is saved on it with what the backward needs, and the list of the
     level buffers in `keys` order."""
     B, V, _, H, W = img_list.shape
-    convs, bns = mod._image_layers()
+    bns = mod._image_layers()[1]
     train = _bn_train_mode(bns, "ImageConv")
     sizes = _level_sizes(H, W)
     dev = img_list.device
@@ -423,7 +415,9 @@ def _image_forward(mod, img_list, keys, out, ctx):
         bufs[lev] = buf
         res[k] = buf.permute(0, 1, 4, 2, 3) if mod.channels_last else buf
     keep = []
-    wt = _conv_bn_weights(ImageWeights(), [c.weight for c in convs], bns, train, keep)
+    eps = [float(bn.eps) for bn in bns]
+    running = None if train else [(bn.running_mean, bn.running_var) for bn in bns]
+    wt = _conv_bn_weights(mod._image_params(), eps, running, keep)
     img = img_list.contiguous()
     couts = [bn.num_features for bn in bns]
     sums = torch.empty(V, 2 * sum(couts), device=dev, dtype=torch.float64) if train else None
@@ -432,24 +426,18 @@ def _image_forward(mod, img_list, keys, out, ctx):
                      (lib.pmvs_image_conv_keep_workspace_bytes, lib.pmvs_image_conv_keep))
     with torch.cuda.device(dev):
         nbytes = int(size_fn(B, V, H, W, mod.base_channels))
-        if nbytes == 0:
-            check(1)
-        wsp = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+        wsp = workspace(nbytes, dev)
         check(call(ptr(img), ctypes.byref(wt), 1 if train else 0, ctypes.byref(levels), 1 if mod.channels_last else 0,
                    ptr(sums), ptr(wsp), nbytes, B, V, H, W, mod.base_channels, stream_ptr()))
     if ctx is not None:
         ctx.img, ctx.ws, ctx.sums, ctx.train = img, wsp, sums, train
-        ctx.eps = [float(bn.eps) for bn in bns]
+        ctx.eps = eps
         ctx.shape = (B, V, H, W, mod.base_channels)
         ctx.channels_last = mod.channels_last
         ctx.levels = [_IMAGE_LEVELS.index(k) for k in keys]
     if train:
-        key = (B, H, W, str(dev))
-        if getattr(mod, "_pmvs_counts", (None,))[0] != key:  # one small upload per shape, not per call
-            n = torch.cat([torch.full((c,), float(B * sizes[l][0] * sizes[l][1]), dtype=torch.float64)
-                           for c, l in zip(couts, _IMAGE_LEVEL)]).to(dev)
-            object.__setattr__(mod, "_pmvs_counts", (key, n))
-        _update_running_rows(bns, sums, couts, mod._pmvs_counts[1])
+        n = _bn_counts(mod, (B, H, W, str(dev)), couts, [B * sizes[l][0] * sizes[l][1] for l in _IMAGE_LEVEL])
+        _update_running_rows(bns, sums, couts, n)
     return res if ctx is None else [bufs[_IMAGE_LEVELS.index(k)] for k in keys]
 
 
@@ -487,29 +475,12 @@ class _ImageConvFn(torch.autograd.Function):
         if top < 0:
             return tuple(res + [None] * len(params))
         keep = []
-
-        def p32(t):
-            t = f32c(t.detach())
-            keep.append(t)
-            return t.data_ptr()
-
-        wt = ImageWeights()
-        for l in range(11):
-            wt.weight[l] = p32(params[l])
-        for l in range(10):
-            wt.gamma[l], wt.beta[l], wt.eps[l] = p32(params[11 + l]), p32(params[21 + l]), ctx.eps[l]
-        grads = [torch.empty(p.shape, device=dev, dtype=torch.float32) for p in params]
-        g = ImageGrads()
-        for l in range(11):
-            g.weight[l] = grads[l].data_ptr()
-        for l in range(10):
-            g.gamma[l], g.beta[l] = grads[11 + l].data_ptr(), grads[21 + l].data_ptr()
+        wt = _conv_bn_weights(params, ctx.eps, None, keep)  # eval mode: the kernels read the forward's kept copy
+        grads, g = _conv_bn_grads(params, dev)
         lv = (ctypes.c_void_p * 4)(*[ptr(t) for t in levels])
         with torch.cuda.device(dev):
             nbytes = int(lib.pmvs_image_conv_backward_workspace_bytes(B, V, H, W, base))
-            if nbytes == 0:
-                check(1)
-            ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+            ws = workspace(nbytes, dev)
             check(lib.pmvs_image_conv_backward(ptr(img), ctypes.byref(wt), 1 if ctx.train else 0, ptr(ctx.ws),
                                                ptr(ctx.sums), ctypes.byref(lv), 1 if ctx.channels_last else 0,
                                                ctypes.byref(g), ptr(ws), nbytes, B, V, H, W, base, stream_ptr()))
@@ -576,7 +547,7 @@ class VolumeConv(nn.Module):
 
     def forward(self, x):
         if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters())):
-            if not _volume_backward_enabled:
+            if not _backward["volume"]:
                 raise NotImplementedError("pointmvsnet_b200 VolumeConv is forward-only; wrap the call in "
                                           "torch.no_grad() or call pointmvsnet_b200.networks.enable_volume_backward()")
             self._check_input(x)
@@ -602,39 +573,60 @@ class VolumeConv(nn.Module):
             raise RuntimeError("VolumeConv: input has %d channels, the module expects %d" % (C, self.in_channels))
         if B < 1 or min(D, H, W) < 8 or D % 8 or H % 8 or W % 8:
             raise RuntimeError("VolumeConv: D, h, w = %d, %d, %d must be positive multiples of 8" % (D, H, W))
-        if self._train_mode() and B * (D // 8) * (H // 8) * (W // 8) < 2:
-            raise RuntimeError("VolumeConv: in train mode the coarsest level needs more than 1 value per channel "
-                               "(B*D*h*w/512 = %d)" % (B * (D // 8) * (H // 8) * (W // 8)))
-        require_cuda(x, *self.parameters())
-        dev = x.device
-        if any(t.device != dev for t in list(self.parameters()) + list(self.buffers())):
-            raise RuntimeError("VolumeConv: the module's parameters and buffers must be on the input's device")
+        _check_tail(self, x, self._train_mode(), "VolumeConv", B * (D // 8) * (H // 8) * (W // 8), "B*D*h*w/512")
 
     def _train_mode(self):
         return _bn_train_mode(self._bns(), "VolumeConv")
 
 
-def _conv_bn_weights(wt, weights, bns, train, keep):
-    """fill `wt` (pmvs_volume_weights or pmvs_image_weights) from the conv weights and BatchNorm layers: fp32
-    contiguous copies (or the tensors themselves) appended to `keep`"""
+def _conv_bn_weights(params, eps, running, keep):
+    """pmvs_conv_bn_weights from a tower's 31 parameters (11 conv weights, 10 gammas, 10 betas), the 10 BatchNorm eps
+    and, for eval mode, the 10 (running_mean, running_var) pairs (None in train mode): fp32 contiguous copies (or the
+    tensors themselves) appended to `keep`"""
     def p32(t):
         t = f32c(t.detach())
         keep.append(t)
         return t.data_ptr()
 
-    for l, w in enumerate(weights):
-        wt.weight[l] = p32(w)
-    for l, bn in enumerate(bns):
-        wt.gamma[l], wt.beta[l], wt.eps[l] = p32(bn.weight), p32(bn.bias), float(bn.eps)
-        if not train:
-            wt.running_mean[l], wt.running_var[l] = p32(bn.running_mean), p32(bn.running_var)
+    wt = ConvBnWeights()
+    for l in range(11):
+        wt.weight[l] = p32(params[l])
+    for l in range(10):
+        wt.gamma[l], wt.beta[l], wt.eps[l] = p32(params[11 + l]), p32(params[21 + l]), eps[l]
+        if running is not None:
+            wt.running_mean[l], wt.running_var[l] = p32(running[l][0]), p32(running[l][1])
     return wt
 
 
-def _volume_weights(mod, train, keep):
-    """pmvs_volume_weights of `mod`"""
-    weights = [getattr(mod, n).weight if n == "conv6_2" else getattr(mod, n).conv.weight for n in _VOLUME_LAYERS]
-    return _conv_bn_weights(VolumeWeights(), weights, mod._bns(), train, keep)
+def _conv_bn_grads(params, dev):
+    """fp32 buffers shaped like a tower's 31 parameters and the pmvs_conv_bn_grads that points at them"""
+    grads = [torch.empty(p.shape, device=dev, dtype=torch.float32) for p in params]
+    g = ConvBnGrads()
+    for l in range(11):
+        g.weight[l] = grads[l].data_ptr()
+    for l in range(10):
+        g.gamma[l], g.beta[l] = grads[11 + l].data_ptr(), grads[21 + l].data_ptr()
+    return grads, g
+
+
+def _check_tail(mod, x, train, what, values, values_expr):
+    """the argument checks both towers end with: more than 1 value per channel at the coarsest level in train mode
+    (`values` of them, computed as `values_expr`), and a CUDA input with the module's tensors on its device"""
+    if train and values < 2:
+        raise RuntimeError("%s: in train mode the coarsest level needs more than 1 value per channel (%s = %d)"
+                           % (what, values_expr, values))
+    require_cuda(x, *mod.parameters())
+    if any(t.device != x.device for t in list(mod.parameters()) + list(mod.buffers())):
+        raise RuntimeError("%s: the module's parameters and buffers must be on the input's device" % what)
+
+
+def _bn_counts(mod, key, couts, counts):
+    """the per-channel value counts of a tower's BatchNorm layers (layer l: couts[l] channels of counts[l] values)
+    as one fp64 tensor on key[-1], the device; one small upload per shape `key`, not per call"""
+    if getattr(mod, "_pmvs_counts", (None,))[0] != key:
+        n = torch.cat([torch.full((c,), float(k), dtype=torch.float64) for c, k in zip(couts, counts)]).to(key[-1])
+        object.__setattr__(mod, "_pmvs_counts", (key, n))
+    return mod._pmvs_counts[1]
 
 
 def _volume_forward(mod, x, ctx):
@@ -645,16 +637,16 @@ def _volume_forward(mod, x, ctx):
     bns = mod._bns()
     dev = x.device
     keep = []
-    wt = _volume_weights(mod, train, keep)
+    eps = [float(bn.eps) for bn in bns]
+    running = None if train else [(bn.running_mean, bn.running_var) for bn in bns]
+    wt = _conv_bn_weights(mod._volume_params(), eps, running, keep)
     xin = x.contiguous()
     out = torch.empty(B, 1, D, H, W, device=dev, dtype=torch.float32)
     couts = [bn.num_features for bn in bns]
     sums = torch.empty(2 * sum(couts), device=dev, dtype=torch.float64) if train else None
     with torch.cuda.device(dev):
         nbytes = int(lib.pmvs_volume_conv_workspace_bytes(B, C, mod.base_channels, D, H, W))
-        if nbytes == 0:
-            check(1)
-        ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)  # the caching allocator aligns to 512 bytes
+        ws = workspace(nbytes, dev)
         check(lib.pmvs_volume_conv(ptr(xin), ctypes.byref(wt), 1 if train else 0, ptr(out), ptr(sums),
                                    ptr(ws), nbytes, B, C, mod.base_channels, D, H, W, stream_ptr()))
     if ctx is not None:
@@ -662,14 +654,10 @@ def _volume_forward(mod, x, ctx):
         # eval mode normalised with the running statistics: keep copies of what the forward read
         ctx.running = None if train else [(bn.running_mean.detach().float().clone(),
                                            bn.running_var.detach().float().clone()) for bn in bns]
-        ctx.eps = [float(bn.eps) for bn in bns]
+        ctx.eps = eps
     if train:
-        key = (B, D, H, W, str(dev))
-        if getattr(mod, "_pmvs_counts", (None,))[0] != key:  # one small upload per shape, not per call
-            n = torch.cat([torch.full((c,), float(B * (D >> l) * (H >> l) * (W >> l)), dtype=torch.float64)
-                           for c, l in zip(couts, _LEVEL)]).to(dev)
-            object.__setattr__(mod, "_pmvs_counts", (key, n))
-        _update_running_rows(bns, sums, couts, mod._pmvs_counts[1])
+        n = _bn_counts(mod, (B, D, H, W, str(dev)), couts, [B * (D >> l) * (H >> l) * (W >> l) for l in _LEVEL])
+        _update_running_rows(bns, sums, couts, n)
     return out
 
 
@@ -694,33 +682,14 @@ class _VolumeConvFn(torch.autograd.Function):
         B, C, D, H, W = x.shape
         dev = x.device
         keep = []
-
-        def p32(t):
-            t = f32c(t.detach())
-            keep.append(t)
-            return t.data_ptr()
-
-        wt = VolumeWeights()
-        for l in range(11):
-            wt.weight[l] = p32(params[l])
-        for l in range(10):
-            wt.gamma[l], wt.beta[l], wt.eps[l] = p32(params[11 + l]), p32(params[21 + l]), ctx.eps[l]
-            if not ctx.train:
-                wt.running_mean[l], wt.running_var[l] = p32(ctx.running[l][0]), p32(ctx.running[l][1])
+        wt = _conv_bn_weights(params, ctx.eps, ctx.running, keep)
         need_dx = ctx.needs_input_grad[0]
-        grads = [torch.empty(p.shape, device=dev, dtype=torch.float32) for p in params]
-        g = VolumeGrads()
-        for l in range(11):
-            g.weight[l] = grads[l].data_ptr()
-        for l in range(10):
-            g.gamma[l], g.beta[l] = grads[11 + l].data_ptr(), grads[21 + l].data_ptr()
+        grads, g = _conv_bn_grads(params, dev)
         dy = f32c(grad_out)
         with torch.cuda.device(dev):
             dx = torch.empty(B, C, D, H, W, device=dev, dtype=torch.float32) if need_dx else None
             nbytes = int(lib.pmvs_volume_conv_backward_workspace_bytes(B, C, ctx.base_channels, D, H, W))
-            if nbytes == 0:
-                check(1)
-            ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+            ws = workspace(nbytes, dev)
             check(lib.pmvs_volume_conv_backward(ptr(x), ctypes.byref(wt), 1 if ctx.train else 0, ptr(ctx.ws),
                                                 ptr(ctx.sums), ptr(dy), ptr(dx), ctypes.byref(g), ptr(ws), nbytes, B,
                                                 C, ctx.base_channels, D, H, W, stream_ptr()))

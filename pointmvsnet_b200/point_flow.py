@@ -187,10 +187,8 @@ class PointFlow(nn.Module):
 
     def _workspace(self, shape, device):
         need = lib.pmvs_point_flow_workspace_bytes(C.byref(shape))
-        if need == 0:
-            raise RuntimeError("libpmvs_b200: " + lib.pmvs_last_error().decode())
-        if self._ws is None or self._ws.numel() < need or self._ws.device != device:
-            self._ws = torch.empty(need, device=device, dtype=torch.uint8)
+        if need == 0 or self._ws is None or self._ws.numel() < need or self._ws.device != device:
+            self._ws = _lib.workspace(need, device)
         return self._ws, need
 
     # ------------------------------------------------------------------ forward
@@ -217,14 +215,14 @@ class PointFlow(nn.Module):
                                       "batch-statistics BatchNorm, test.py:58); call .train() on it")
         if torch.is_grad_enabled() and (estimated_depth_map.requires_grad or
                                         any(p.requires_grad for p in self.parameters())):
-            if not networks._backward_enabled:
+            if not networks.backward_enabled():
                 # without the switch a training loop would run and silently never update flow_edge_conv / flow_mlp.
                 # Inference runs under torch.no_grad() (test.py:62).
                 raise NotImplementedError("pointmvsnet_b200 PointFlow is forward-only; wrap the call in torch.no_grad() "
                                           "(training the flow modules needs the stand-alone operators)")
         given = pyramids_channels_last if pyramids_channels_last is not None else (
             [feature_pyramids[k] for k in PYR_KEYS] if isinstance(feature_pyramids, dict) else list(feature_pyramids))
-        grad_call = networks._backward_enabled and torch.is_grad_enabled() and (
+        grad_call = networks.backward_enabled() and torch.is_grad_enabled() and (
             estimated_depth_map.requires_grad or any(t.requires_grad for t in given) or
             any(p.requires_grad for p in self.parameters()))
         if grad_call:
@@ -276,9 +274,7 @@ class PointFlow(nn.Module):
             ws, need = self._workspace(shape, dev)
         else:
             need = lib.pmvs_point_flow_workspace_bytes(C.byref(shape))
-            if need == 0:
-                raise RuntimeError("libpmvs_b200: " + lib.pmvs_last_error().decode())
-            ws = torch.empty(need, device=dev, dtype=torch.uint8)
+            ws = _lib.workspace(need, dev)
         w, keep = self._weights(dev)
         track = self.update_running_stats and self.training
         bns = self._bn_modules()
@@ -537,9 +533,7 @@ class _PointFlowFn(torch.autograd.Function):
         gd = _lib.f32c(g_depth) if g_depth is not None else torch.zeros(B, 1, shape.flow_h, shape.flow_w, device=dev)
         gp = _lib.f32c(g_prob) if g_prob is not None else None
         nbytes = lib.pmvs_point_flow_backward_workspace_bytes(C.byref(shape))
-        if nbytes == 0:
-            raise RuntimeError("libpmvs_b200: " + lib.pmvs_last_error().decode())
-        bws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+        bws = _lib.workspace(nbytes, dev)
         pyr_ptrs = (C.c_void_p * 3)(p0.data_ptr(), p1.data_ptr(), p2.data_ptr())
         with torch.cuda.device(dev):
             check(lib.pmvs_point_flow_backward(C.byref(shape), C.byref(w), C.byref(pyr_ptrs), ptr(depth), ptr(cams),

@@ -35,14 +35,6 @@ def _points(t, name):
     return t.contiguous()
 
 
-def _workspace(nbytes, dev):
-    import torch
-    from .. import _lib
-    if nbytes == 0:
-        _lib.check(1)
-    return torch.empty(nbytes, device=dev, dtype=torch.uint8)  # the caching allocator aligns to 512 bytes
-
-
 def _thin(points, dst=0.2, seed=0, order=None):
     """-> (keep mask bool [N] on points' device, number of rounds the parallel greedy MIS took)"""
     import torch
@@ -63,7 +55,7 @@ def _thin(points, dst=0.2, seed=0, order=None):
         order = order.to(dev).contiguous()
         if not torch.equal(torch.sort(order).values, torch.arange(n, device=dev)):
             raise RuntimeError("thin_cloud: order must be a permutation of 0..%d" % (n - 1))
-        ws = _workspace(int(_lib.lib.pmvs_thin_cloud_workspace_bytes(n)), dev)
+        ws = _lib.workspace(int(_lib.lib.pmvs_thin_cloud_workspace_bytes(n)), dev)
         state = torch.empty(n, device=dev, dtype=torch.int32)
         undecided = torch.empty(ROUNDS_PER_CALL, device=dev, dtype=torch.int32)
         cell = _pow2_at_least(dst)
@@ -106,7 +98,7 @@ def nearest_distances(query, target, max_dist=20.0):
         raise RuntimeError("nearest_distances: max_dist = %r (must be finite and >= 0)" % max_dist)
     nq, nt, dev = query.shape[0], target.shape[0], query.device
     with torch.cuda.device(dev):
-        ws = _workspace(int(_lib.lib.pmvs_nearest_distances_workspace_bytes(nt)), dev)
+        ws = _lib.workspace(int(_lib.lib.pmvs_nearest_distances_workspace_bytes(nt)), dev)
         dist = torch.empty(nq, device=dev, dtype=torch.float32)
         _lib.check(_lib.lib.pmvs_nearest_distances(query.data_ptr(), nq, target.data_ptr(), nt, max_dist,
                                                    _pow2_at_least(max_dist / 16.0), dist.data_ptr(), ws.data_ptr(),

@@ -134,9 +134,7 @@ def _fusion_maps(depth, block, num_consistent, depth_thresh, reproj_thresh):
         depth = depth.contiguous()
         block = block.to(dev)
         nbytes = int(_lib.lib.pmvs_fuse_depth_maps_workspace_bytes(V, H, W))
-        if nbytes == 0:
-            _lib.check(1)
-        ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)  # the caching allocator aligns to 512 bytes
+        ws = _lib.workspace(nbytes, dev)
         count = torch.empty(V, H, W, device=dev, dtype=torch.int32)
         xyz = torch.empty(V, H, W, 3, device=dev, dtype=torch.float32)
         used = torch.empty(V, H, W, device=dev, dtype=torch.uint8)

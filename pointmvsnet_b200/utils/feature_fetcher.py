@@ -5,7 +5,7 @@ is summed in a fixed order (pmvs_feature_fetch_backward_det) instead of by the a
 import torch
 import torch.nn as nn
 
-from .._lib import lib, check, stream_ptr, ptr, require_cuda, f32c
+from .._lib import lib, check, stream_ptr, ptr, require_cuda, f32c, workspace
 
 
 class _Fetch(torch.autograd.Function):
@@ -35,9 +35,7 @@ class _Fetch(torch.autograd.Function):
         if torch.are_deterministic_algorithms_enabled():
             # fixed summation order (pmvs_feature_fetch_backward_det) in place of the atomicAdd scatter
             nbytes = int(lib.pmvs_feature_fetch_backward_det_workspace_bytes(B, V, Cc, H, W, N))
-            if nbytes == 0:
-                check(1)
-            ws = torch.empty(nbytes, device=g.device, dtype=torch.uint8)  # the caching allocator aligns to 512 bytes
+            ws = workspace(nbytes, g.device)
             with torch.cuda.device(g.device):
                 check(lib.pmvs_feature_fetch_backward_det(ptr(g), ptr(p), ptr(K), ptr(E), ptr(grad_maps), B, V, Cc, H,
                                                           W, N, ptr(ws), nbytes, stream_ptr()))
