@@ -498,6 +498,12 @@ typedef struct pmvs_flow_shape {
    * pixels of depth_out / prob_out are written, and the workspace is sized for sub_count sub-clouds.
    * sub_count == 0 (default): all of them. */
   int sub_begin, sub_count;
+  /* BatchNorm mode of the six flow layers.  0 (default): batch statistics per sub-cloud, as under model.train(); the
+   * running statistics are updated when given.  1: the running statistics, as under model.eval(): ec_run_mean/var and
+   * mlp_run_mean/var are required inputs and nothing is written to them, *_nbt and momentum are ignored.  Served by
+   * the default kernel families only (PMVS_ERR_ARG otherwise, e.g. under edge=0); pmvs_point_flow_backward rejects it.
+   * An eval call needs a smaller workspace: no BatchNorm sums and no flow_mlp activations. */
+  int bn_eval;
 } pmvs_flow_shape;
 
 /* bytes of device workspace pmvs_point_flow_iter needs for this shape */

@@ -39,7 +39,7 @@ class FlowShape(C.Structure):
         ("B", C.c_int), ("V", C.c_int), ("pyr_h", C.c_int * 3), ("pyr_w", C.c_int * 3),
         ("prev_h", C.c_int), ("prev_w", C.c_int), ("flow_h", C.c_int), ("flow_w", C.c_int),
         ("image_scale", C.c_float), ("ratio", C.c_int), ("is_test", C.c_int), ("interval_scale", C.c_float),
-        ("sub_begin", C.c_int), ("sub_count", C.c_int),
+        ("sub_begin", C.c_int), ("sub_count", C.c_int), ("bn_eval", C.c_int),
     ]
 
 

@@ -146,6 +146,8 @@ struct FlowPlan {
   size_t st_ticket;    // 3*S unsigned arrival counters of the tile statistics kernels (inside the zeroed region)
   size_t stats_doubles;
   size_t coef;         // [3][S][6*64] floats: per (layer, group) BatchNorm coefficients of the tile apply kernels
+  size_t mlp_coef;     // bn_eval: FLOW_EVAL_MLP_COEF floats after the tile tables (flow_mlp's BatchNorms)
+  bool eval;           // bn_eval: running statistics; no stats, h0, h1 or h2 regions (their offsets are 0)
 };
 
 static int make_plan(const pmvs_flow_shape* s, FlowPlan& p) {
@@ -170,6 +172,11 @@ static int make_plan(const pmvs_flow_shape* s, FlowPlan& p) {
   p.N = PMVS_NUM_HYP * p.hs * p.ws;
   p.R = (size_t)p.S * s->B * p.N;
   PMVS_REQUIRE(p.R * 224 < (size_t)1 << 40, "point_flow: problem too large");
+  PMVS_REQUIRE(s->bn_eval == 0 || s->bn_eval == 1, "point_flow: bn_eval must be 0 or 1, got %d", s->bn_eval);
+  p.eval = s->bn_eval != 0;
+  // the running-statistics path is built on the tile EdgeConv family (its apply kernel reads a coefficient table)
+  PMVS_REQUIRE(!p.eval || opt(OPT_EDGE) != 0,
+               "point_flow: bn_eval = 1 is served by the tile EdgeConv kernels only (option edge=%d)", opt(OPT_EDGE));
   size_t o = 0;
   p.cam = o; o += up256(cam_block_bytes(s->B, s->V));
   p.feature = o; o += up256(p.R * PMVS_FEAT_CH * 4);
@@ -177,9 +184,12 @@ static int make_plan(const pmvs_flow_shape* s, FlowPlan& p) {
   p.idx = o; o += up256(p.R * PMVS_KNN * 4);
   p.le = o; o += up256(p.R * 128 * 4);
   p.ecat = o; o += up256(p.R * 224 * 4);
-  p.h0 = o; o += up256(p.R * 64 * 4);
-  p.h1 = o; o += up256(p.R * 64 * 4);
-  p.h2 = o; o += up256(p.R * 16 * 4);
+  p.h0 = p.h1 = p.h2 = 0;
+  if (!p.eval) {
+    p.h0 = o; o += up256(p.R * 64 * 4);
+    p.h1 = o; o += up256(p.R * 64 * 4);
+    p.h2 = o; o += up256(p.R * 16 * 4);
+  }
   p.warp_src = o; o += up256(warp_source_bytes(s->B, s->V, s->flow_h, s->flow_w));
   p.cand = o; o += up256(p.R * PMVS_KNN * 2);
   size_t d = 0;
@@ -192,8 +202,15 @@ static int make_plan(const pmvs_flow_shape* s, FlowPlan& p) {
   for (int l = 0; l < 3; ++l) { p.st_mlp[l] = d; d += (size_t)p.S * 2 * mlp_cout[l]; }
   p.st_ticket = d; d += (3 * (size_t)p.S + 1) / 2 + 1;
   p.stats_doubles = d;
-  p.stats = o; o += up256(d * 8);
+  p.stats = 0;
+  if (!p.eval) {
+    p.stats = o; o += up256(d * 8);
+  }
   p.coef = o; o += up256(3 * (size_t)p.S * 6 * 64 * sizeof(float));
+  p.mlp_coef = 0;
+  if (p.eval) {
+    p.mlp_coef = o; o += up256(FLOW_EVAL_MLP_COEF * sizeof(float));
+  }
   p.total = o;
   return PMVS_OK;
 }
@@ -224,7 +241,7 @@ int flow_regions(const pmvs_flow_shape* s, FlowRegions& r) {
 
 using namespace pmvs;
 
-extern "C" int pmvs_version(void) { return 100; }
+extern "C" int pmvs_version(void) { return 101; }
 extern "C" const char* pmvs_last_error(void) { return g_err; }
 extern "C" unsigned long long pmvs_launch_count(void) { return g_launches.load(); }
 
@@ -352,7 +369,7 @@ extern "C" size_t pmvs_point_flow_workspace_bytes(const pmvs_flow_shape* shape) 
 extern "C" int pmvs_point_flow_debug_offsets(const pmvs_flow_shape* shape, size_t off[10]) {
   FlowPlan p;
   PMVS_TRY(make_plan(shape, p));
-  off[0] = p.feature; off[1] = p.xyz; off[2] = p.idx; off[3] = p.ecat; off[4] = p.h2;
+  off[0] = p.feature; off[1] = p.xyz; off[2] = p.idx; off[3] = p.ecat; off[4] = p.h2;  // h2, stats: 0 under bn_eval
   off[5] = p.le; off[6] = p.stats; off[7] = p.total;
   off[8] = p.cand;
   off[9] = (opt(OPT_EDGE) == 0 || opt(OPT_DEBUG_IDX) != 0) ? 1 : 0;  // 1: idx32 is materialised, 0: only cand
@@ -392,7 +409,13 @@ extern "C" int pmvs_point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flo
   const int B = shape->B, S = p.S;
   const int rows_per_group = B * p.N;
 
-  PMVS_TRY(memset_async("point_flow", stats, p.stats_doubles * sizeof(double), st));
+  if (p.eval) {
+    for (int l = 0; l < 3; ++l)
+      PMVS_REQUIRE(wts->ec_run_mean[l] && wts->ec_run_var[l] && wts->mlp_run_mean[l] && wts->mlp_run_var[l],
+                   "point_flow: bn_eval = 1 needs the running mean and variance of all six BatchNorm layers");
+  } else {
+    PMVS_TRY(memset_async("point_flow", stats, p.stats_doubles * sizeof(double), st));
+  }
   // model.py:159-163: K rows 0,1 scaled by image_scale (test) or 4*image_scale (train)
   const float kscale = shape->is_test ? shape->image_scale : (float)(4.0 * (double)shape->image_scale);
   PMVS_TRY(launch_cam_setup(cam_params, interval, mean, stdv, cam, B, shape->V, kscale, shape->interval_scale, st));
@@ -425,6 +448,10 @@ extern "C" int pmvs_point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flo
   else
     PMVS_TRY(launch_knn3d(xyz, nullptr, idx, S * B, PMVS_NUM_HYP, p.hs, p.ws, PMVS_NUM_HYP, PMVS_KNN, st));
 
+  // running statistics: every BatchNorm coefficient is known before the first layer (flow_eval.cu)
+  if (p.eval)
+    PMVS_TRY(launch_flow_eval_coef(*wts, S, (float*)(ws + p.coef), (float*)(ws + p.mlp_coef), st));
+
   // flow_edge_conv (model.py:213-216): EdgeConvNoC(136,32), EdgeConv(32,32), EdgeConv(64,64)
   const int cin[3] = {136, 32, 64}, cout[3] = {32, 32, 64}, in_off[3] = {0, 0, 32}, out_off[3] = {0, 32, 96};
   for (int l = 0; l < 3; ++l) {
@@ -434,18 +461,21 @@ extern "C" int pmvs_point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flo
     g.w = wts->ec_w12[l]; g.y = le; g.ldy = 2 * cout[l];
     g.groups = S; g.rows_per_group = rows_per_group; g.cin = cin[l]; g.cout = 2 * cout[l]; g.eps = wts->eps;
     // column sums of LE: the central half's BN statistics, which EdgeConvNoC (layer 0) does not have
-    if (edge_impl != 0 && l > 0) g.out_stats = stats + p.st_ec[l];
+    if (edge_impl != 0 && l > 0 && !p.eval) g.out_stats = stats + p.st_ec[l];
     if (l > 0 || !fused_le0) PMVS_TRY(launch_gemm(g, st));
     if (edge_impl != 0) {
       EdgeTileArgs e{};
-      e.le = le; e.cand = cand; e.cstats = stats + p.st_ec[l]; e.nstats = stats + p.st_ecn[l];
+      e.le = le; e.cand = cand;
       e.coef = (float*)(ws + p.coef) + (size_t)l * S * 6 * 64;
-      e.ticket = (unsigned*)(stats + p.st_ticket) + (size_t)l * S;
+      if (!p.eval) {
+        e.cstats = stats + p.st_ec[l]; e.nstats = stats + p.st_ecn[l];
+        e.ticket = (unsigned*)(stats + p.st_ticket) + (size_t)l * S;
+      }
       e.gamma = wts->ec_gamma[l]; e.beta = wts->ec_beta[l]; e.eps = wts->eps; e.concat_central = l > 0;
       e.out = ecat + out_off[l]; e.ldo = 224; e.groups = S; e.clouds_per_group = B; e.gh = p.hs; e.gw = p.ws;
       e.cout = cout[l];
       const int tile_w = edge_impl == 2 ? 16 : 8;
-      PMVS_TRY(launch_edge_tile_stats(e, tile_w, st));
+      if (!p.eval) PMVS_TRY(launch_edge_tile_stats(e, tile_w, st));
       PMVS_TRY(launch_edge_tile_apply(e, tile_w, st));
     } else {
       EdgeArgs e{};
@@ -455,6 +485,19 @@ extern "C" int pmvs_point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flo
       PMVS_TRY(launch_edge_stats(e, st));
       PMVS_TRY(launch_edge_apply(e, st));
     }
+  }
+
+  if (p.eval) {
+    // flow_mlp and the head in one launch; nothing to update
+    FlowEvalArgs fa{};
+    fa.ecat = ecat; fa.w[0] = wts->mlp_w[0]; fa.w[1] = wts->mlp_w[1]; fa.w[2] = wts->mlp_w[2];
+    fa.mlp_coef = (const float*)(ws + p.mlp_coef);
+    HeadArgs& h = fa.head;
+    h.w3 = wts->mlp_w[3]; h.depth_prev = depth_prev; h.interval = interval; h.depth_out = depth_out;
+    h.prob_out = prob_out; h.eps = wts->eps; h.interval_scale = shape->interval_scale; h.B = B; h.S = S;
+    h.ratio = shape->ratio; h.sub_begin = p.sub_begin; h.h = shape->flow_h; h.w = shape->flow_w;
+    h.hp = shape->prev_h; h.wp = shape->prev_w;
+    return launch_flow_mlp_head_eval(fa, st);
   }
 
   // flow_mlp (model.py:40-43,220): 224 -> 64 -> 64 -> 16 -> 1, BN batch statistics per sub-cloud

@@ -330,6 +330,59 @@ struct HeadArgs {
   int sub_begin;            // group s of this launch is sub-cloud sub_begin + s of the iteration
 };
 int launch_flow_head(const HeadArgs& a, cudaStream_t st);
+// The end of the flow head for pixel pp of cloud b in group s, given its five raw flow_mlp outputs: softmax(-raw) over
+// the hypotheses (model.py:222), the expected offset (:224-227), depth_up (nearest, :153-158) + flow, scattered to the
+// full grid at the pixel of sub-cloud s + sub_begin (:244-266).  Used by flow_head_kernel and the eval-mode
+// flow_mlp_head_eval_kernel (flow_eval.cu).
+__device__ __forceinline__ void flow_head_store(const HeadArgs& a, const float (&raw)[PMVS_NUM_HYP], int s, int b,
+                                                int pp) {
+  const int ws = a.w / a.ratio;
+  const int yy = pp / ws, xx = pp - yy * ws;
+  const int sg = s + a.sub_begin;  // sub-cloud index inside the iteration (model.py:244-245: i, j)
+  const int ii = sg / a.ratio, jj = sg - ii * a.ratio;
+  const int Y = yy * a.ratio + ii, X = xx * a.ratio + jj;
+  float mx = -raw[0];
+#pragma unroll
+  for (int m = 1; m < PMVS_NUM_HYP; ++m) mx = fmaxf(mx, -raw[m]);
+  float e[PMVS_NUM_HYP], sum = 0.f;
+#pragma unroll
+  for (int m = 0; m < PMVS_NUM_HYP; ++m) {
+    e[m] = expf(-raw[m] - mx);
+    sum += e[m];
+  }
+  const float itv = __fmul_rn(a.interval_scale, a.interval[b]);
+  float flow = 0.f;
+  const size_t plane = (size_t)a.h * a.w;
+  const size_t pix = (size_t)Y * a.w + X;
+#pragma unroll
+  for (int m = 0; m < PMVS_NUM_HYP; ++m) {
+    const float pr = __fdiv_rn(e[m], sum);
+    flow = __fadd_rn(flow, __fmul_rn(pr, __fmul_rn((float)(m - 2), itv)));  // model.py:224-227
+    if (a.prob_out) a.prob_out[((size_t)b * PMVS_NUM_HYP + m) * plane + pix] = pr;
+  }
+  const float nsy = (float)a.hp / (float)a.h, nsx = (float)a.wp / (float)a.w;
+  int ys = (int)floorf((float)Y * nsy), xs = (int)floorf((float)X * nsx);
+  ys = ys < a.hp - 1 ? ys : a.hp - 1;
+  xs = xs < a.wp - 1 ? xs : a.wp - 1;
+  const float dprev = __ldg(a.depth_prev + ((size_t)b * a.hp + ys) * a.wp + xs);
+  a.depth_out[(size_t)b * plane + pix] = __fadd_rn(dprev, flow);
+}
+
+// ---- running-statistics BatchNorm of the PointFlow path (pmvs_flow_shape.bn_eval = 1; flow_eval.cu) ---------------
+// flow_mlp's three BatchNorms as relu(fma(x, A, B)): [A0 | B0] x 64, [A1 | B1] x 64, [A2 | B2] x 16
+constexpr int FLOW_EVAL_MLP_COEF = 2 * (64 + 64 + 16);
+// From the running statistics of `w`: the edge_tile coefficient table of the three EdgeConv layers for each of the S
+// groups (ec_coef + l * S * 6 * 64 + g * 6 * cout, the layout of edge_tile.cu) and flow_mlp's table (mlp_coef).  One
+// launch, on the device, so a replayed CUDA graph reads the buffers as they are at replay time.
+int launch_flow_eval_coef(const pmvs_flow_weights& w, int S, float* ec_coef, float* mlp_coef, cudaStream_t st);
+struct FlowEvalArgs {
+  const float* ecat;      // [S*B*N, 224], the concatenated EdgeConv outputs
+  const float* w[3];      // flow_mlp.0.{0,1,2}.conv.weight [64,224], [64,64], [16,64]
+  const float* mlp_coef;  // FLOW_EVAL_MLP_COEF floats (launch_flow_eval_coef)
+  HeadArgs head;          // w3, depth_prev, interval, outputs and grid; h2 / stats / gamma / beta are not read
+};
+// flow_mlp (224 -> 64 -> 64 -> 16 -> 1) and the flow head in one persistent launch: h0, h1, h2 never leave the SM
+int launch_flow_mlp_head_eval(const FlowEvalArgs& a, cudaStream_t st);
 // byte offsets of the regions of pmvs_point_flow_iter's workspace (api.cu make_plan) and the double offsets of the
 // BatchNorm sums inside `stats`, for the backward that reads it
 struct FlowRegions {

@@ -339,7 +339,8 @@ int launch_variant(const EdgeTileArgs& a, cudaStream_t st) {
 
 template <bool APPLY>
 int launch_edge_tile(const EdgeTileArgs& a, int tile_w, cudaStream_t st) {
-  PMVS_REQUIRE(a.le && a.cand && a.cstats && a.nstats && a.gamma && a.beta && a.coef && a.ticket && (!APPLY || a.out),
+  // apply reads only the coefficient table, so it also serves a table written from running statistics
+  PMVS_REQUIRE(a.le && a.cand && a.coef && (APPLY ? a.out != nullptr : (a.cstats && a.nstats && a.gamma && a.beta && a.ticket)),
                "edge_tile: NULL pointer");
   PMVS_REQUIRE(a.cout == 32 || a.cout == 64, "edge_tile: out_channels %d (supported: 32, 64)", a.cout);
   PMVS_REQUIRE(a.gh > 0 && a.gw > 0 && a.groups > 0 && a.clouds_per_group > 0, "edge_tile: bad cloud shape");

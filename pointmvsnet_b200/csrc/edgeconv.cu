@@ -407,10 +407,6 @@ __global__ void __launch_bounds__(256) flow_head_kernel(const HeadArgs a) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= a.B * P) return;
   const int b = t / P, pp = t - b * P;
-  const int yy = pp / ws, xx = pp - yy * ws;
-  const int sg = s + a.sub_begin;  // sub-cloud index inside the iteration (model.py:244-245: i, j)
-  const int ii = sg / a.ratio, jj = sg - ii * a.ratio;
-  const int Y = yy * a.ratio + ii, X = xx * a.ratio + jj;
   const size_t cloud_row = ((size_t)s * a.B + b) * N;
   float raw[PMVS_NUM_HYP];
 #pragma unroll
@@ -427,33 +423,7 @@ __global__ void __launch_bounds__(256) flow_head_kernel(const HeadArgs a) {
     }
     raw[m] = acc;
   }
-  // softmax(-raw) over hypotheses (model.py:222)
-  float mx = -raw[0];
-#pragma unroll
-  for (int m = 1; m < PMVS_NUM_HYP; ++m) mx = fmaxf(mx, -raw[m]);
-  float e[PMVS_NUM_HYP], sum = 0.f;
-#pragma unroll
-  for (int m = 0; m < PMVS_NUM_HYP; ++m) {
-    e[m] = expf(-raw[m] - mx);
-    sum += e[m];
-  }
-  const float itv = __fmul_rn(a.interval_scale, a.interval[b]);
-  float flow = 0.f;
-  const size_t plane = (size_t)a.h * a.w;
-  const size_t pix = (size_t)Y * a.w + X;
-#pragma unroll
-  for (int m = 0; m < PMVS_NUM_HYP; ++m) {
-    const float pr = __fdiv_rn(e[m], sum);
-    flow = __fadd_rn(flow, __fmul_rn(pr, __fmul_rn((float)(m - 2), itv)));  // model.py:224-227
-    if (a.prob_out) a.prob_out[((size_t)b * PMVS_NUM_HYP + m) * plane + pix] = pr;
-  }
-  // depth_up (nearest, model.py:153-158) + flow
-  const float nsy = (float)a.hp / (float)a.h, nsx = (float)a.wp / (float)a.w;
-  int ys = (int)floorf((float)Y * nsy), xs = (int)floorf((float)X * nsx);
-  ys = ys < a.hp - 1 ? ys : a.hp - 1;
-  xs = xs < a.wp - 1 ? xs : a.wp - 1;
-  const float dprev = __ldg(a.depth_prev + ((size_t)b * a.hp + ys) * a.wp + xs);
-  a.depth_out[(size_t)b * plane + pix] = __fadd_rn(dprev, flow);
+  flow_head_store(a, raw, s, b, pp);
 }
 
 int launch_flow_head(const HeadArgs& a, cudaStream_t st) {

@@ -296,6 +296,8 @@ struct BwdFlowPlan {
 // the backward takes S = 1: the train branch (ratio 1) and the test branch at scale 0.125
 int bwd_flow_plan(const pmvs_flow_shape* s, BwdFlowPlan& p) {
   PMVS_REQUIRE(s != nullptr, "point_flow_backward: NULL shape");
+  PMVS_REQUIRE(s->bn_eval == 0, "point_flow_backward: the forward ran with bn_eval = 1 (running-statistics BatchNorm), "
+               "which has no backward");
   PMVS_REQUIRE(s->ratio == 1 && s->sub_count == 0 && s->sub_begin == 0,
                "point_flow_backward: only one cloud per call (ratio 1, no sub_count); got ratio %d, sub_count %d",
                s->ratio, s->sub_count);

@@ -52,8 +52,9 @@ class PointMVSNet(nn.Module):
 
     The state dict has the reference's 223 entries.  The ``PointFlow`` that runs the refinement shares
     ``flow_edge_conv`` and ``flow_mlp`` and is deliberately not a sub-module (it would add ``point_flow.*`` keys).
-    The flow stage runs only in ``train()`` mode (test.py:58 keeps the model there: BatchNorm uses batch statistics);
-    the coarse stage also runs in ``eval()``."""
+    In ``train()`` mode (test.py:58 keeps the model there) BatchNorm uses batch statistics; in ``eval()`` every stage
+    uses the running statistics, under ``torch.no_grad()`` (a grad-enabled ``eval()`` forward raises
+    ``NotImplementedError`` in the flow stage)."""
 
     def __init__(self, img_base_channels=8, vol_base_channels=8, flow_channels=(64, 64, 16, 1), k=16):
         super().__init__()
@@ -107,8 +108,9 @@ class PointMVSNet(nn.Module):
         if isTest:  # model.py:146-148
             pyr = {k: v.detach() for k, v in pyr.items()}
         pyr_cl = PointFlow.pyramids_to_channels_last(pyr)
+        # PointFlow takes the BatchNorm mode from the shared flow_edge_conv / flow_mlp modules, which net.train() /
+        # net.eval() have set; a per-layer choice made after that (frozen BatchNorm) is kept
         pf = self._point_flow
-        pf.train(self.training)
         depth_interval = cams[:, 0, 1, 3, 1]
         depth = preds["coarse_depth_map"]
         for i, (img_scale, inter_scale) in enumerate(zip(img_scales, inter_scales)):

@@ -2,7 +2,8 @@
 as an nn.Module, executed by libpmvs_b200.so.
 
 Inference runs as test.py runs it: under torch.no_grad() with the module in train() mode so that BatchNorm uses batch
-statistics.  Training (the train branch, one cloud per call) runs through an autograd Function whose backward is
+statistics.  Under .eval() (all six BatchNorm layers in eval mode) a call that needs no gradient uses the running
+statistics instead, as the reference's model.eval() does; that mode has no backward.  Training (the train branch, one cloud per call) runs through an autograd Function whose backward is
 ``pmvs_point_flow_backward`` once ``networks.enable_backward()`` is on; without it a grad-enabled call raises.
 
 One call = one refinement iteration = ~16 kernel launches enqueued by a single C-ABI
@@ -167,8 +168,28 @@ class PointFlow(nn.Module):
         return res
 
     # ------------------------------------------------------------------ shape / workspace
+    def _bn_eval(self, needs_grad):
+        """The BatchNorm mode of a call, from the six BatchNorm modules: False (all in train mode: batch statistics),
+        True (all in eval mode: running statistics).  Raises before any launch for a mode the path does not serve."""
+        bns = self._bn_modules()
+        if all(bn.training for bn in bns):
+            return False
+        if needs_grad:
+            raise NotImplementedError("PointFlow: BatchNorm in eval mode (running statistics) has no backward on the "
+                                      "fused path; wrap the call in torch.no_grad(), or call .train() on the module")
+        if any(bn.training for bn in bns):
+            raise RuntimeError("PointFlow: the six BatchNorm layers must all be in train mode or all in eval mode, got "
+                               "%s" % ["train" if bn.training else "eval" for bn in bns])
+        for bn in bns:
+            if not bn.track_running_stats or bn.running_mean is None or bn.running_var is None:
+                raise RuntimeError("PointFlow: a BatchNorm layer in eval mode without running statistics "
+                                   "(track_running_stats=False) uses batch statistics; the fused path serves eval mode "
+                                   "with running statistics only")
+        return True
+
     @staticmethod
-    def make_shape(B, V, pyr_hw, prev_hw, img_hw, image_scale, is_test, interval_scale=1.0, sub_range=None):
+    def make_shape(B, V, pyr_hw, prev_hw, img_hw, image_scale, is_test, interval_scale=1.0, sub_range=None,
+                   bn_eval=False):
         s = FlowShape()
         s.B, s.V = B, V
         for l in range(3):
@@ -183,6 +204,7 @@ class PointFlow(nn.Module):
             s.sub_begin, s.sub_count = int(sub_range[0]), int(sub_range[1])
             if s.sub_count <= 0 or s.sub_begin < 0 or s.sub_begin + s.sub_count > s.ratio * s.ratio:
                 raise RuntimeError("PointFlow: sub_range %r outside the %d sub-clouds" % (sub_range, s.ratio * s.ratio))
+        s.bn_eval = 1 if bn_eval else 0
         return s
 
     def _workspace(self, shape, device):
@@ -205,14 +227,19 @@ class PointFlow(nn.Module):
         without a separate elementwise launch).  ``sub_range=(first, count)`` processes only
         those of the ratio^2 strided sub-clouds (the independent calls of model.py:236-267; used to
         shard one view over GPUs, parallel.SubCloudShardedPass): only their pixels of the outputs are
-        written.  Returns (flow_result [B,1,h,w], flow_prob [B,5,h,w])."""
+        written.  Returns (flow_result [B,1,h,w], flow_prob [B,5,h,w]).
+
+        BatchNorm follows the six BatchNorm modules: in train mode (the reference's test.py:58) batch statistics per
+        sub-cloud, and the running statistics are updated; in eval mode (``.eval()``) the running statistics, which
+        are then only read.  Eval mode serves calls that need no gradient (under torch.no_grad(), or with nothing
+        requiring grad); a grad-needing call raises NotImplementedError, a mix of modes RuntimeError."""
         require_cuda(estimated_depth_map, interval, cam_params_list, mean, std)
-        if not self.training:
-            # the reference runs inference under model.train() (test.py:58): BatchNorm uses batch
-            # statistics.  The fused path implements exactly that; running-statistics BN is only
-            # available through the stand-alone EdgeConv modules.
-            raise NotImplementedError("PointFlow implements the reference's inference mode (module.train(), "
-                                      "batch-statistics BatchNorm, test.py:58); call .train() on it")
+        given = pyramids_channels_last if pyramids_channels_last is not None else (
+            [feature_pyramids[k] for k in PYR_KEYS] if isinstance(feature_pyramids, dict) else list(feature_pyramids))
+        needs_grad = torch.is_grad_enabled() and (
+            estimated_depth_map.requires_grad or any(t.requires_grad for t in given) or
+            any(p.requires_grad for p in self.parameters()))
+        bn_eval = self._bn_eval(needs_grad)
         if torch.is_grad_enabled() and (estimated_depth_map.requires_grad or
                                         any(p.requires_grad for p in self.parameters())):
             if not networks.backward_enabled():
@@ -220,8 +247,6 @@ class PointFlow(nn.Module):
                 # Inference runs under torch.no_grad() (test.py:62).
                 raise NotImplementedError("pointmvsnet_b200 PointFlow is forward-only; wrap the call in torch.no_grad() "
                                           "(training the flow modules needs the stand-alone operators)")
-        given = pyramids_channels_last if pyramids_channels_last is not None else (
-            [feature_pyramids[k] for k in PYR_KEYS] if isinstance(feature_pyramids, dict) else list(feature_pyramids))
         grad_call = networks.backward_enabled() and torch.is_grad_enabled() and (
             estimated_depth_map.requires_grad or any(t.requires_grad for t in given) or
             any(p.requires_grad for p in self.parameters()))
@@ -236,6 +261,17 @@ class PointFlow(nn.Module):
                                        "differentiate it (the reference's fetch coordinates are under no_grad)" % name)
             if out is not None:
                 raise RuntimeError("PointFlow: `out` buffers are for inference (no_grad) calls")
+        if bn_eval and estimated_depth_map.dim() == 4 and cam_params_list.dim() == 5 and all(t.dim() == 5 for t in given):
+            # a shape or kernel-family choice the eval path does not serve is the library's error, raised before the
+            # pyramid transposes launch
+            pyr_hw = [tuple(int(v) for v in (t.shape[2:4] if pyramids_channels_last is not None else t.shape[3:5]))
+                      for t in given]
+            hw = img_hw if img_hw is not None else (pyr_hw[0][0] * 2, pyr_hw[0][1] * 2)
+            shape = self.make_shape(int(cam_params_list.shape[0]), int(cam_params_list.shape[1]), pyr_hw,
+                                    tuple(estimated_depth_map.shape[2:]), hw, image_scale, is_test, interval_scale,
+                                    sub_range, True)
+            if lib.pmvs_point_flow_workspace_bytes(C.byref(shape)) == 0:
+                check(1)  # PMVS_ERR_ARG, with the library's message
         if pyramids_channels_last is None:
             pyramids_channels_last = self.pyramids_to_channels_last(feature_pyramids)
         pyr = list(pyramids_channels_last)
@@ -244,7 +280,7 @@ class PointFlow(nn.Module):
             return _PointFlowFn.apply(self, (interval, image_scale, cam_params_list, mean, std, is_test, img_hw,
                                              interval_scale), estimated_depth_map, pyr[0], pyr[1], pyr[2], *params)
         return self._run(estimated_depth_map, interval, image_scale, cam_params_list, mean, std, is_test, img_hw,
-                         pyr, out, interval_scale, sub_range, None)
+                         pyr, out, interval_scale, sub_range, None, bn_eval)
 
     def _grad_params(self):
         """The 22 parameters the backward fills, in pmvs_flow_grads order."""
@@ -257,9 +293,9 @@ class PointFlow(nn.Module):
         return ps + [self.flow_mlp[1].weight]
 
     def _run(self, estimated_depth_map, interval, image_scale, cam_params_list, mean, std, is_test, img_hw, pyr, out,
-             interval_scale, sub_range, ctx):
+             interval_scale, sub_range, ctx, bn_eval=False):
         """The forward launches.  ctx None: the module's shared workspace; else (an autograd context) a workspace of
-        the call's own, kept with what the backward reads."""
+        the call's own, kept with what the backward reads.  bn_eval: BatchNorm from the running statistics."""
         dev = estimated_depth_map.device
         B, V = cam_params_list.shape[:2]
         pyr_hw = [(int(t.shape[2]), int(t.shape[3])) for t in pyr]
@@ -267,22 +303,23 @@ class PointFlow(nn.Module):
             img_hw = (pyr_hw[0][0] * 2, pyr_hw[0][1] * 2)  # conv1 is at half resolution (networks.py:84-124)
         depth = _lib.f32c(estimated_depth_map.detach())
         pyr = [t.detach() for t in pyr]
-        self._validate(dev, B, V, pyr, depth, interval, mean, std, cam_params_list)
+        self._validate(dev, B, V, pyr, depth, interval, mean, std, cam_params_list, bn_eval)
         shape = self.make_shape(B, V, pyr_hw, tuple(depth.shape[2:]), img_hw, image_scale, is_test, interval_scale,
-                                sub_range)
+                                sub_range, bn_eval)
         if ctx is None:
             ws, need = self._workspace(shape, dev)
         else:
             need = lib.pmvs_point_flow_workspace_bytes(C.byref(shape))
             ws = _lib.workspace(need, dev)
         w, keep = self._weights(dev)
-        track = self.update_running_stats and self.training
+        track = self.update_running_stats and not bn_eval  # the six BatchNorm layers are in train mode
+        stats = track or bn_eval  # updated in train mode, read in eval mode
         bns = self._bn_modules()
         for l in range(3):
-            w.ec_run_mean[l] = ptr(bns[l].running_mean) if track else None
-            w.ec_run_var[l] = ptr(bns[l].running_var) if track else None
-            w.mlp_run_mean[l] = ptr(bns[3 + l].running_mean) if track else None
-            w.mlp_run_var[l] = ptr(bns[3 + l].running_var) if track else None
+            w.ec_run_mean[l] = ptr(bns[l].running_mean) if stats else None
+            w.ec_run_var[l] = ptr(bns[l].running_var) if stats else None
+            w.mlp_run_mean[l] = ptr(bns[3 + l].running_mean) if stats else None
+            w.mlp_run_var[l] = ptr(bns[3 + l].running_var) if stats else None
             w.ec_nbt[l] = ptr(bns[l].num_batches_tracked) if track else None
             w.mlp_nbt[l] = ptr(bns[3 + l].num_batches_tracked) if track else None
         h, wd = shape.flow_h, shape.flow_w
@@ -309,7 +346,7 @@ class PointFlow(nn.Module):
             ctx.fwd = (shape, w, keep, int(B), tuple(depth.shape))
         return depth_out, prob_out
 
-    def _validate(self, dev, B, V, pyr, depth, interval, mean, std, cams):
+    def _validate(self, dev, B, V, pyr, depth, interval, mean, std, cams, bn_eval=False):
         """The C ABI takes raw pointers: everything it will dereference is checked here (device, dtype, sizes)
         so that a mismatch is a RuntimeError and not an out-of-bounds device access."""
         for name, t in (("interval", interval), ("mean", mean), ("std", std), ("cam_params_list", cams)):
@@ -336,6 +373,13 @@ class PointFlow(nn.Module):
             if bn.running_mean is not None and (bn.running_mean.dtype != torch.float32 or
                                                 bn.num_batches_tracked.dtype != torch.int64):
                 raise RuntimeError("PointFlow: BatchNorm buffers must be fp32 / int64")
+            if bn_eval:  # the kernels read num_features fp32 values of each
+                for t in (bn.running_mean, bn.running_var):
+                    if (t.device != dev or t.dtype != torch.float32 or tuple(t.shape) != (bn.num_features,) or
+                            not t.is_contiguous()):
+                        raise RuntimeError("PointFlow: BatchNorm running statistics must be contiguous fp32 [%d] on "
+                                           "%s, got %s %s on %s" % (bn.num_features, dev, t.dtype, tuple(t.shape),
+                                                                    t.device))
 
     # ------------------------------------------------------------------ debugging / parity
     def debug_stages(self):
@@ -343,7 +387,8 @@ class PointFlow(nn.Module):
         feature [B,136,5,h,w]-equivalent per sub-cloud etc.  Returns a dict of tensors
         indexed [S, B, ...].  The fused fetch of PMVS_OPT_FETCH 3 does not write `feature`: it is recomputed here
         by the unfused fetch kernel from the workspace and the last call's previous depth map, which must not have
-        been modified since."""
+        been modified since.  After an eval-mode call (running statistics) there is no "h2": flow_mlp and the head run
+        in one kernel and its activations never reach memory."""
         shape, ws, depth = self._last
         off = (C.c_size_t * 10)()
         check(lib.pmvs_point_flow_debug_offsets(C.byref(shape), C.byref(off)))
@@ -373,11 +418,14 @@ class PointFlow(nn.Module):
             dw = torch.where(out, j % 5, c % 12) - 2
             n = torch.arange(N, device=ws.device).view(1, 1, N, 1)
             idx = (n + dd * (hs * wsub) + dh * wsub + dw).clamp_(0, N - 1).int()
-        return {
+        res = {
             "feature": view(off[0], 136), "xyz": ws[off[1]:off[1] + R * 12].view(torch.float32).view(S, shape.B, 3, N),
-            "idx": idx, "cand": cand, "edge": view(off[3], 224), "h2": view(off[4], 16),
+            "idx": idx, "cand": cand, "edge": view(off[3], 224),
             "S": S, "hs": hs, "ws": wsub, "N": N,
         }
+        if not shape.bn_eval:
+            res["h2"] = view(off[4], 16)
+        return res
 
 
 class PointFlowPass(object):
