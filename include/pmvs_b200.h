@@ -501,7 +501,8 @@ typedef struct pmvs_flow_shape {
   /* BatchNorm mode of the six flow layers.  0 (default): batch statistics per sub-cloud, as under model.train(); the
    * running statistics are updated when given.  1: the running statistics, as under model.eval(): ec_run_mean/var and
    * mlp_run_mean/var are required inputs and nothing is written to them, *_nbt and momentum are ignored.  Served by
-   * the default kernel families only (PMVS_ERR_ARG otherwise, e.g. under edge=0); pmvs_point_flow_backward rejects it.
+   * the default kernel families only (PMVS_ERR_ARG otherwise, e.g. under edge=0); pmvs_point_flow_backward rejects it
+   * (its backward is pmvs_point_flow_eval_backward, after pmvs_point_flow_eval_keep).
    * An eval call needs a smaller workspace: no BatchNorm sums and no flow_mlp activations. */
   int bn_eval;
 } pmvs_flow_shape;
@@ -577,6 +578,38 @@ int pmvs_point_flow_backward(const pmvs_flow_shape* shape, const pmvs_flow_weigh
                              const float* std, const void* fwd_workspace, const float* grad_depth_out,
                              const float* grad_prob_out, const pmvs_flow_grads* grads, void* workspace,
                              size_t workspace_bytes, pmvs_stream_t stream);
+
+/* ---- backward with running-statistics BatchNorm (bn_eval = 1: fine-tuning with frozen BatchNorm) ------------- */
+/* bytes of device workspace pmvs_point_flow_eval_keep needs: pmvs_point_flow_workspace_bytes plus h0, h1, h2
+ * (R x 144 floats), the raw flow_mlp outputs (R floats) and a copy of the running statistics, R = 5 B flow_h flow_w.
+ * 0 (with pmvs_last_error) unless bn_eval = 1, ratio 1 and sub_count 0. */
+size_t pmvs_point_flow_eval_keep_workspace_bytes(const pmvs_flow_shape* shape);
+
+/* pmvs_point_flow_iter with bn_eval = 1 (required; anything else is PMVS_ERR_ARG), one cloud per call, that also keeps
+ * in its workspace what pmvs_point_flow_eval_backward reads: flow_mlp's pre-BatchNorm outputs, the flow head's
+ * inputs and the running mean and variance of the six layers as this call read them.  Same launches as the eval
+ * iteration; depth_out and prob_out are bit-identical to pmvs_point_flow_iter's. */
+int pmvs_point_flow_eval_keep(const pmvs_flow_shape* shape, const pmvs_flow_weights* weights,
+                              const float* const pyramids_cl[3], const float* depth_prev,
+                              const float* cam_params, const float* interval, const float* mean,
+                              const float* std, float* depth_out, float* prob_out, void* workspace,
+                              size_t workspace_bytes, pmvs_stream_t stream);
+
+/* bytes of device workspace pmvs_point_flow_eval_backward needs; 0 (with pmvs_last_error) for a shape it does not
+ * take (bn_eval != 1, ratio != 1, sub_count != 0). */
+size_t pmvs_point_flow_eval_backward_workspace_bytes(const pmvs_flow_shape* shape);
+
+/* pmvs_point_flow_backward for a pmvs_point_flow_eval_keep forward: fwd_workspace is that call's workspace, unchanged
+ * since.  Each BatchNorm is the affine map of the running statistics the forward read (its kept copy; the live
+ * buffers are not read): dx = g gamma / sqrt(running_var + eps), dgamma = sum g xhat, dbeta = sum g, g the upstream
+ * gradient after the forward's ReLU mask, recomputed from the forward's own coefficients.  The running statistics
+ * are not written.  Same outputs, options and determinism as pmvs_point_flow_backward. */
+int pmvs_point_flow_eval_backward(const pmvs_flow_shape* shape, const pmvs_flow_weights* weights,
+                                  const float* const pyramids_cl[3], const float* depth_prev,
+                                  const float* cam_params, const float* interval, const float* mean,
+                                  const float* std, const void* fwd_workspace, const float* grad_depth_out,
+                                  const float* grad_prob_out, const pmvs_flow_grads* grads, void* workspace,
+                                  size_t workspace_bytes, pmvs_stream_t stream);
 
 /* ---- training loss and metrics (DESIGN 3.16; model.py:308-420, networks.py:170-181 MAELoss) ------------------- */
 /* The T predicted depth maps a step is scored on: T = 1 (coarse_depth_map, isFlow false) or T = 3 (coarse_depth_map,

@@ -142,6 +142,12 @@ _sig("pmvs_point_flow_debug_feature", I, [C.POINTER(FlowShape), P, P, P])
 _sig("pmvs_point_flow_backward_workspace_bytes", C.c_size_t, [C.POINTER(FlowShape)])
 _sig("pmvs_point_flow_backward", I, [C.POINTER(FlowShape), C.POINTER(FlowWeights), C.POINTER(C.c_void_p * 3),
                                      P, P, P, P, P, P, P, P, C.POINTER(FlowGrads), P, C.c_size_t, P])
+_sig("pmvs_point_flow_eval_keep_workspace_bytes", C.c_size_t, [C.POINTER(FlowShape)])
+_sig("pmvs_point_flow_eval_keep", I, [C.POINTER(FlowShape), C.POINTER(FlowWeights), C.POINTER(C.c_void_p * 3),
+                                      P, P, P, P, P, P, P, P, C.c_size_t, P])
+_sig("pmvs_point_flow_eval_backward_workspace_bytes", C.c_size_t, [C.POINTER(FlowShape)])
+_sig("pmvs_point_flow_eval_backward", I, [C.POINTER(FlowShape), C.POINTER(FlowWeights), C.POINTER(C.c_void_p * 3),
+                                          P, P, P, P, P, P, P, P, C.POINTER(FlowGrads), P, C.c_size_t, P])
 _sig("pmvs_depth_loss", I, [C.POINTER(DepthTerms), P, I, I, P, I, I, F, P, P, P, P])
 _sig("pmvs_depth_loss_backward", I, [C.POINTER(DepthTerms), P, I, I, P, I, I, P, P, C.POINTER(C.c_void_p * 3), P])
 
@@ -159,7 +165,8 @@ EXPORTED = [
     "pmvs_transpose", "pmvs_idx64_to_idx32", "pmvs_edgeconv_pm", "pmvs_edgeconv_pm_backward_workspace_bytes", "pmvs_edgeconv_pm_backward", "pmvs_linear_pm", "pmvs_point_flow_workspace_bytes",
     "pmvs_point_flow_iter", "pmvs_pyramid_to_channels_last", "pmvs_point_flow_debug_offsets",
     "pmvs_point_flow_debug_feature", "pmvs_point_flow_backward_workspace_bytes", "pmvs_point_flow_backward",
-    "pmvs_depth_loss", "pmvs_depth_loss_backward",
+    "pmvs_depth_loss", "pmvs_depth_loss_backward", "pmvs_point_flow_eval_keep_workspace_bytes",
+    "pmvs_point_flow_eval_keep", "pmvs_point_flow_eval_backward_workspace_bytes", "pmvs_point_flow_eval_backward",
 ]
 
 

@@ -148,9 +148,12 @@ struct FlowPlan {
   size_t coef;         // [3][S][6*64] floats: per (layer, group) BatchNorm coefficients of the tile apply kernels
   size_t mlp_coef;     // bn_eval: FLOW_EVAL_MLP_COEF floats after the tile tables (flow_mlp's BatchNorms)
   bool eval;           // bn_eval: running statistics; no stats, h0, h1 or h2 regions (their offsets are 0)
+  // keep (pmvs_point_flow_eval_keep): h0, h1, h2 after every eval region, then the raw flow_mlp outputs [R] and the
+  // copy of the running statistics (FLOW_EVAL_RUN floats); 0 otherwise
+  size_t raw, run;
 };
 
-static int make_plan(const pmvs_flow_shape* s, FlowPlan& p) {
+static int make_plan(const pmvs_flow_shape* s, FlowPlan& p, bool keep = false) {
   PMVS_REQUIRE(s != nullptr, "point_flow: NULL shape");
   PMVS_REQUIRE(s->B > 0 && s->V > 0 && s->V <= PMVS_MAX_VIEWS, "point_flow: B=%d V=%d (V <= %d)", s->B, s->V,
                PMVS_MAX_VIEWS);
@@ -211,6 +214,19 @@ static int make_plan(const pmvs_flow_shape* s, FlowPlan& p) {
   if (p.eval) {
     p.mlp_coef = o; o += up256(FLOW_EVAL_MLP_COEF * sizeof(float));
   }
+  p.raw = p.run = 0;
+  if (keep) {
+    // what the eval backward reads, which serves one cloud per call
+    PMVS_REQUIRE(p.eval, "point_flow_eval_keep: bn_eval must be 1, got %d", s->bn_eval);
+    PMVS_REQUIRE(s->ratio == 1 && s->sub_count == 0 && s->sub_begin == 0,
+                 "point_flow_eval_keep: only one cloud per call (ratio 1, no sub_count); got ratio %d, sub_count %d",
+                 s->ratio, s->sub_count);
+    p.h0 = o; o += up256(p.R * 64 * 4);
+    p.h1 = o; o += up256(p.R * 64 * 4);
+    p.h2 = o; o += up256(p.R * 16 * 4);
+    p.raw = o; o += up256(p.R * 4);
+    p.run = o; o += up256(FLOW_EVAL_RUN * sizeof(float));
+  }
   p.total = o;
   return PMVS_OK;
 }
@@ -226,12 +242,12 @@ static FusedFetchParams fetch_params(const pmvs_flow_shape* s, const FlowPlan& p
   return f;
 }
 
-int flow_regions(const pmvs_flow_shape* s, FlowRegions& r) {
+int flow_regions(const pmvs_flow_shape* s, FlowRegions& r, bool keep) {
   FlowPlan p;
-  PMVS_TRY(make_plan(s, p));
+  PMVS_TRY(make_plan(s, p, keep));
   r.cam = p.cam; r.feature = p.feature; r.xyz = p.xyz; r.idx = p.idx; r.le = p.le; r.ecat = p.ecat; r.h0 = p.h0;
   r.h1 = p.h1; r.h2 = p.h2; r.warp_src = p.warp_src; r.cand = p.cand; r.stats = p.stats; r.coef = p.coef;
-  r.total = p.total;
+  r.mlp_coef = p.mlp_coef; r.raw = p.raw; r.run = p.run; r.total = p.total;
   for (int l = 0; l < 3; ++l) { r.st_ec[l] = p.st_ec[l]; r.st_ecn[l] = p.st_ecn[l]; r.st_mlp[l] = p.st_mlp[l]; }
   r.S = p.S;
   return PMVS_OK;
@@ -384,13 +400,13 @@ extern "C" int pmvs_point_flow_debug_feature(const pmvs_flow_shape* shape, const
   return launch_fused_fetch(fetch_params(shape, p, (char*)workspace, depth_prev), (cudaStream_t)stream);
 }
 
-extern "C" int pmvs_point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flow_weights* wts,
-                                    const float* const pyramids_cl[3], const float* depth_prev,
-                                    const float* cam_params, const float* interval, const float* mean,
-                                    const float* stdv, float* depth_out, float* prob_out, void* workspace,
-                                    size_t workspace_bytes, pmvs_stream_t stream) {
+// pmvs_point_flow_iter, and with keep pmvs_point_flow_eval_keep
+static int point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flow_weights* wts,
+                           const float* const pyramids_cl[3], const float* depth_prev, const float* cam_params,
+                           const float* interval, const float* mean, const float* stdv, float* depth_out,
+                           float* prob_out, void* workspace, size_t workspace_bytes, pmvs_stream_t stream, bool keep) {
   FlowPlan p;
-  PMVS_TRY(make_plan(shape, p));
+  PMVS_TRY(make_plan(shape, p, keep));
   PMVS_REQUIRE(wts && pyramids_cl && depth_prev && cam_params && interval && mean && stdv && depth_out && workspace,
                "point_flow: NULL pointer");
   PMVS_TRY(check_workspace("point_flow", workspace, workspace_bytes, p.total));
@@ -450,7 +466,8 @@ extern "C" int pmvs_point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flo
 
   // running statistics: every BatchNorm coefficient is known before the first layer (flow_eval.cu)
   if (p.eval)
-    PMVS_TRY(launch_flow_eval_coef(*wts, S, (float*)(ws + p.coef), (float*)(ws + p.mlp_coef), st));
+    PMVS_TRY(launch_flow_eval_coef(*wts, S, (float*)(ws + p.coef), (float*)(ws + p.mlp_coef),
+                                   keep ? (float*)(ws + p.run) : nullptr, st));
 
   // flow_edge_conv (model.py:213-216): EdgeConvNoC(136,32), EdgeConv(32,32), EdgeConv(64,64)
   const int cin[3] = {136, 32, 64}, cout[3] = {32, 32, 64}, in_off[3] = {0, 0, 32}, out_off[3] = {0, 32, 96};
@@ -497,6 +514,9 @@ extern "C" int pmvs_point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flo
     h.prob_out = prob_out; h.eps = wts->eps; h.interval_scale = shape->interval_scale; h.B = B; h.S = S;
     h.ratio = shape->ratio; h.sub_begin = p.sub_begin; h.h = shape->flow_h; h.w = shape->flow_w;
     h.hp = shape->prev_h; h.wp = shape->prev_w;
+    if (keep) {
+      fa.keep_h[0] = h0; fa.keep_h[1] = h1; fa.keep_h[2] = h2; fa.keep_raw = (float*)(ws + p.raw);
+    }
     return launch_flow_mlp_head_eval(fa, st);
   }
 
@@ -563,4 +583,28 @@ extern "C" int pmvs_point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flo
   }
   PMVS_TRY(launch_bn_running_update(rb, st));
   return PMVS_OK;
+}
+
+extern "C" int pmvs_point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flow_weights* wts,
+                                    const float* const pyramids_cl[3], const float* depth_prev,
+                                    const float* cam_params, const float* interval, const float* mean,
+                                    const float* stdv, float* depth_out, float* prob_out, void* workspace,
+                                    size_t workspace_bytes, pmvs_stream_t stream) {
+  return point_flow_iter(shape, wts, pyramids_cl, depth_prev, cam_params, interval, mean, stdv, depth_out, prob_out,
+                         workspace, workspace_bytes, stream, false);
+}
+
+extern "C" size_t pmvs_point_flow_eval_keep_workspace_bytes(const pmvs_flow_shape* shape) {
+  FlowPlan p;
+  if (make_plan(shape, p, true) != PMVS_OK) return 0;
+  return p.total;
+}
+
+extern "C" int pmvs_point_flow_eval_keep(const pmvs_flow_shape* shape, const pmvs_flow_weights* wts,
+                                         const float* const pyramids_cl[3], const float* depth_prev,
+                                         const float* cam_params, const float* interval, const float* mean,
+                                         const float* stdv, float* depth_out, float* prob_out, void* workspace,
+                                         size_t workspace_bytes, pmvs_stream_t stream) {
+  return point_flow_iter(shape, wts, pyramids_cl, depth_prev, cam_params, interval, mean, stdv, depth_out, prob_out,
+                         workspace, workspace_bytes, stream, true);
 }

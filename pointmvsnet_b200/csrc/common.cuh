@@ -374,23 +374,41 @@ constexpr int FLOW_EVAL_MLP_COEF = 2 * (64 + 64 + 16);
 // From the running statistics of `w`: the edge_tile coefficient table of the three EdgeConv layers for each of the S
 // groups (ec_coef + l * S * 6 * 64 + g * 6 * cout, the layout of edge_tile.cu) and flow_mlp's table (mlp_coef).  One
 // launch, on the device, so a replayed CUDA graph reads the buffers as they are at replay time.
-int launch_flow_eval_coef(const pmvs_flow_weights& w, int S, float* ec_coef, float* mlp_coef, cudaStream_t st);
+// run_copy != NULL (pmvs_point_flow_eval_keep): the running mean and variance as read, FLOW_EVAL_RUN floats at
+// flow_eval_run_offset(l) (layers 0-2 the EdgeConvs, 3-5 flow_mlp): [mean | var] x flow_eval_run_channels(l).
+int launch_flow_eval_coef(const pmvs_flow_weights& w, int S, float* ec_coef, float* mlp_coef, float* run_copy,
+                          cudaStream_t st);
+constexpr int FLOW_EVAL_RUN = 2 * (32 + 64 + 128 + 64 + 64 + 16);
+__host__ __device__ __forceinline__ int flow_eval_run_channels(int l) {
+  return l == 0 ? 32 : l == 1 ? 64 : l == 2 ? 128 : l == 5 ? 16 : 64;
+}
+__host__ __device__ __forceinline__ int flow_eval_run_offset(int l) {
+  int o = 0;
+  for (int i = 0; i < l; ++i) o += 2 * flow_eval_run_channels(i);
+  return o;
+}
 struct FlowEvalArgs {
   const float* ecat;      // [S*B*N, 224], the concatenated EdgeConv outputs
   const float* w[3];      // flow_mlp.0.{0,1,2}.conv.weight [64,224], [64,64], [16,64]
   const float* mlp_coef;  // FLOW_EVAL_MLP_COEF floats (launch_flow_eval_coef)
   HeadArgs head;          // w3, depth_prev, interval, outputs and grid; h2 / stats / gamma / beta are not read
+  // NULL, or (pmvs_point_flow_eval_keep) what the backward reads: the pre-BatchNorm h0 [R, 64], h1 [R, 64],
+  // h2 [R, 16] and the raw flow_mlp output [R] as the kernel computed them, rows in the batch-statistics layout
+  float* keep_h[3];
+  float* keep_raw;
 };
 // flow_mlp (224 -> 64 -> 64 -> 16 -> 1) and the flow head in one persistent launch: h0, h1, h2 never leave the SM
+// (unless keep_h is given)
 int launch_flow_mlp_head_eval(const FlowEvalArgs& a, cudaStream_t st);
 // byte offsets of the regions of pmvs_point_flow_iter's workspace (api.cu make_plan) and the double offsets of the
-// BatchNorm sums inside `stats`, for the backward that reads it
+// BatchNorm sums inside `stats`, for the backward that reads it.  keep: pmvs_point_flow_eval_keep's workspace, whose
+// h0-h2, raw (the flow head's input [R]), run (FLOW_EVAL_RUN floats) and mlp_coef regions the eval backward reads.
 struct FlowRegions {
-  size_t cam, feature, xyz, idx, le, ecat, h0, h1, h2, warp_src, cand, stats, coef, total;
+  size_t cam, feature, xyz, idx, le, ecat, h0, h1, h2, warp_src, cand, stats, coef, mlp_coef, raw, run, total;
   size_t st_ec[3], st_ecn[3], st_mlp[3];
   int S;
 };
-int flow_regions(const pmvs_flow_shape* s, FlowRegions& r);
+int flow_regions(const pmvs_flow_shape* s, FlowRegions& r, bool keep = false);
 // whether launch_gemm applies a fused input BatchNorm as relu(fma(x, A, B)) (gemm_ws.cu) rather than ATen's
 // ((x - mean) * invstd) * gamma + beta (the other kernels); the two can differ in the last bit of the pre-activation
 bool gemm_in_bn_fma_form(const GemmArgs& a);

@@ -53,7 +53,8 @@ struct BwdArgs {
   float* dle;  // [R, 2*cout]
   int R, N, K, cout;
   // NULL: the neighbour pre-activation is edge_nb_pre(e, A, edge_nb_offset(mean, l, A, beta)) (edge_kernel's sequence);
-  // else the tile family's table (edge_tile.cu, [A | B] x cout): fma(e, A, fma(-l, A, B)), the sequence it applied
+  // else the tile family's table (edge_tile.cu, [A | B | mean | invstd | gamma | beta] x cout): fma(e, A, fma(-l, A, B)),
+  // the sequence it applied, and the central half's mean and invstd as it applied them
   const float* tcoef;
 };
 
@@ -61,6 +62,13 @@ struct BwdArgs {
 __device__ __forceinline__ float bwd_nb_offset(const float* tcoef, int c, int cout, float mean, float l, float A,
                                                float beta) {
   return tcoef ? __fmaf_rn(-l, A, __ldg(tcoef + cout + c)) : edge_nb_offset(mean, l, A, beta);
+}
+
+// the central half's mean and invstd: the tile table's (with batch statistics the same bn_coef of the same sums; with
+// running statistics the values the forward computed from them), else from the sums
+__device__ __forceinline__ BnCoef central_coef(const BwdArgs& a, int c, int cout) {
+  if (a.tcoef) return BnCoef{__ldg(a.tcoef + 2 * cout + c), __ldg(a.tcoef + 3 * cout + c)};
+  return bn_coef(a.stats[c], a.stats[cout + c], (double)a.R, a.eps);
 }
 
 __device__ __forceinline__ float bwd_xhat(float d, float mean, float istd) { return __fmul_rn(__fsub_rn(d, mean), istd); }
@@ -92,7 +100,7 @@ __global__ void __launch_bounds__(EB_THREADS) edge_bwd_stats_kernel(const BwdArg
     const int gn = a.concat_central ? COUT + c : c;
     c_mean[1][c] = kn.mean; c_istd[1][c] = kn.invstd; c_g[1][c] = a.gamma[gn]; c_b[1][c] = a.beta[gn];
     if (a.concat_central) {
-      BnCoef kc = bn_coef(a.stats[c], a.stats[COUT + c], (double)a.R, a.eps);
+      BnCoef kc = central_coef(a, c, COUT);
       c_mean[0][c] = kc.mean; c_istd[0][c] = kc.invstd; c_g[0][c] = a.gamma[c]; c_b[0][c] = a.beta[c];
     }
   }
@@ -203,7 +211,7 @@ __global__ void __launch_bounds__(FIN_THREADS) edge_bwd_finish_kernel(const BwdA
   a.dbeta[gn] = (float)sums[2];
   a.dgamma[gn] = (float)sums[3];
   if (a.concat_central) {
-    BnCoef kc = bn_coef(a.stats[c], a.stats[C + c], Mc, a.eps);
+    BnCoef kc = central_coef(a, c, C);
     float* cc = a.coef;
     cc[CF_MEAN * C + c] = kc.mean; cc[CF_ISTD * C + c] = kc.invstd;
     cc[CF_GAMMA * C + c] = a.gamma[c]; cc[CF_BETA * C + c] = a.beta[c];

@@ -15,6 +15,16 @@
 //             the records sorted by texel (build_inv_lists) and summed per texel in record order; the transposes of
 //             the bilinear and nearest resizes as gathers over fixed windows
 // No floating-point atomics: every sum has an order fixed by the shapes, so two calls give the same bits.
+//
+// pmvs_point_flow_eval_backward is the same chain for a forward with running-statistics BatchNorm
+// (pmvs_point_flow_eval_keep, which kept h0-h2, the raw flow_mlp outputs and a copy of the running statistics).  Each
+// BatchNorm is then the affine map relu(fma(h, A, B)): dh = g A, dgamma = sum g xhat, dbeta = sum g with no batch
+// terms, so
+//   head      as above, from the kept raw outputs (the fused kernel's summation order) and the kept coefficient table
+//   MLP x3    mlp_bwd_eval: dh and the per-CTA partial sums in one pass (nothing global to wait for)
+//   EdgeConv  edge_layer_backward with bn_train = 0, the kept running statistics as sums (ec_run_sums_kernel) and the
+//             forward's tile table for every ReLU mask
+// and everything else (rows, inverse lists, F0, LE, fetch, resizes) is shared with the batch-statistics backward.
 #include <algorithm>
 
 #include "common.cuh"
@@ -52,17 +62,25 @@ __global__ void __launch_bounds__(256) flow_idx_kernel(const unsigned short* __r
 }
 
 // one thread per pixel: d prob and d depth through flow = sum_m softmax(-raw)_m (m - 2) interval (model.py:222-227) ->
-// draw_m; dA2[row][c] = draw * w3[c]; per-CTA partials of dw3[c] = sum draw * relu(bn(h2))[c]
+// draw_m; dA2[row][c] = draw * w3[c]; per-CTA partials of dw3[c] = sum draw * relu(bn(h2))[c].
+// EVAL: raw is the forward's (eraw [R]) and relu(bn(h2)) = relu(fma(h2, A2, B2)) from its table (ecoef [A2 | B2]).
+template <bool EVAL>
 __global__ void __launch_bounds__(HEAD_THREADS) head_bwd_kernel(const HeadArgs a, const float* __restrict__ dprob,
                                                                 const float* __restrict__ ddepth, float* __restrict__ dA,
-                                                                float* __restrict__ part) {
+                                                                float* __restrict__ part, const float* __restrict__ eraw,
+                                                                const float* __restrict__ ecoef) {
   __shared__ float cm[16], ci[16], cg[16], cb[16], cw[16];
   __shared__ float red[HEAD_THREADS / 32][16];
   const int P = a.h * a.w, N = PMVS_NUM_HYP * P;
   if (threadIdx.x < 16) {
-    BnCoef k = bn_coef(a.stats[threadIdx.x], a.stats[16 + threadIdx.x], (double)a.B * N, a.eps);
-    cm[threadIdx.x] = k.mean; ci[threadIdx.x] = k.invstd;
-    cg[threadIdx.x] = a.gamma[threadIdx.x]; cb[threadIdx.x] = a.beta[threadIdx.x]; cw[threadIdx.x] = a.w3[threadIdx.x];
+    if constexpr (EVAL) {
+      cm[threadIdx.x] = ecoef[threadIdx.x]; ci[threadIdx.x] = ecoef[16 + threadIdx.x];  // A2, B2
+    } else {
+      BnCoef k = bn_coef(a.stats[threadIdx.x], a.stats[16 + threadIdx.x], (double)a.B * N, a.eps);
+      cm[threadIdx.x] = k.mean; ci[threadIdx.x] = k.invstd;
+      cg[threadIdx.x] = a.gamma[threadIdx.x]; cb[threadIdx.x] = a.beta[threadIdx.x];
+    }
+    cw[threadIdx.x] = a.w3[threadIdx.x];
   }
   __syncthreads();
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -74,7 +92,8 @@ __global__ void __launch_bounds__(HEAD_THREADS) head_bwd_kernel(const HeadArgs a
     float act[PMVS_NUM_HYP][16], raw[PMVS_NUM_HYP];
 #pragma unroll
     for (int m = 0; m < PMVS_NUM_HYP; ++m) {  // flow_head_kernel's arithmetic
-      const float* hrow = a.h2 + ((size_t)b * N + (size_t)m * P + pp) * 16;
+      const size_t row = (size_t)b * N + (size_t)m * P + pp;
+      const float* hrow = a.h2 + row * 16;
       float acc = 0.f;
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
@@ -83,11 +102,15 @@ __global__ void __launch_bounds__(HEAD_THREADS) head_bwd_kernel(const HeadArgs a
 #pragma unroll
         for (int r = 0; r < 4; ++r) {
           const int c = q * 4 + r;
-          act[m][c] = fmaxf(bn_apply(vv[r], cm[c], ci[c], cg[c], cb[c]), 0.f);
-          acc = fmaf(act[m][c], cw[c], acc);
+          if constexpr (EVAL) {
+            act[m][c] = fmaxf(fmaf(vv[r], cm[c], ci[c]), 0.f);
+          } else {
+            act[m][c] = fmaxf(bn_apply(vv[r], cm[c], ci[c], cg[c], cb[c]), 0.f);
+            acc = fmaf(act[m][c], cw[c], acc);
+          }
         }
       }
-      raw[m] = acc;
+      raw[m] = EVAL ? __ldg(eraw + row) : acc;
     }
     float mx = -raw[0];
 #pragma unroll
@@ -155,11 +178,24 @@ struct MlpBn {
   float eps;
   int fma_form;  // 1: relu(fma(x, A, B)) (gemm_ws.cu), 0: ATen's ((x - mean) * invstd) * gamma + beta
   int R, C;
+  // running statistics (the eval backward): the forward's [A | B] table and the running mean / variance it was built
+  // from; stats and count are then not read, and the form is fma
+  const float* ecoef;
+  const float* rmean;
+  const float* rvar;
 };
 struct MlpCoef {
   float mean, istd, A, B;
 };
 __device__ __forceinline__ MlpCoef mlp_coef(const MlpBn& a, int c) {
+  if (a.ecoef) {
+    MlpCoef o;
+    o.mean = a.rmean[c];
+    o.istd = (float)(1.0 / sqrt((double)a.rvar[c] + (double)a.eps));  // flow_eval_coef_kernel's
+    o.A = a.ecoef[c];
+    o.B = a.ecoef[a.C + c];
+    return o;
+  }
   const BnCoef k = bn_coef(a.stats[c], a.stats[a.C + c], a.count, a.eps);
   MlpCoef o;
   o.mean = k.mean; o.istd = k.invstd;
@@ -246,6 +282,56 @@ __global__ void __launch_bounds__(256) mlp_bwd_apply_kernel(const MlpBn a, const
   dh[e] = __fmul_rn(k.A, __fsub_rn(__fsub_rn(g, coef[2 * c]), __fmul_rn(xh, coef[2 * c + 1])));
 }
 
+// running statistics: dh = A g, g = dA [pre > 0], and per-CTA partial sums of g and g * xhat over FB_ROWS rows (the
+// layout of mlp_bwd_stats_kernel, for mlp_bwd_finish_kernel)
+__global__ void __launch_bounds__(256) mlp_bwd_eval_kernel(const MlpBn a, const float* __restrict__ dA,
+                                                           float* __restrict__ dh, double* __restrict__ part) {
+  __shared__ float red[256][2];
+  const int C = a.C, slots = 256 / C, c = threadIdx.x % C, slot = threadIdx.x / C;
+  const MlpCoef k = mlp_coef(a, c);
+  float s1 = 0.f, s2 = 0.f;
+  const int r0 = blockIdx.x * FB_ROWS;
+  for (int r = r0 + slot; r < min(r0 + FB_ROWS, a.R); r += slots) {
+    const size_t e = (size_t)r * C + c;
+    const float x = a.h[e];
+    const float g = fmaf(x, k.A, k.B) > 0.f ? dA[e] : 0.f;
+    dh[e] = __fmul_rn(k.A, g);
+    s1 += g;
+    s2 = fmaf(g, __fmul_rn(__fsub_rn(x, k.mean), k.istd), s2);
+  }
+  red[threadIdx.x][0] = s1;
+  red[threadIdx.x][1] = s2;
+  __syncthreads();
+  if (threadIdx.x < C) {
+    double t1 = 0.0, t2 = 0.0;
+    for (int q = 0; q < slots; ++q) {
+      t1 += (double)red[q * C + threadIdx.x][0];
+      t2 += (double)red[q * C + threadIdx.x][1];
+    }
+    part[(size_t)blockIdx.x * 2 * C + threadIdx.x] = t1;
+    part[(size_t)blockIdx.x * 2 * C + C + threadIdx.x] = t2;
+  }
+}
+
+// the kept running statistics of the three EdgeConv layers as the sums edge_layer_backward reads, in the form the
+// stand-alone EdgeConv's eval mode builds (networks.py): [m R | (v + m^2) R | m' R K | (v' + m'^2) R K] per layer at
+// s4 + l * 4 * 64, m / v the central half's (channels [0, C)), m' / v' the neighbour half's
+__global__ void __launch_bounds__(128) ec_run_sums_kernel(const float* __restrict__ run, double* __restrict__ s4,
+                                                          double R) {
+  const int l = blockIdx.x, C = l == 2 ? 64 : 32, c = threadIdx.x;
+  if (c >= C) return;
+  const float* rm = run + flow_eval_run_offset(l);
+  const int ctot = flow_eval_run_channels(l);
+  const float* rv = rm + ctot;
+  const int gn = l > 0 ? C + c : c;
+  const double mc = rm[c], vc = rv[c], mn = rm[gn], vn = rv[gn];
+  double* o = s4 + (size_t)l * 4 * 64;
+  o[c] = mc * R;
+  o[C + c] = (vc + mc * mc) * R;
+  o[2 * C + c] = mn * (R * PMVS_KNN);
+  o[3 * C + c] = (vn + mn * mn) * (R * PMVS_KNN);
+}
+
 // y[r, 0:n] += x[r, 0:n]  (row strides ldy, n)
 __global__ void __launch_bounds__(256) add_cols_kernel(float* __restrict__ y, int ldy, const float* __restrict__ x, int n,
                                                        long long R) {
@@ -293,15 +379,24 @@ struct BwdFlowPlan {
   size_t ddup, dfv, rec_idx, rec_w, rec_inv, dsrc, total;
 };
 
-// the backward takes S = 1: the train branch (ratio 1) and the test branch at scale 0.125
-int bwd_flow_plan(const pmvs_flow_shape* s, BwdFlowPlan& p) {
+// the backward takes S = 1: the train branch (ratio 1) and the test branch at scale 0.125.  eval: the backward of
+// pmvs_point_flow_eval_keep (bn_eval = 1)
+int bwd_flow_plan(const pmvs_flow_shape* s, BwdFlowPlan& p, bool eval) {
   PMVS_REQUIRE(s != nullptr, "point_flow_backward: NULL shape");
-  PMVS_REQUIRE(s->bn_eval == 0, "point_flow_backward: the forward ran with bn_eval = 1 (running-statistics BatchNorm), "
-               "which has no backward");
+  if (eval) {
+    PMVS_REQUIRE(s->bn_eval == 1, "point_flow_eval_backward: bn_eval must be 1, got %d", s->bn_eval);
+    // the keep forward runs on the tile EdgeConv family only, so its workspace has no gather-family rows or sums
+    PMVS_REQUIRE(opt(OPT_EDGE) != 0, "point_flow_eval_backward: served by the tile EdgeConv kernels only (option "
+                 "edge=%d)", opt(OPT_EDGE));
+  } else {
+    PMVS_REQUIRE(s->bn_eval == 0, "point_flow_backward: the forward ran with bn_eval = 1 (running-statistics "
+                 "BatchNorm); its backward is pmvs_point_flow_eval_backward");
+  }
   PMVS_REQUIRE(s->ratio == 1 && s->sub_count == 0 && s->sub_begin == 0,
                "point_flow_backward: only one cloud per call (ratio 1, no sub_count); got ratio %d, sub_count %d",
                s->ratio, s->sub_count);
-  PMVS_REQUIRE(pmvs_point_flow_workspace_bytes(s) != 0, "%s", pmvs_last_error());
+  PMVS_REQUIRE((eval ? pmvs_point_flow_eval_keep_workspace_bytes(s) : pmvs_point_flow_workspace_bytes(s)) != 0, "%s",
+               pmvs_last_error());
   p.N = PMVS_NUM_HYP * s->flow_h * s->flow_w;
   p.R = (size_t)s->B * p.N;
   p.npix = (size_t)s->B * s->flow_h * s->flow_w;
@@ -362,6 +457,16 @@ int mlp_layer_backward(const MlpBn& a, const float* dA, float* dh, double* part,
   return check_launch("mlp_bwd_apply_kernel", st);
 }
 
+int mlp_layer_backward_eval(const MlpBn& a, const float* dA, float* dh, double* part, float* coef, float* dgamma,
+                            float* dbeta, int ctas, cudaStream_t st) {
+  prof_begin("mlp_bwd_eval", st);
+  mlp_bwd_eval_kernel<<<ctas, 256, 0, st>>>(a, dA, dh, part);
+  PMVS_TRY(check_launch("mlp_bwd_eval_kernel", st));
+  prof_begin("mlp_bwd_finish", st);
+  mlp_bwd_finish_kernel<<<a.C, 256, 0, st>>>(part, ctas, a.C, 1.0, dgamma, dbeta, coef);
+  return check_launch("mlp_bwd_finish_kernel", st);
+}
+
 int mlp_act(const MlpBn& a, float* out, cudaStream_t st) {
   prof_begin("mlp_bwd_act", st);
   mlp_act_kernel<<<cdiv((long long)a.R * a.C, 256), 256, 0, st>>>(a, out);
@@ -384,26 +489,14 @@ int add_cols(float* y, int ldy, const float* x, int n, long long R, cudaStream_t
   return check_launch("add_cols_kernel", st);
 }
 
-}  // namespace
-
-}  // namespace pmvs
-
-using namespace pmvs;
-
-extern "C" size_t pmvs_point_flow_backward_workspace_bytes(const pmvs_flow_shape* shape) {
+// pmvs_point_flow_backward, and with eval pmvs_point_flow_eval_backward
+int point_flow_backward(const pmvs_flow_shape* shape, const pmvs_flow_weights* wts, const float* const pyramids_cl[3],
+                        const float* depth_prev, const float* cam_params, const float* interval, const float* mean,
+                        const float* stdv, const void* fwd_workspace, const float* grad_depth_out,
+                        const float* grad_prob_out, const pmvs_flow_grads* grads, void* workspace,
+                        size_t workspace_bytes, pmvs_stream_t stream, bool eval) {
   BwdFlowPlan p;
-  if (bwd_flow_plan(shape, p) != PMVS_OK) return 0;
-  return p.total;
-}
-
-extern "C" int pmvs_point_flow_backward(const pmvs_flow_shape* shape, const pmvs_flow_weights* wts,
-                                        const float* const pyramids_cl[3], const float* depth_prev,
-                                        const float* cam_params, const float* interval, const float* mean,
-                                        const float* stdv, const void* fwd_workspace, const float* grad_depth_out,
-                                        const float* grad_prob_out, const pmvs_flow_grads* grads, void* workspace,
-                                        size_t workspace_bytes, pmvs_stream_t stream) {
-  BwdFlowPlan p;
-  PMVS_TRY(bwd_flow_plan(shape, p));
+  PMVS_TRY(bwd_flow_plan(shape, p, eval));
   PMVS_REQUIRE(wts && pyramids_cl && depth_prev && cam_params && interval && mean && stdv && fwd_workspace &&
                    grad_depth_out && grads && workspace,
                "point_flow_backward: NULL pointer");
@@ -416,7 +509,7 @@ extern "C" int pmvs_point_flow_backward(const pmvs_flow_shape* shape, const pmvs
   PMVS_TRY(check_workspace("point_flow_backward", workspace, workspace_bytes, p.total));
   (void)cam_params; (void)mean; (void)stdv;  // the forward's camera blocks already hold them
   FlowRegions fr;
-  PMVS_TRY(flow_regions(shape, fr));
+  PMVS_TRY(flow_regions(shape, fr, eval));
   const bool gather = opt(OPT_EDGE) == 0;  // the EdgeConv family of the forward (the options must not change between)
   cudaStream_t st = (cudaStream_t)stream;
   const char* fw = (const char*)fwd_workspace;
@@ -432,6 +525,9 @@ extern "C" int pmvs_point_flow_backward(const pmvs_flow_shape* shape, const pmvs
   const float* fcoef = (const float*)(fw + fr.coef);
   const float* warp_src = (const float*)(fw + fr.warp_src);
   const float* cam_blocks = (const float*)(fw + fr.cam);
+  // eval: the forward's flow_mlp table, raw outputs and running statistics
+  const float* ecoef = eval ? (const float*)(fw + fr.mlp_coef) : nullptr;
+  const float* run = eval ? (const float*)(fw + fr.run) : nullptr;
   const int ec_cout[3] = {32, 32, 64}, ec_cin[3] = {136, 32, 64}, mlp_cout[3] = {64, 64, 16}, mlp_cin[3] = {224, 64, 64};
   const size_t* st_ec = fr.st_ec;
   const size_t* st_ecn = fr.st_ecn;
@@ -449,8 +545,15 @@ extern "C" int pmvs_point_flow_backward(const pmvs_flow_shape* shape, const pmvs
   ha.h2 = h2; ha.stats = stats + st_mlp[2]; ha.gamma = wts->mlp_gamma[2]; ha.beta = wts->mlp_beta[2];
   ha.w3 = wts->mlp_w[3]; ha.interval = interval; ha.eps = eps; ha.interval_scale = shape->interval_scale;
   ha.B = B; ha.S = 1; ha.ratio = 1; ha.h = h; ha.w = w;
-  prof_begin("head_bwd", st);
-  head_bwd_kernel<<<p.head_ctas, HEAD_THREADS, 0, st>>>(ha, grad_prob_out, grad_depth_out, F(p.dA), F(p.hpart));
+  if (eval) {
+    prof_begin("head_bwd_eval", st);
+    head_bwd_kernel<true><<<p.head_ctas, HEAD_THREADS, 0, st>>>(ha, grad_prob_out, grad_depth_out, F(p.dA),
+                                                                F(p.hpart), (const float*)(fw + fr.raw), ecoef + 256);
+  } else {
+    prof_begin("head_bwd", st);
+    head_bwd_kernel<false><<<p.head_ctas, HEAD_THREADS, 0, st>>>(ha, grad_prob_out, grad_depth_out, F(p.dA),
+                                                                 F(p.hpart), nullptr, nullptr);
+  }
   PMVS_TRY(check_launch("head_bwd_kernel", st));
   prof_begin("head_bwd_reduce", st);
   ordered_sum_kernel<<<1, 256, 0, st>>>(F(p.hpart), grads->mlp_dw[3], 16, p.head_ctas);
@@ -463,11 +566,18 @@ extern "C" int pmvs_point_flow_backward(const pmvs_flow_shape* shape, const pmvs
       MlpBn a{};
       a.h = hs[l]; a.stats = stats + st_mlp[l]; a.gamma = wts->mlp_gamma[l]; a.beta = wts->mlp_beta[l];
       a.count = (double)R; a.eps = eps; a.fma_form = fma_form; a.R = R; a.C = mlp_cout[l];
+      if (eval) {
+        const int coff[3] = {0, 128, 256};
+        a.ecoef = ecoef + coff[l];
+        a.rmean = run + flow_eval_run_offset(3 + l);
+        a.rvar = a.rmean + mlp_cout[l];
+        a.fma_form = 1;
+      }
       return a;
     };
     // the mask of layer l is the one its consumer applied: the head for layer 2, the contraction of layer l + 1
     auto consumer_fma = [&](int l) {
-      if (l == 2) return 0;
+      if (l == 2 || eval) return 0;  // eval: the fused kernel's fma form (mlp_coef)
       GemmArgs g{};
       g.x = hs[l]; g.ldx = mlp_cout[l]; g.w = wts->mlp_w[l + 1]; g.y = (float*)hs[l + 1]; g.ldy = mlp_cout[l + 1];
       g.groups = 1; g.rows_per_group = R; g.cin = mlp_cin[l + 1]; g.cout = mlp_cout[l + 1];
@@ -477,7 +587,11 @@ extern "C" int pmvs_point_flow_backward(const pmvs_flow_shape* shape, const pmvs
     float* dh = F(p.dh);
     for (int l = 2; l >= 0; --l) {
       const MlpBn a = bn(l, consumer_fma(l));
-      PMVS_TRY(mlp_layer_backward(a, dA, dh, part, mcoef, grads->mlp_dgamma[l], grads->mlp_dbeta[l], p.mlp_ctas, st));
+      if (eval)
+        PMVS_TRY(mlp_layer_backward_eval(a, dA, dh, part, mcoef, grads->mlp_dgamma[l], grads->mlp_dbeta[l], p.mlp_ctas,
+                                         st));
+      else
+        PMVS_TRY(mlp_layer_backward(a, dA, dh, part, mcoef, grads->mlp_dgamma[l], grads->mlp_dbeta[l], p.mlp_ctas, st));
       const float* x = ecat;
       if (l > 0) {
         PMVS_TRY(mlp_act(bn(l - 1, consumer_fma(l - 1)), F(p.act), st));
@@ -515,10 +629,17 @@ extern "C" int pmvs_point_flow_backward(const pmvs_flow_shape* shape, const pmvs
   {
     const int in_off[3] = {0, 0, 32}, out_off[3] = {0, 32, 96};
     double* st4 = (double*)(ws + p.st4);
+    if (eval) {  // the three layers' sums from the kept running statistics
+      prof_begin("flow_bwd_run_sums", st);
+      ec_run_sums_kernel<<<3, 128, 0, st>>>(run, st4, (double)R);
+      PMVS_TRY(check_launch("ec_run_sums_kernel", st));
+    }
     for (int l = 2; l >= 0; --l) {
       const int c = ec_cout[l];
       double* s4 = st4 + (size_t)l * 4 * 64;
-      if (gather) {
+      if (eval) {
+        // s4 holds ec_run_sums_kernel's sums
+      } else if (gather) {
         if (cudaMemcpyAsync(s4, stats + st_ec[l], 4 * c * sizeof(double), cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
           set_error("point_flow_backward: copy failed");
           return PMVS_ERR_CUDA;
@@ -546,7 +667,7 @@ extern "C" int pmvs_point_flow_backward(const pmvs_flow_shape* shape, const pmvs
       EdgeLayerBwd L{};
       L.x = x; L.ldx = ldx; L.idx32 = (const int32_t*)(ws + p.idx32); L.inv_off = inv_off; L.inv_list = inv_list;
       L.w12 = wts->ec_w12[l]; L.gamma = wts->ec_gamma[l]; L.beta = wts->ec_beta[l]; L.eps = eps;
-      L.concat_central = l > 0; L.bn_train = 1; L.le = le; L.stats = s4;
+      L.concat_central = l > 0; L.bn_train = eval ? 0 : 1; L.le = le; L.stats = s4;
       L.tile_coef = gather ? nullptr : fcoef + (size_t)l * 6 * 64;
       L.dy = F(p.decat) + out_off[l]; L.lddy = 224;
       L.dx = l > 0 ? F(p.dtmp) : (need_fetch ? F(p.df0) : nullptr);
@@ -587,4 +708,43 @@ extern "C" int pmvs_point_flow_backward(const pmvs_flow_shape* shape, const pmvs
                                          w, st));
   }
   return PMVS_OK;
+}
+
+}  // namespace
+
+}  // namespace pmvs
+
+using namespace pmvs;
+
+extern "C" size_t pmvs_point_flow_backward_workspace_bytes(const pmvs_flow_shape* shape) {
+  BwdFlowPlan p;
+  if (bwd_flow_plan(shape, p, false) != PMVS_OK) return 0;
+  return p.total;
+}
+
+extern "C" int pmvs_point_flow_backward(const pmvs_flow_shape* shape, const pmvs_flow_weights* wts,
+                                        const float* const pyramids_cl[3], const float* depth_prev,
+                                        const float* cam_params, const float* interval, const float* mean,
+                                        const float* stdv, const void* fwd_workspace, const float* grad_depth_out,
+                                        const float* grad_prob_out, const pmvs_flow_grads* grads, void* workspace,
+                                        size_t workspace_bytes, pmvs_stream_t stream) {
+  return point_flow_backward(shape, wts, pyramids_cl, depth_prev, cam_params, interval, mean, stdv, fwd_workspace,
+                             grad_depth_out, grad_prob_out, grads, workspace, workspace_bytes, stream, false);
+}
+
+extern "C" size_t pmvs_point_flow_eval_backward_workspace_bytes(const pmvs_flow_shape* shape) {
+  BwdFlowPlan p;
+  if (bwd_flow_plan(shape, p, true) != PMVS_OK) return 0;
+  return p.total;
+}
+
+extern "C" int pmvs_point_flow_eval_backward(const pmvs_flow_shape* shape, const pmvs_flow_weights* wts,
+                                             const float* const pyramids_cl[3], const float* depth_prev,
+                                             const float* cam_params, const float* interval, const float* mean,
+                                             const float* stdv, const void* fwd_workspace,
+                                             const float* grad_depth_out, const float* grad_prob_out,
+                                             const pmvs_flow_grads* grads, void* workspace, size_t workspace_bytes,
+                                             pmvs_stream_t stream) {
+  return point_flow_backward(shape, wts, pyramids_cl, depth_prev, cam_params, interval, mean, stdv, fwd_workspace,
+                             grad_depth_out, grad_prob_out, grads, workspace, workspace_bytes, stream, true);
 }

@@ -21,6 +21,9 @@
 // After the fifth block the warpgroup holds all five hypotheses of its 64 pixels and finishes them with the flow
 // head's own code (flow_head_store).  Every product is 3xTF32 (hi * hi + hi * lo + lo * hi), as in the
 // batch-statistics path.
+// The KEEP variant (pmvs_point_flow_eval_keep) also stores each block's accumulators h0, h1, h2 (pre-BatchNorm, the
+// values the fma above reads) and the raw outputs for the backward; its arithmetic is the same instruction for
+// instruction, so depth and prob are the same bits.
 // Shared memory: the hi / lo planes of the three weight matrices (152 KB), a 4-stage ring of 8 KB boxes per
 // warpgroup, the coefficient tables and the barriers.
 #include <algorithm>
@@ -105,6 +108,27 @@ __device__ __forceinline__ void bn_relu_fragments(const float* acc, int half, co
   }
 }
 
+// KEEP: columns [0, 8 NB) of the accumulator of this thread's rows r, r + 8 (the values bn_relu_fragments reads) ->
+// rows row0 + r, row0 + r + 8 of h [., 8 NB], rows at or past `valid` skipped
+template <int NB, bool STACKED>
+__device__ __forceinline__ void keep_acc(const float* acc, float* __restrict__ h, long long row0, int r, int q,
+                                         int valid) {
+#pragma unroll
+  for (int half = 0; half < 2; ++half) {
+    const int rr = r + 8 * half;
+    if (rr >= valid) continue;
+    float* dst = h + (size_t)(row0 + rr) * (8 * NB) + 2 * q;
+#pragma unroll
+    for (int i = 0; i < NB; ++i) {
+      const int e = 2 * half;
+      const float y0 = STACKED ? acc[4 * i + e] + acc[4 * NB + 4 * i + e] : acc[4 * i + e];
+      const float y1 = STACKED ? acc[4 * i + e + 1] + acc[4 * NB + 4 * i + e + 1] : acc[4 * i + e + 1];
+      *reinterpret_cast<float2*>(dst + 8 * i) = make_float2(y0, y1);
+    }
+  }
+}
+
+template <bool KEEP>
 __global__ void __launch_bounds__(FE_THREADS, 1) flow_mlp_head_eval_kernel(const __grid_constant__ CUtensorMap tm,
                                                                            const FlowEvalArgs a) {
   extern __shared__ __align__(1024) unsigned char smem[];
@@ -176,8 +200,10 @@ __global__ void __launch_bounds__(FE_THREADS, 1) flow_mlp_head_eval_kernel(const
   for (int u = u_lo + wgi; u < u_hi; u += 2) {
     const int cloud = u / upc, pix0 = (u - cloud * upc) * FE_NT;
     float raw[PMVS_NUM_HYP];  // lane q = 0: row r, q = 1: row r + 8 (the lane that finishes it)
+    const int valid = P - pix0;  // rows of the block inside the cloud
 #pragma unroll 1
     for (int m = 0; m < PMVS_NUM_HYP; ++m) {
+      const long long row0 = (long long)cloud * PMVS_NUM_HYP * P + (long long)m * P + pix0;
       // h0 = ecat * W0^T
       float acc0[64];
       {
@@ -193,6 +219,7 @@ __global__ void __launch_bounds__(FE_THREADS, 1) flow_mlp_head_eval_kernel(const
         }
       }
       fence_regs(acc0);
+      if constexpr (KEEP) keep_acc<8, true>(acc0, a.keep_h[0], row0, r, q, valid);
       // Layers 1 and 2 accumulate the three products in one accumulator (small terms first), not stacked as layer 0:
       // with the A operand in registers stacking saves no shared-memory reads, and it would cost 40 registers.  They
       // run one 32-column K chunk at a time, so that the fragments of only one chunk are live.
@@ -216,6 +243,7 @@ __global__ void __launch_bounds__(FE_THREADS, 1) flow_mlp_head_eval_kernel(const
         fence_regs(fl);
       }
       fence_regs(acc1);
+      if constexpr (KEEP) keep_acc<8, false>(acc1, a.keep_h[1], row0, r, q, valid);
       // h2 = relu(BN(h1)) * W2^T
       float acc2[8];
 #pragma unroll
@@ -235,6 +263,7 @@ __global__ void __launch_bounds__(FE_THREADS, 1) flow_mlp_head_eval_kernel(const
         fence_regs(fl);
       }
       fence_regs(acc2);
+      if constexpr (KEEP) keep_acc<2, false>(acc2, a.keep_h[2], row0, r, q, valid);
       // raw = relu(BN(h2)) * w3^T: this thread's 4 columns, then the 4 lanes of the row
       float s0 = 0.f, s1 = 0.f;
 #pragma unroll
@@ -257,12 +286,18 @@ __global__ void __launch_bounds__(FE_THREADS, 1) flow_mlp_head_eval_kernel(const
     }
     // lane q = 0 finishes row r, lane q = 1 row r + 8
     const int pp = pix0 + r + 8 * q;
-    if (q < 2 && pp < P) flow_head_store(h, raw, cloud / h.B, cloud % h.B, pp);
+    if (q < 2 && pp < P) {
+      flow_head_store(h, raw, cloud / h.B, cloud % h.B, pp);
+      if constexpr (KEEP) {
+#pragma unroll
+        for (int m = 0; m < PMVS_NUM_HYP; ++m) a.keep_raw[(size_t)cloud * PMVS_NUM_HYP * P + (size_t)m * P + pp] = raw[m];
+      }
+    }
   }
 }
 
 __global__ void flow_eval_coef_kernel(const pmvs_flow_weights w, int S, float* __restrict__ ec_coef,
-                                      float* __restrict__ mlp_coef) {
+                                      float* __restrict__ mlp_coef, float* __restrict__ run_copy) {
   const int g = blockIdx.x;
   const float eps = w.eps;
   auto istd = [&](float rv) { return (float)(1.0 / sqrt((double)rv + (double)eps)); };
@@ -298,19 +333,31 @@ __global__ void flow_eval_coef_kernel(const pmvs_flow_weights w, int S, float* _
       }
       t += 2 * C;
     }
+    if (run_copy != nullptr)
+      for (int l = 0; l < 6; ++l) {
+        const int C = flow_eval_run_channels(l);
+        const float* rm = l < 3 ? w.ec_run_mean[l] : w.mlp_run_mean[l - 3];
+        const float* rv = l < 3 ? w.ec_run_var[l] : w.mlp_run_var[l - 3];
+        float* o = run_copy + flow_eval_run_offset(l);
+        for (int c = threadIdx.x; c < C; c += blockDim.x) {
+          o[c] = rm[c];
+          o[C + c] = rv[c];
+        }
+      }
   }
 }
 
 }  // namespace
 
-int launch_flow_eval_coef(const pmvs_flow_weights& w, int S, float* ec_coef, float* mlp_coef, cudaStream_t st) {
+int launch_flow_eval_coef(const pmvs_flow_weights& w, int S, float* ec_coef, float* mlp_coef, float* run_copy,
+                          cudaStream_t st) {
   for (int l = 0; l < 3; ++l)
     PMVS_REQUIRE(w.ec_run_mean[l] && w.ec_run_var[l] && w.mlp_run_mean[l] && w.mlp_run_var[l] && w.ec_gamma[l] &&
                      w.ec_beta[l] && w.mlp_gamma[l] && w.mlp_beta[l],
                  "point_flow: bn_eval = 1 needs the running mean and variance of all six BatchNorm layers");
   PMVS_REQUIRE(S > 0 && S <= 65535 && ec_coef && mlp_coef, "flow_eval_coef: bad arguments");
   prof_begin("flow_eval_coef", st);
-  flow_eval_coef_kernel<<<S, 64, 0, st>>>(w, S, ec_coef, mlp_coef);
+  flow_eval_coef_kernel<<<S, 64, 0, st>>>(w, S, ec_coef, mlp_coef, run_copy);
   return check_launch("flow_eval_coef_kernel", st);
 }
 
@@ -319,6 +366,11 @@ int launch_flow_mlp_head_eval(const FlowEvalArgs& a, cudaStream_t st) {
   PMVS_REQUIRE(a.ecat && a.w[0] && a.w[1] && a.w[2] && a.mlp_coef && h.w3 && h.depth_prev && h.interval && h.depth_out,
                "flow_mlp_head_eval: NULL pointer");
   PMVS_REQUIRE(((uintptr_t)a.ecat & 15) == 0, "flow_mlp_head_eval: ecat must be 16-byte aligned");
+  // the KEEP variant writes all four; a partial set is a caller error, not a silent plain launch
+  const int kept = (a.keep_h[0] != nullptr) + (a.keep_h[1] != nullptr) + (a.keep_h[2] != nullptr) +
+                   (a.keep_raw != nullptr);
+  PMVS_REQUIRE(kept == 0 || kept == 4, "flow_mlp_head_eval: keep_h[0..2] and keep_raw must all be set or all be NULL");
+  const bool keep = kept == 4;
   PMVS_REQUIRE(h.B > 0 && h.S > 0 && h.ratio > 0 && h.h % h.ratio == 0 && h.w % h.ratio == 0,
                "flow_mlp_head_eval: bad shape");
   const long long P = (long long)(h.h / h.ratio) * (h.w / h.ratio);
@@ -344,11 +396,18 @@ int launch_flow_mlp_head_eval(const FlowEvalArgs& a, cudaStream_t st) {
     set_error("flow_mlp_head_eval: cuTensorMapEncodeTiled failed (%d) for %lld pixels", (int)rc, P);
     return PMVS_ERR_CUDA;
   }
-  static unsigned long long smem_done = 0;
-  PMVS_TRY(ensure_dyn_smem(flow_mlp_head_eval_kernel, FE_SMEM, smem_done, "flow_mlp_head_eval"));
   const int grid = (int)std::min<long long>(units, sm_count());
+  if (keep) {
+    static unsigned long long smem_keep = 0;
+    PMVS_TRY(ensure_dyn_smem(flow_mlp_head_eval_kernel<true>, FE_SMEM, smem_keep, "flow_mlp_head_eval_keep"));
+    prof_begin("flow_mlp_head_eval_keep", st);
+    flow_mlp_head_eval_kernel<true><<<grid, FE_THREADS, FE_SMEM, st>>>(tm, a);
+    return check_launch("flow_mlp_head_eval_kernel<KEEP>", st);
+  }
+  static unsigned long long smem_done = 0;
+  PMVS_TRY(ensure_dyn_smem(flow_mlp_head_eval_kernel<false>, FE_SMEM, smem_done, "flow_mlp_head_eval"));
   prof_begin("flow_mlp_head_eval", st);
-  flow_mlp_head_eval_kernel<<<grid, FE_THREADS, FE_SMEM, st>>>(tm, a);
+  flow_mlp_head_eval_kernel<false><<<grid, FE_THREADS, FE_SMEM, st>>>(tm, a);
   return check_launch("flow_mlp_head_eval_kernel", st);
 }
 

@@ -53,8 +53,10 @@ class PointMVSNet(nn.Module):
     The state dict has the reference's 223 entries.  The ``PointFlow`` that runs the refinement shares
     ``flow_edge_conv`` and ``flow_mlp`` and is deliberately not a sub-module (it would add ``point_flow.*`` keys).
     In ``train()`` mode (test.py:58 keeps the model there) BatchNorm uses batch statistics; in ``eval()`` every stage
-    uses the running statistics, under ``torch.no_grad()`` (a grad-enabled ``eval()`` forward raises
-    ``NotImplementedError`` in the flow stage)."""
+    uses the running statistics.  A grad-enabled forward in ``eval()``, or with every BatchNorm frozen in eval mode
+    (``freeze_by_patterns(net, ("module:bn",))``), trains on the running statistics, which it leaves untouched, once
+    ``networks.enable_flow_eval_backward()`` is on besides the three training switches; without it such a forward
+    raises ``NotImplementedError`` before any launch."""
 
     def __init__(self, img_base_channels=8, vol_base_channels=8, flow_channels=(64, 64, 16, 1), k=16):
         super().__init__()
@@ -86,6 +88,11 @@ class PointMVSNet(nn.Module):
                     "PointMVSNet: a grad-enabled forward needs the three training switches %s; call "
                     "pointmvsnet_b200.model.enable_training() (build_pointmvsnet does), or run under torch.no_grad()"
                     % ", ".join(_SWITCHES))
+            if (not networks.flow_eval_backward_enabled() and
+                    not all(bn.training for bn in self._point_flow._bn_modules())):
+                raise NotImplementedError(
+                    "PointMVSNet: a grad-enabled forward with the flow stage's BatchNorm in eval mode needs "
+                    "pointmvsnet_b200.networks.enable_flow_eval_backward(); or run under torch.no_grad()")
         if img_list.dim() != 5 or cams.dim() != 5 or tuple(cams.shape[2:]) != (2, 4, 4):
             raise RuntimeError("PointMVSNet: img_list must be [B,V,3,H,W] and cam_params_list [B,V,2,4,4], got %s "
                                "and %s" % (tuple(img_list.shape), tuple(cams.shape)))

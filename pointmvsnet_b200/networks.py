@@ -18,8 +18,8 @@ from .nn.conv import Conv2d, Conv3d, Deconv3d
 
 _SUPPORTED_COUT = (16, 32, 64, 128)
 # the process-wide training switches: "edge" (EdgeConv, EdgeConvNoC, PointFlow), "volume" (VolumeConv, coarse_depth)
-# and "image" (ImageConv.forward_views)
-_backward = {"edge": False, "volume": False, "image": False}
+# and "image" (ImageConv.forward_views), and "flow_eval" (PointFlow's backward with running-statistics BatchNorm)
+_backward = {"edge": False, "volume": False, "image": False, "flow_eval": False}
 
 
 def _enable(which, enabled):
@@ -44,6 +44,23 @@ def enable_backward(enabled=True):
 
 def backward_enabled():
     return _backward["edge"]
+
+
+def enable_flow_eval_backward(enabled=True):
+    """Process-wide switch for fine-tuning with frozen BatchNorm: while on (together with ``enable_backward()``), a
+    grad-enabled ``PointFlow`` call whose six BatchNorm layers are in eval mode (``.eval()``, or frozen by
+    ``freeze_by_patterns(net, ("module:bn",))``) runs on the running statistics through an autograd Function whose
+    backward is ``pmvs_point_flow_eval_backward``; the running statistics are read and never updated.  While off (the
+    default) such a call raises ``NotImplementedError``.  Returns the previous setting.
+
+    It is opt-in for the same reason as ``enable_backward()``: the forward keeps its workspace until backward runs,
+    which in eval mode also holds flow_mlp's activations (``pmvs_point_flow_eval_keep_workspace_bytes``, about 580
+    bytes per point more than an inference call)."""
+    return _enable("flow_eval", enabled)
+
+
+def flow_eval_backward_enabled():
+    return _backward["flow_eval"]
 
 
 def enable_volume_backward(enabled=True):

@@ -2,9 +2,12 @@
 as an nn.Module, executed by libpmvs_b200.so.
 
 Inference runs as test.py runs it: under torch.no_grad() with the module in train() mode so that BatchNorm uses batch
-statistics.  Under .eval() (all six BatchNorm layers in eval mode) a call that needs no gradient uses the running
-statistics instead, as the reference's model.eval() does; that mode has no backward.  Training (the train branch, one cloud per call) runs through an autograd Function whose backward is
-``pmvs_point_flow_backward`` once ``networks.enable_backward()`` is on; without it a grad-enabled call raises.
+statistics.  Under .eval() (all six BatchNorm layers in eval mode) the running statistics are used instead, as the
+reference's model.eval() does.  Training (the train branch, one cloud per call) runs through an autograd Function
+whose backward is ``pmvs_point_flow_backward`` once ``networks.enable_backward()`` is on; without it a grad-enabled
+call raises.  Training with the BatchNorm layers in eval mode (fine-tuning with frozen BatchNorm) also needs
+``networks.enable_flow_eval_backward()``; its forward is ``pmvs_point_flow_eval_keep`` and its backward
+``pmvs_point_flow_eval_backward``.
 
 One call = one refinement iteration = ~16 kernel launches enqueued by a single C-ABI
 call (``pmvs_point_flow_iter``); ``PointFlowPass`` runs the reference's iteration loop
@@ -174,9 +177,11 @@ class PointFlow(nn.Module):
         bns = self._bn_modules()
         if all(bn.training for bn in bns):
             return False
-        if needs_grad:
-            raise NotImplementedError("PointFlow: BatchNorm in eval mode (running statistics) has no backward on the "
-                                      "fused path; wrap the call in torch.no_grad(), or call .train() on the module")
+        if needs_grad and not (networks.flow_eval_backward_enabled() and networks.backward_enabled()):
+            raise NotImplementedError("PointFlow: a grad-enabled call with BatchNorm in eval mode (running statistics) "
+                                      "needs pointmvsnet_b200.networks.enable_flow_eval_backward() and "
+                                      "enable_backward(); or wrap the call in torch.no_grad(), or call .train() on "
+                                      "the module")
         if any(bn.training for bn in bns):
             raise RuntimeError("PointFlow: the six BatchNorm layers must all be in train mode or all in eval mode, got "
                                "%s" % ["train" if bn.training else "eval" for bn in bns])
@@ -231,8 +236,10 @@ class PointFlow(nn.Module):
 
         BatchNorm follows the six BatchNorm modules: in train mode (the reference's test.py:58) batch statistics per
         sub-cloud, and the running statistics are updated; in eval mode (``.eval()``) the running statistics, which
-        are then only read.  Eval mode serves calls that need no gradient (under torch.no_grad(), or with nothing
-        requiring grad); a grad-needing call raises NotImplementedError, a mix of modes RuntimeError."""
+        are then only read.  A grad-needing eval-mode call (fine-tuning with frozen BatchNorm) needs both
+        ``networks.enable_backward()`` and ``networks.enable_flow_eval_backward()``, and raises NotImplementedError
+        without them; its backward fills the same gradients as in train mode, BatchNorm differentiated as the affine
+        map of the running statistics, which it leaves untouched.  A mix of modes raises RuntimeError."""
         require_cuda(estimated_depth_map, interval, cam_params_list, mean, std)
         given = pyramids_channels_last if pyramids_channels_last is not None else (
             [feature_pyramids[k] for k in PYR_KEYS] if isinstance(feature_pyramids, dict) else list(feature_pyramids))
@@ -278,7 +285,8 @@ class PointFlow(nn.Module):
         if grad_call:
             params = self._grad_params()
             return _PointFlowFn.apply(self, (interval, image_scale, cam_params_list, mean, std, is_test, img_hw,
-                                             interval_scale), estimated_depth_map, pyr[0], pyr[1], pyr[2], *params)
+                                             interval_scale, bn_eval), estimated_depth_map, pyr[0], pyr[1], pyr[2],
+                                      *params)
         return self._run(estimated_depth_map, interval, image_scale, cam_params_list, mean, std, is_test, img_hw,
                          pyr, out, interval_scale, sub_range, None, bn_eval)
 
@@ -295,7 +303,9 @@ class PointFlow(nn.Module):
     def _run(self, estimated_depth_map, interval, image_scale, cam_params_list, mean, std, is_test, img_hw, pyr, out,
              interval_scale, sub_range, ctx, bn_eval=False):
         """The forward launches.  ctx None: the module's shared workspace; else (an autograd context) a workspace of
-        the call's own, kept with what the backward reads.  bn_eval: BatchNorm from the running statistics."""
+        the call's own, kept with what the backward reads (with bn_eval, pmvs_point_flow_eval_keep's, which also
+        holds flow_mlp's activations and a copy of the running statistics).  bn_eval: BatchNorm from the running
+        statistics."""
         dev = estimated_depth_map.device
         B, V = cam_params_list.shape[:2]
         pyr_hw = [(int(t.shape[2]), int(t.shape[3])) for t in pyr]
@@ -309,7 +319,8 @@ class PointFlow(nn.Module):
         if ctx is None:
             ws, need = self._workspace(shape, dev)
         else:
-            need = lib.pmvs_point_flow_workspace_bytes(C.byref(shape))
+            size = lib.pmvs_point_flow_eval_keep_workspace_bytes if bn_eval else lib.pmvs_point_flow_workspace_bytes
+            need = size(C.byref(shape))
             ws = _lib.workspace(need, dev)
         w, keep = self._weights(dev)
         track = self.update_running_stats and not bn_eval  # the six BatchNorm layers are in train mode
@@ -335,10 +346,10 @@ class PointFlow(nn.Module):
         itv = _lib.f32c(interval.detach().reshape(-1))
         mean_c, std_c = _lib.f32c(mean.detach()), _lib.f32c(std.detach())
         pyr_ptrs = (C.c_void_p * 3)(*[t.data_ptr() for t in pyr])
+        run = lib.pmvs_point_flow_eval_keep if ctx is not None and bn_eval else lib.pmvs_point_flow_iter
         with torch.cuda.device(dev):
-            check(lib.pmvs_point_flow_iter(C.byref(shape), C.byref(w), C.byref(pyr_ptrs), ptr(depth), ptr(cams),
-                                           ptr(itv), ptr(mean_c), ptr(std_c), ptr(depth_out), ptr(prob_out),
-                                           ptr(ws), need, stream_ptr()))
+            check(run(C.byref(shape), C.byref(w), C.byref(pyr_ptrs), ptr(depth), ptr(cams), ptr(itv), ptr(mean_c),
+                      ptr(std_c), ptr(depth_out), ptr(prob_out), ptr(ws), need, stream_ptr()))
         self._last = (shape, ws, depth)  # debug_stages() recomputes the point features from `depth`
         if ctx is not None:
             ctx.fwd_tensors = (depth, pyr[0], pyr[1], pyr[2], cams, itv, mean_c, std_c, ws)
@@ -534,10 +545,11 @@ class _PointFlowFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, mod, args, depth, pyr0, pyr1, pyr2, *params):
-        interval, image_scale, cams, mean, std, is_test, img_hw, interval_scale = args
+        interval, image_scale, cams, mean, std, is_test, img_hw, interval_scale, bn_eval = args
         ctx.dtypes = (depth.dtype,) + tuple(p.dtype for p in params)
+        ctx.bn_eval = bn_eval
         res = mod._run(depth, interval, image_scale, cams, mean, std, is_test, img_hw, [pyr0, pyr1, pyr2], None,
-                       interval_scale, None, ctx)
+                       interval_scale, None, ctx, bn_eval)
         # the parameters too: an in-place update before backward is then autograd's version error
         ctx.save_for_backward(*ctx.fwd_tensors, *params)
         del ctx.fwd_tensors
@@ -580,13 +592,16 @@ class _PointFlowFn(torch.autograd.Function):
         gr.ddepth_prev = ptr(ddepth)
         gd = _lib.f32c(g_depth) if g_depth is not None else torch.zeros(B, 1, shape.flow_h, shape.flow_w, device=dev)
         gp = _lib.f32c(g_prob) if g_prob is not None else None
-        nbytes = lib.pmvs_point_flow_backward_workspace_bytes(C.byref(shape))
+        if ctx.bn_eval:
+            size, bwd = lib.pmvs_point_flow_eval_backward_workspace_bytes, lib.pmvs_point_flow_eval_backward
+        else:
+            size, bwd = lib.pmvs_point_flow_backward_workspace_bytes, lib.pmvs_point_flow_backward
+        nbytes = size(C.byref(shape))
         bws = _lib.workspace(nbytes, dev)
         pyr_ptrs = (C.c_void_p * 3)(p0.data_ptr(), p1.data_ptr(), p2.data_ptr())
         with torch.cuda.device(dev):
-            check(lib.pmvs_point_flow_backward(C.byref(shape), C.byref(w), C.byref(pyr_ptrs), ptr(depth), ptr(cams),
-                                               ptr(itv), ptr(mean_c), ptr(std_c), ptr(ws), ptr(gd), ptr(gp),
-                                               C.byref(gr), ptr(bws), nbytes, stream_ptr()))
+            check(bwd(C.byref(shape), C.byref(w), C.byref(pyr_ptrs), ptr(depth), ptr(cams), ptr(itv), ptr(mean_c),
+                      ptr(std_c), ptr(ws), ptr(gd), ptr(gp), C.byref(gr), ptr(bws), nbytes, stream_ptr()))
         out = []
         for l in range(3):
             c = ps[4 * l].shape[0]
