@@ -641,6 +641,25 @@ int pmvs_depth_loss_backward(const pmvs_depth_terms* terms, const float* gt, int
                              int V, const double* stats, const float* grad_loss, float* const grad_pred[3],
                              pmvs_stream_t stream);
 
+/* ---- input side: resize, crop and normalise every view of a batch (DESIGN 3.19) ---------------------------------- */
+/* bytes of device workspace pmvs_prepare_views needs (the exact per-view sums, 48 N bytes rounded up to 256); 0 (with
+ * pmvs_last_error) for arguments pmvs_prepare_views rejects. */
+size_t pmvs_prepare_views_workspace_bytes(int N, int V, int H0, int W0, double scale, int crop_y, int crop_x, int H,
+                                          int W);
+/* src [N, H0, W0, 3] uint8 (N = B V views, as cv2.imread returns them, BGR kept) -> img_out [N, 3, H, W] float32.
+ * Each view is resized by `scale` (0 < scale <= 1) to round(H0 scale) x round(W0 scale) (half to even) with OpenCV's
+ * 8-bit bilinear rule, bit for bit with cv2.resize(view, None, fx=scale, fy=scale, interpolation=INTER_LINEAR)
+ * (which copies the view when that size is H0 x W0),
+ * cropped to H x W at (crop_y, crop_x) of the resized frame (the uncropped image is never written), and normalised
+ * per (view, channel): (x - mean) / (sqrt(var) + 1e-7) in IEEE float32, where mean and the population variance are
+ * the exact statistics of the cropped uint8 values, each correctly rounded to float32.  ref_out (NULL: not written)
+ * [N / V, H, W, 3] uint8 receives the crop of view 0 of each group of V views.  Rejected (PMVS_ERR_ARG): N < 1 or
+ * > 65535, N not a multiple of V, scale outside (0, 1], a crop outside the resized view, H0 W0 or H W >= 2^31.  Two
+ * launches and one memset on `stream`; no floating-point atomics, so two calls give the same bits. */
+int pmvs_prepare_views(const unsigned char* src, int N, int V, int H0, int W0, double scale, int crop_y, int crop_x,
+                       int H, int W, float* img_out, unsigned char* ref_out, void* workspace, size_t workspace_bytes,
+                       pmvs_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -10,13 +10,14 @@ Mirrors the reference's import surface (pointmvsnet/model.py:8-12):
     pointmvsnet_b200.utils.io / utils.eval_file_logger   PFM / camera files, per-view outputs (test.py:76)
 plus the new ``PointFlow`` module that replaces the ``point_flow`` closure
 (pointmvsnet/model.py:150-295), and ``pointmvsnet_b200.model``, the whole model with its loss and metrics
-(pointmvsnet/model.py:15-438).  ``install_as_pointmvsnet()`` aliases these modules
+(pointmvsnet/model.py:15-438), and ``pointmvsnet_b200.dataset``, the DTU loaders with the pixel work on the device
+(pointmvsnet/dataset.py).  ``install_as_pointmvsnet()`` aliases these modules
 under the reference's own names so an unchanged ``pointmvsnet/model.py`` imports them.
 """
 __version__ = "0.1.0"
 
 
-def install_as_pointmvsnet(reference_root=None, model=False):
+def install_as_pointmvsnet(reference_root=None, model=False, dataset=False):
     """Make ``import pointmvsnet.<hot-path module>`` resolve to this package.
 
     With ``reference_root`` (a checkout of callmeray/PointMVSNet) the rest of the
@@ -26,7 +27,9 @@ def install_as_pointmvsnet(reference_root=None, model=False):
     this package mirrors is aliased (enough for ``from pointmvsnet.utils.torch_utils
     import get_knn_3d`` style imports).  With ``model=True`` ``pointmvsnet.model`` is aliased to
     ``pointmvsnet_b200.model`` as well, so an unchanged train.py / test.py builds the whole model on the library
-    (``from pointmvsnet.model import build_pointmvsnet``).  See INTEGRATION.md."""
+    (``from pointmvsnet.model import build_pointmvsnet``).  With ``dataset=True`` ``pointmvsnet.dataset`` and
+    ``pointmvsnet.utils.preprocess`` are aliased to ``pointmvsnet_b200.dataset`` / ``pointmvsnet_b200.utils.preprocess``,
+    so ``build_data_loader`` yields batches prepared on the device.  See INTEGRATION.md."""
     import importlib
     import sys
     import types
@@ -41,6 +44,9 @@ def install_as_pointmvsnet(reference_root=None, model=False):
     }
     if model:
         hot["pointmvsnet.model"] = "pointmvsnet_b200.model"
+    if dataset:
+        hot["pointmvsnet.dataset"] = "pointmvsnet_b200.dataset"
+        hot["pointmvsnet.utils.preprocess"] = "pointmvsnet_b200.utils.preprocess"
     extra = {
         "pointmvsnet.functions.functions": "pointmvsnet_b200.functions.functions",
         "pointmvsnet.networks": "pointmvsnet_b200.networks",

@@ -150,6 +150,8 @@ _sig("pmvs_point_flow_eval_backward", I, [C.POINTER(FlowShape), C.POINTER(FlowWe
                                           P, P, P, P, P, P, P, P, C.POINTER(FlowGrads), P, C.c_size_t, P])
 _sig("pmvs_depth_loss", I, [C.POINTER(DepthTerms), P, I, I, P, I, I, F, P, P, P, P])
 _sig("pmvs_depth_loss_backward", I, [C.POINTER(DepthTerms), P, I, I, P, I, I, P, P, C.POINTER(C.c_void_p * 3), P])
+_sig("pmvs_prepare_views_workspace_bytes", C.c_size_t, [I, I, I, I, C.c_double, I, I, I, I])
+_sig("pmvs_prepare_views", I, [P, I, I, I, I, C.c_double, I, I, I, I, P, P, P, C.c_size_t, P])
 
 EXPORTED = [
     "pmvs_version", "pmvs_last_error", "pmvs_launch_count", "pmvs_set_option", "pmvs_get_option", "pmvs_profile_enable", "pmvs_profile_collect", "pmvs_set_gemm_mode", "pmvs_get_gemm_mode", "pmvs_gather_knn_forward",
@@ -167,6 +169,7 @@ EXPORTED = [
     "pmvs_point_flow_debug_feature", "pmvs_point_flow_backward_workspace_bytes", "pmvs_point_flow_backward",
     "pmvs_depth_loss", "pmvs_depth_loss_backward", "pmvs_point_flow_eval_keep_workspace_bytes",
     "pmvs_point_flow_eval_keep", "pmvs_point_flow_eval_backward_workspace_bytes", "pmvs_point_flow_eval_backward",
+    "pmvs_prepare_views_workspace_bytes", "pmvs_prepare_views",
 ]
 
 
