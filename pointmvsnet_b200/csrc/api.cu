@@ -132,29 +132,12 @@ __global__ void __launch_bounds__(256)
 // ---------------------------------------------------------------------------------------
 // PointFlow iteration: workspace plan
 // ---------------------------------------------------------------------------------------
-struct FlowPlan {
-  int S, hs, ws, N;  // S = sub-clouds PROCESSED by this call (all ratio^2 unless sharded)
-  int sub_begin;
-  size_t R;  // rows = S * B * N
-  size_t cam, feature, xyz, idx, le, ecat, h0, h1, h2, stats, total;
-  size_t warp_src;     // the pyramid levels resized to the flow grid, [B,V,h,w,112]
-  size_t cand;         // [R, 16] uint16: kNN neighbour codes for the tile EdgeConv kernels
-  // offsets (in doubles) inside the stats region.  Per EdgeConv layer and group 6*cout doubles: st_ec = 4*cout
-  // (gather path: [sum_c | sumsq_c | sum_n | sumsq_n]; tile path: column sums / sums of squares of the
-  // 2*cout GEMM outputs), st_ecn = 2*cout ([sum_n | sumsq_n] of the tile path)
-  size_t st_ec[3], st_ecn[3], st_mlp[3];
-  size_t st_ticket;    // 3*S unsigned arrival counters of the tile statistics kernels (inside the zeroed region)
-  size_t stats_doubles;
-  size_t coef;         // [3][S][6*64] floats: per (layer, group) BatchNorm coefficients of the tile apply kernels
-  size_t mlp_coef;     // bn_eval: FLOW_EVAL_MLP_COEF floats after the tile tables (flow_mlp's BatchNorms)
-  bool eval;           // bn_eval: running statistics; no stats, h0, h1 or h2 regions (their offsets are 0)
-  // keep (pmvs_point_flow_eval_keep): h0, h1, h2 after every eval region, then the raw flow_mlp outputs [R] and the
-  // copy of the running statistics (FLOW_EVAL_RUN floats); 0 otherwise
-  size_t raw, run;
-};
-
-static int make_plan(const pmvs_flow_shape* s, FlowPlan& p, bool keep = false) {
+int flow_plan(const pmvs_flow_shape* s, FlowPlan& p, bool keep) {
   PMVS_REQUIRE(s != nullptr, "point_flow: NULL shape");
+  const int edge = opt(OPT_EDGE);
+  p.tile = edge != 0;
+  p.tile_w = edge == 2 ? 16 : 8;
+  p.write_idx32 = !p.tile || opt(OPT_DEBUG_IDX) != 0;
   PMVS_REQUIRE(s->B > 0 && s->V > 0 && s->V <= PMVS_MAX_VIEWS, "point_flow: B=%d V=%d (V <= %d)", s->B, s->V,
                PMVS_MAX_VIEWS);
   PMVS_REQUIRE(s->ratio >= 1 && s->flow_h > 0 && s->flow_w > 0, "point_flow: bad flow size / ratio");
@@ -178,8 +161,8 @@ static int make_plan(const pmvs_flow_shape* s, FlowPlan& p, bool keep = false) {
   PMVS_REQUIRE(s->bn_eval == 0 || s->bn_eval == 1, "point_flow: bn_eval must be 0 or 1, got %d", s->bn_eval);
   p.eval = s->bn_eval != 0;
   // the running-statistics path is built on the tile EdgeConv family (its apply kernel reads a coefficient table)
-  PMVS_REQUIRE(!p.eval || opt(OPT_EDGE) != 0,
-               "point_flow: bn_eval = 1 is served by the tile EdgeConv kernels only (option edge=%d)", opt(OPT_EDGE));
+  PMVS_REQUIRE(!p.eval || p.tile,
+               "point_flow: bn_eval = 1 is served by the tile EdgeConv kernels only (option edge=%d)", edge);
   size_t o = 0;
   p.cam = o; o += up256(cam_block_bytes(s->B, s->V));
   p.feature = o; o += up256(p.R * PMVS_FEAT_CH * 4);
@@ -196,20 +179,18 @@ static int make_plan(const pmvs_flow_shape* s, FlowPlan& p, bool keep = false) {
   p.warp_src = o; o += up256(warp_source_bytes(s->B, s->V, s->flow_h, s->flow_w));
   p.cand = o; o += up256(p.R * PMVS_KNN * 2);
   size_t d = 0;
-  const int ec_cout[3] = {32, 32, 64};
-  const int mlp_cout[3] = {64, 64, 16};
   for (int l = 0; l < 3; ++l) {
-    p.st_ec[l] = d; d += (size_t)p.S * 4 * ec_cout[l];
-    p.st_ecn[l] = d; d += (size_t)p.S * 2 * ec_cout[l];
+    p.st_ec[l] = d; d += (size_t)p.S * 4 * flow_ec_cout(l);
+    p.st_ecn[l] = d; d += (size_t)p.S * 2 * flow_ec_cout(l);
   }
-  for (int l = 0; l < 3; ++l) { p.st_mlp[l] = d; d += (size_t)p.S * 2 * mlp_cout[l]; }
+  for (int l = 0; l < 3; ++l) { p.st_mlp[l] = d; d += (size_t)p.S * 2 * flow_mlp_cout(l); }
   p.st_ticket = d; d += (3 * (size_t)p.S + 1) / 2 + 1;
   p.stats_doubles = d;
   p.stats = 0;
   if (!p.eval) {
     p.stats = o; o += up256(d * 8);
   }
-  p.coef = o; o += up256(3 * (size_t)p.S * 6 * 64 * sizeof(float));
+  p.coef = o; o += up256(flow_ec_coef_offset(3, p.S, 0) * sizeof(float));
   p.mlp_coef = 0;
   if (p.eval) {
     p.mlp_coef = o; o += up256(FLOW_EVAL_MLP_COEF * sizeof(float));
@@ -228,28 +209,6 @@ static int make_plan(const pmvs_flow_shape* s, FlowPlan& p, bool keep = false) {
     p.run = o; o += up256(FLOW_EVAL_RUN * sizeof(float));
   }
   p.total = o;
-  return PMVS_OK;
-}
-
-// the fetch of an iteration (rows a2-a9) over the workspace of plan p
-static FusedFetchParams fetch_params(const pmvs_flow_shape* s, const FlowPlan& p, char* ws, const float* depth_prev) {
-  FusedFetchParams f{};
-  f.src = (const float*)(ws + p.warp_src);
-  f.depth_prev = depth_prev; f.cam_blocks = (const float*)(ws + p.cam); f.feature = (float*)(ws + p.feature);
-  f.xyz = (float*)(ws + p.xyz);
-  f.B = s->B; f.V = s->V; f.h = s->flow_h; f.w = s->flow_w; f.hp = s->prev_h; f.wp = s->prev_w;
-  f.ratio = s->ratio; f.sub_begin = p.sub_begin; f.sub_count = p.S;
-  return f;
-}
-
-int flow_regions(const pmvs_flow_shape* s, FlowRegions& r, bool keep) {
-  FlowPlan p;
-  PMVS_TRY(make_plan(s, p, keep));
-  r.cam = p.cam; r.feature = p.feature; r.xyz = p.xyz; r.idx = p.idx; r.le = p.le; r.ecat = p.ecat; r.h0 = p.h0;
-  r.h1 = p.h1; r.h2 = p.h2; r.warp_src = p.warp_src; r.cand = p.cand; r.stats = p.stats; r.coef = p.coef;
-  r.mlp_coef = p.mlp_coef; r.raw = p.raw; r.run = p.run; r.total = p.total;
-  for (int l = 0; l < 3; ++l) { r.st_ec[l] = p.st_ec[l]; r.st_ecn[l] = p.st_ecn[l]; r.st_mlp[l] = p.st_mlp[l]; }
-  r.S = p.S;
   return PMVS_OK;
 }
 
@@ -378,24 +337,24 @@ extern "C" int pmvs_linear_pm(const float* x, int ldx, const float* w, float* y,
 
 extern "C" size_t pmvs_point_flow_workspace_bytes(const pmvs_flow_shape* shape) {
   FlowPlan p;
-  if (make_plan(shape, p) != PMVS_OK) return 0;
+  if (flow_plan(shape, p, false) != PMVS_OK) return 0;
   return p.total;
 }
 
 extern "C" int pmvs_point_flow_debug_offsets(const pmvs_flow_shape* shape, size_t off[10]) {
   FlowPlan p;
-  PMVS_TRY(make_plan(shape, p));
+  PMVS_TRY(flow_plan(shape, p, false));
   off[0] = p.feature; off[1] = p.xyz; off[2] = p.idx; off[3] = p.ecat; off[4] = p.h2;  // h2, stats: 0 under bn_eval
   off[5] = p.le; off[6] = p.stats; off[7] = p.total;
   off[8] = p.cand;
-  off[9] = (opt(OPT_EDGE) == 0 || opt(OPT_DEBUG_IDX) != 0) ? 1 : 0;  // 1: idx32 is materialised, 0: only cand
+  off[9] = p.write_idx32 ? 1 : 0;  // 1: idx32 is materialised, 0: only cand
   return PMVS_OK;
 }
 
 extern "C" int pmvs_point_flow_debug_feature(const pmvs_flow_shape* shape, const float* depth_prev, void* workspace,
                                              pmvs_stream_t stream) {
   FlowPlan p;
-  PMVS_TRY(make_plan(shape, p));
+  PMVS_TRY(flow_plan(shape, p, false));
   PMVS_REQUIRE(depth_prev && workspace, "point_flow_debug_feature: NULL pointer");
   return launch_fused_fetch(fetch_params(shape, p, (char*)workspace, depth_prev), (cudaStream_t)stream);
 }
@@ -406,7 +365,7 @@ static int point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flow_weights
                            const float* interval, const float* mean, const float* stdv, float* depth_out,
                            float* prob_out, void* workspace, size_t workspace_bytes, pmvs_stream_t stream, bool keep) {
   FlowPlan p;
-  PMVS_TRY(make_plan(shape, p, keep));
+  PMVS_TRY(flow_plan(shape, p, keep));
   PMVS_REQUIRE(wts && pyramids_cl && depth_prev && cam_params && interval && mean && stdv && depth_out && workspace,
                "point_flow: NULL pointer");
   PMVS_TRY(check_workspace("point_flow", workspace, workspace_bytes, p.total));
@@ -440,12 +399,11 @@ static int point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flow_weights
   float* warp_src = (float*)(ws + p.warp_src);
   PMVS_TRY(launch_warp_source(pyramids_cl, shape->pyr_h, shape->pyr_w, warp_src, B, shape->V, shape->flow_h,
                               shape->flow_w, st));
-  const int edge_impl = opt(OPT_EDGE);
   const FusedFetchParams f = fetch_params(shape, p, ws, depth_prev);
   // a2-a9 and EdgeConvNoC's contraction LE = F0 * W12^T in one launch, so that F0 never reaches memory.  Layer 0 has
   // no input BatchNorm, and the column statistics of its LE are never read (below), so nothing else needs F0.
   bool fused_le0 = false;
-  if (opt(OPT_FETCH) == 3 && opt(OPT_GEMM) == 3 && pmvs_get_gemm_mode() == 3 && edge_impl != 0) {
+  if (opt(OPT_FETCH) == 3 && opt(OPT_GEMM) == 3 && pmvs_get_gemm_mode() == 3 && p.tile) {
     const int rc = launch_fetch_gemm(f, wts->ec_w12[0], le, st);
     if (rc > 0) return rc;
     fused_le0 = rc == 0;
@@ -459,8 +417,8 @@ static int point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flow_weights
   // a10: neighbour lists.  The tile EdgeConv path consumes 16-bit neighbour codes; the int32 row indices are only
   // materialised for the gather path (or on request, for the tests)
   unsigned short* cand = (unsigned short*)(ws + p.cand);
-  if (edge_impl != 0)
-    PMVS_TRY(launch_knn3d_cand(xyz, opt(OPT_DEBUG_IDX) ? idx : nullptr, cand, S * B, PMVS_NUM_HYP, p.hs, p.ws, st));
+  if (p.tile)
+    PMVS_TRY(launch_knn3d_cand(xyz, p.write_idx32 ? idx : nullptr, cand, S * B, PMVS_NUM_HYP, p.hs, p.ws, st));
   else
     PMVS_TRY(launch_knn3d(xyz, nullptr, idx, S * B, PMVS_NUM_HYP, p.hs, p.ws, PMVS_NUM_HYP, PMVS_KNN, st));
 
@@ -470,35 +428,34 @@ static int point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flow_weights
                                    keep ? (float*)(ws + p.run) : nullptr, st));
 
   // flow_edge_conv (model.py:213-216): EdgeConvNoC(136,32), EdgeConv(32,32), EdgeConv(64,64)
-  const int cin[3] = {136, 32, 64}, cout[3] = {32, 32, 64}, in_off[3] = {0, 0, 32}, out_off[3] = {0, 32, 96};
   for (int l = 0; l < 3; ++l) {
+    const int cout = flow_ec_cout(l);
     GemmArgs g{};
-    g.x = l == 0 ? feature : ecat + in_off[l];
+    g.x = l == 0 ? feature : ecat + flow_ec_in_off(l);
     g.ldx = l == 0 ? PMVS_FEAT_CH : 224;
-    g.w = wts->ec_w12[l]; g.y = le; g.ldy = 2 * cout[l];
-    g.groups = S; g.rows_per_group = rows_per_group; g.cin = cin[l]; g.cout = 2 * cout[l]; g.eps = wts->eps;
+    g.w = wts->ec_w12[l]; g.y = le; g.ldy = 2 * cout;
+    g.groups = S; g.rows_per_group = rows_per_group; g.cin = flow_ec_cin(l); g.cout = 2 * cout; g.eps = wts->eps;
     // column sums of LE: the central half's BN statistics, which EdgeConvNoC (layer 0) does not have
-    if (edge_impl != 0 && l > 0 && !p.eval) g.out_stats = stats + p.st_ec[l];
+    if (p.tile && l > 0 && !p.eval) g.out_stats = stats + p.st_ec[l];
     if (l > 0 || !fused_le0) PMVS_TRY(launch_gemm(g, st));
-    if (edge_impl != 0) {
+    if (p.tile) {
       EdgeTileArgs e{};
       e.le = le; e.cand = cand;
-      e.coef = (float*)(ws + p.coef) + (size_t)l * S * 6 * 64;
+      e.coef = (float*)(ws + p.coef) + flow_ec_coef_offset(l, S, 0);
       if (!p.eval) {
         e.cstats = stats + p.st_ec[l]; e.nstats = stats + p.st_ecn[l];
         e.ticket = (unsigned*)(stats + p.st_ticket) + (size_t)l * S;
       }
       e.gamma = wts->ec_gamma[l]; e.beta = wts->ec_beta[l]; e.eps = wts->eps; e.concat_central = l > 0;
-      e.out = ecat + out_off[l]; e.ldo = 224; e.groups = S; e.clouds_per_group = B; e.gh = p.hs; e.gw = p.ws;
-      e.cout = cout[l];
-      const int tile_w = edge_impl == 2 ? 16 : 8;
-      if (!p.eval) PMVS_TRY(launch_edge_tile_stats(e, tile_w, st));
-      PMVS_TRY(launch_edge_tile_apply(e, tile_w, st));
+      e.out = ecat + flow_ec_out_off(l); e.ldo = 224; e.groups = S; e.clouds_per_group = B; e.gh = p.hs;
+      e.gw = p.ws; e.cout = cout;
+      if (!p.eval) PMVS_TRY(launch_edge_tile_stats(e, p.tile_w, st));
+      PMVS_TRY(launch_edge_tile_apply(e, p.tile_w, st));
     } else {
       EdgeArgs e{};
       e.le = le; e.idx = idx; e.stats = stats + p.st_ec[l]; e.gamma = wts->ec_gamma[l]; e.beta = wts->ec_beta[l];
-      e.eps = wts->eps; e.concat_central = l > 0; e.out = ecat + out_off[l]; e.ldo = 224; e.groups = S;
-      e.rows_per_group = rows_per_group; e.N = p.N; e.K = PMVS_KNN; e.cout = cout[l];
+      e.eps = wts->eps; e.concat_central = l > 0; e.out = ecat + flow_ec_out_off(l); e.ldo = 224; e.groups = S;
+      e.rows_per_group = rows_per_group; e.N = p.N; e.K = PMVS_KNN; e.cout = cout;
       PMVS_TRY(launch_edge_stats(e, st));
       PMVS_TRY(launch_edge_apply(e, st));
     }
@@ -509,11 +466,7 @@ static int point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flow_weights
     FlowEvalArgs fa{};
     fa.ecat = ecat; fa.w[0] = wts->mlp_w[0]; fa.w[1] = wts->mlp_w[1]; fa.w[2] = wts->mlp_w[2];
     fa.mlp_coef = (const float*)(ws + p.mlp_coef);
-    HeadArgs& h = fa.head;
-    h.w3 = wts->mlp_w[3]; h.depth_prev = depth_prev; h.interval = interval; h.depth_out = depth_out;
-    h.prob_out = prob_out; h.eps = wts->eps; h.interval_scale = shape->interval_scale; h.B = B; h.S = S;
-    h.ratio = shape->ratio; h.sub_begin = p.sub_begin; h.h = shape->flow_h; h.w = shape->flow_w;
-    h.hp = shape->prev_h; h.wp = shape->prev_w;
+    fa.head = head_args(shape, p, wts, depth_prev, interval, depth_out, prob_out);
     if (keep) {
       fa.keep_h[0] = h0; fa.keep_h[1] = h1; fa.keep_h[2] = h2; fa.keep_raw = (float*)(ws + p.raw);
     }
@@ -524,11 +477,11 @@ static int point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flow_weights
   {
     const float* xin[3] = {ecat, h0, h1};
     float* yout[3] = {h0, h1, h2};
-    const int mcin[3] = {224, 64, 64}, mcout[3] = {64, 64, 16};
     for (int l = 0; l < 3; ++l) {
+      const int cin = flow_mlp_cin(l), cout = flow_mlp_cout(l);
       GemmArgs g{};
-      g.x = xin[l]; g.ldx = mcin[l]; g.w = wts->mlp_w[l]; g.y = yout[l]; g.ldy = mcout[l];
-      g.groups = S; g.rows_per_group = rows_per_group; g.cin = mcin[l]; g.cout = mcout[l]; g.eps = wts->eps;
+      g.x = xin[l]; g.ldx = cin; g.w = wts->mlp_w[l]; g.y = yout[l]; g.ldy = cout;
+      g.groups = S; g.rows_per_group = rows_per_group; g.cin = cin; g.cout = cout; g.eps = wts->eps;
       if (l > 0) {
         g.in_stats = stats + p.st_mlp[l - 1]; g.in_gamma = wts->mlp_gamma[l - 1]; g.in_beta = wts->mlp_beta[l - 1];
         g.in_count = (double)rows_per_group;
@@ -537,11 +490,8 @@ static int point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flow_weights
       PMVS_TRY(launch_gemm(g, st));
     }
   }
-  HeadArgs h{};
+  HeadArgs h = head_args(shape, p, wts, depth_prev, interval, depth_out, prob_out);
   h.h2 = h2; h.stats = stats + p.st_mlp[2]; h.gamma = wts->mlp_gamma[2]; h.beta = wts->mlp_beta[2];
-  h.w3 = wts->mlp_w[3]; h.depth_prev = depth_prev; h.interval = interval; h.depth_out = depth_out;
-  h.prob_out = prob_out; h.eps = wts->eps; h.interval_scale = shape->interval_scale; h.B = B; h.S = S; h.ratio = shape->ratio; h.sub_begin = p.sub_begin; h.h = shape->flow_h;
-  h.w = shape->flow_w; h.hp = shape->prev_h; h.wp = shape->prev_w;
   PMVS_TRY(launch_flow_head(h, st));
 
   // BatchNorm running statistics (side effect of running under model.train(), test.py:58)
@@ -549,35 +499,28 @@ static int point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flow_weights
   rb.groups = S; rb.momentum = wts->momentum;
   for (int l = 0; l < 3; ++l) {
     if (wts->ec_run_mean[l] && wts->ec_run_var[l]) {
-      const int c = cout[l];
-      const double* sl = stats + p.st_ec[l];
-      const bool tile = edge_impl != 0;
+      const int c = flow_ec_cout(l);
       if (l > 0) {  // central half: channels [0, c)
         RunUpdate& u = rb.u[rb.n++];
-        u.stats = sl; u.run_mean = wts->ec_run_mean[l]; u.run_var = wts->ec_run_var[l]; u.C = c;
+        u = ec_sums(p, stats, l, true);
+        u.run_mean = wts->ec_run_mean[l]; u.run_var = wts->ec_run_var[l]; u.C = c;
         // statistics of a value repeated K times equal the per-point statistics; only the
         // unbiased correction sees the count, which is N*K as in the reference's BN input
-        u.off_sum = 0; u.off_sq = tile ? 2 * c : c; u.gstride = 4 * c; u.count = (double)rows_per_group;
-        u.ncorr = (double)rows_per_group * PMVS_KNN;
+        u.count = (double)rows_per_group; u.ncorr = (double)rows_per_group * PMVS_KNN;
       }
       RunUpdate& u = rb.u[rb.n++];
+      u = ec_sums(p, stats, l, false);
       u.run_mean = wts->ec_run_mean[l] + (l > 0 ? c : 0); u.run_var = wts->ec_run_var[l] + (l > 0 ? c : 0);
-      u.C = c;
-      if (tile) {
-        u.stats = stats + p.st_ecn[l]; u.off_sum = 0; u.off_sq = c; u.gstride = 2 * c;
-      } else {
-        u.stats = sl; u.off_sum = 2 * c; u.off_sq = 3 * c; u.gstride = 4 * c;
-      }
-      u.count = (double)rows_per_group * PMVS_KNN;
+      u.C = c; u.count = (double)rows_per_group * PMVS_KNN;
       u.ncorr = u.count; u.nbt = wts->ec_nbt[l];
     }
   }
-  const int mcout2[3] = {64, 64, 16};
   for (int l = 0; l < 3; ++l) {
     if (wts->mlp_run_mean[l] && wts->mlp_run_var[l]) {
+      const int c = flow_mlp_cout(l);
       RunUpdate& u = rb.u[rb.n++];
       u.stats = stats + p.st_mlp[l]; u.run_mean = wts->mlp_run_mean[l]; u.run_var = wts->mlp_run_var[l];
-      u.C = mcout2[l]; u.off_sum = 0; u.off_sq = mcout2[l]; u.gstride = 2 * mcout2[l];
+      u.C = c; u.off_sum = 0; u.off_sq = c; u.gstride = 2 * c;
       u.count = (double)rows_per_group; u.ncorr = u.count; u.nbt = wts->mlp_nbt[l];
     }
   }
@@ -596,7 +539,7 @@ extern "C" int pmvs_point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flo
 
 extern "C" size_t pmvs_point_flow_eval_keep_workspace_bytes(const pmvs_flow_shape* shape) {
   FlowPlan p;
-  if (make_plan(shape, p, true) != PMVS_OK) return 0;
+  if (flow_plan(shape, p, true) != PMVS_OK) return 0;
   return p.total;
 }
 

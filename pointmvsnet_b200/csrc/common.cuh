@@ -368,25 +368,51 @@ __device__ __forceinline__ void flow_head_store(const HeadArgs& a, const float (
   a.depth_out[(size_t)b * plane + pix] = __fadd_rn(dprev, flow);
 }
 
+// ---- the PointFlow network's layers (model.py:213-220) -------------------------------------------------------------
+// flow_edge_conv: EdgeConvNoC(136, 32), EdgeConv(32, 32), EdgeConv(64, 64).  Layer l writes flow_ec_channels(l)
+// columns (the neighbour half, after the central half for l > 0) of the 224-wide concatenation at flow_ec_out_off(l);
+// layers 1 and 2 read the previous layer's columns, layer 0 reads F0.  flow_mlp: 224 -> 64 -> 64 -> 16.
+__host__ __device__ constexpr int flow_ec_cin(int l) { return l == 0 ? PMVS_FEAT_CH : l == 1 ? 32 : 64; }
+__host__ __device__ constexpr int flow_ec_cout(int l) { return l == 2 ? 64 : 32; }
+__host__ __device__ constexpr int flow_ec_channels(int l) { return (l > 0 ? 2 : 1) * flow_ec_cout(l); }
+__host__ __device__ constexpr int flow_ec_out_off(int l) {
+  int o = 0;
+  for (int i = 0; i < l; ++i) o += flow_ec_channels(i);
+  return o;
+}
+__host__ __device__ constexpr int flow_ec_in_off(int l) { return l > 0 ? flow_ec_out_off(l - 1) : 0; }
+__host__ __device__ constexpr int flow_mlp_cin(int l) { return l == 0 ? flow_ec_out_off(3) : 64; }
+__host__ __device__ constexpr int flow_mlp_cout(int l) { return l == 2 ? 16 : 64; }
+// The EdgeConv BatchNorm coefficient table (edge_tile.cu layout): per layer S groups of 6 * 64 floats, group g of layer
+// l at this offset
+__host__ __device__ constexpr size_t flow_ec_coef_offset(int l, int S, int g) {
+  return (size_t)l * S * 6 * 64 + (size_t)g * 6 * flow_ec_cout(l);
+}
+// flow_mlp's three BatchNorms as relu(fma(x, A, B)): [A_l | B_l] x flow_mlp_cout(l) at this offset
+__host__ __device__ constexpr int flow_mlp_coef_offset(int l) {
+  int o = 0;
+  for (int i = 0; i < l; ++i) o += 2 * flow_mlp_cout(i);
+  return o;
+}
+
 // ---- running-statistics BatchNorm of the PointFlow path (pmvs_flow_shape.bn_eval = 1; flow_eval.cu) ---------------
-// flow_mlp's three BatchNorms as relu(fma(x, A, B)): [A0 | B0] x 64, [A1 | B1] x 64, [A2 | B2] x 16
-constexpr int FLOW_EVAL_MLP_COEF = 2 * (64 + 64 + 16);
+constexpr int FLOW_EVAL_MLP_COEF = flow_mlp_coef_offset(3);
 // From the running statistics of `w`: the edge_tile coefficient table of the three EdgeConv layers for each of the S
-// groups (ec_coef + l * S * 6 * 64 + g * 6 * cout, the layout of edge_tile.cu) and flow_mlp's table (mlp_coef).  One
-// launch, on the device, so a replayed CUDA graph reads the buffers as they are at replay time.
+// groups (at flow_ec_coef_offset) and flow_mlp's table (mlp_coef, at flow_mlp_coef_offset).  One launch, on the
+// device, so a replayed CUDA graph reads the buffers as they are at replay time.
 // run_copy != NULL (pmvs_point_flow_eval_keep): the running mean and variance as read, FLOW_EVAL_RUN floats at
 // flow_eval_run_offset(l) (layers 0-2 the EdgeConvs, 3-5 flow_mlp): [mean | var] x flow_eval_run_channels(l).
 int launch_flow_eval_coef(const pmvs_flow_weights& w, int S, float* ec_coef, float* mlp_coef, float* run_copy,
                           cudaStream_t st);
-constexpr int FLOW_EVAL_RUN = 2 * (32 + 64 + 128 + 64 + 64 + 16);
-__host__ __device__ __forceinline__ int flow_eval_run_channels(int l) {
-  return l == 0 ? 32 : l == 1 ? 64 : l == 2 ? 128 : l == 5 ? 16 : 64;
+__host__ __device__ constexpr int flow_eval_run_channels(int l) {
+  return l < 3 ? flow_ec_channels(l) : flow_mlp_cout(l - 3);
 }
-__host__ __device__ __forceinline__ int flow_eval_run_offset(int l) {
+__host__ __device__ constexpr int flow_eval_run_offset(int l) {
   int o = 0;
   for (int i = 0; i < l; ++i) o += 2 * flow_eval_run_channels(i);
   return o;
 }
+constexpr int FLOW_EVAL_RUN = flow_eval_run_offset(6);
 struct FlowEvalArgs {
   const float* ecat;      // [S*B*N, 224], the concatenated EdgeConv outputs
   const float* w[3];      // flow_mlp.0.{0,1,2}.conv.weight [64,224], [64,64], [16,64]
@@ -400,15 +426,6 @@ struct FlowEvalArgs {
 // flow_mlp (224 -> 64 -> 64 -> 16 -> 1) and the flow head in one persistent launch: h0, h1, h2 never leave the SM
 // (unless keep_h is given)
 int launch_flow_mlp_head_eval(const FlowEvalArgs& a, cudaStream_t st);
-// byte offsets of the regions of pmvs_point_flow_iter's workspace (api.cu make_plan) and the double offsets of the
-// BatchNorm sums inside `stats`, for the backward that reads it.  keep: pmvs_point_flow_eval_keep's workspace, whose
-// h0-h2, raw (the flow head's input [R]), run (FLOW_EVAL_RUN floats) and mlp_coef regions the eval backward reads.
-struct FlowRegions {
-  size_t cam, feature, xyz, idx, le, ecat, h0, h1, h2, warp_src, cand, stats, coef, mlp_coef, raw, run, total;
-  size_t st_ec[3], st_ecn[3], st_mlp[3];
-  int S;
-};
-int flow_regions(const pmvs_flow_shape* s, FlowRegions& r, bool keep = false);
 // whether launch_gemm applies a fused input BatchNorm as relu(fma(x, A, B)) (gemm_ws.cu) rather than ATen's
 // ((x - mean) * invstd) * gamma + beta (the other kernels); the two can differ in the last bit of the pre-activation
 bool gemm_in_bn_fma_form(const GemmArgs& a);
@@ -428,5 +445,66 @@ struct RunUpdateBatch {
   float momentum;
 };
 int launch_bn_running_update(const RunUpdateBatch& rb, cudaStream_t st);
+
+// The workspace of pmvs_point_flow_iter (byte offsets of its regions) and the EdgeConv family that serves the call,
+// for the forward and for the backward that reads it.
+struct FlowPlan {
+  int S, hs, ws, N;  // S = sub-clouds PROCESSED by this call (all ratio^2 unless sharded)
+  int sub_begin;
+  size_t R;  // rows = S * B * N
+  size_t cam, feature, xyz, idx, le, ecat, h0, h1, h2, stats, total;
+  size_t warp_src;     // the pyramid levels resized to the flow grid, [B,V,h,w,112]
+  size_t cand;         // [R, 16] uint16: kNN neighbour codes for the tile EdgeConv kernels
+  // offsets (in doubles) inside the stats region.  Per EdgeConv layer and group 6*cout doubles: st_ec = 4*cout
+  // (gather path: [sum_c | sumsq_c | sum_n | sumsq_n]; tile path: column sums / sums of squares of the
+  // 2*cout GEMM outputs), st_ecn = 2*cout ([sum_n | sumsq_n] of the tile path)
+  size_t st_ec[3], st_ecn[3], st_mlp[3];
+  size_t st_ticket;    // 3*S unsigned arrival counters of the tile statistics kernels (inside the zeroed region)
+  size_t stats_doubles;
+  size_t coef;         // [3][S][6*64] floats: per (layer, group) BatchNorm coefficients of the tile apply kernels
+  size_t mlp_coef;     // bn_eval: FLOW_EVAL_MLP_COEF floats after the tile tables (flow_mlp's BatchNorms)
+  bool eval;           // bn_eval: running statistics; no stats, h0, h1 or h2 regions (their offsets are 0)
+  // keep (pmvs_point_flow_eval_keep): h0, h1, h2 after every eval region, then the raw flow_mlp outputs [R] and the
+  // copy of the running statistics (FLOW_EVAL_RUN floats); 0 otherwise
+  size_t raw, run;
+  // the EdgeConv family (option edge): the TMA halo tile of width tile_w, else the L2 gathers (edge_kernel); and
+  // whether the int32 neighbour rows (region idx) are written: always for the gathers, on request for the tile
+  bool tile, write_idx32;
+  int tile_w;
+};
+int flow_plan(const pmvs_flow_shape* s, FlowPlan& p, bool keep);
+// the fetch of an iteration (rows a2-a9) over the workspace ws of plan p
+inline FusedFetchParams fetch_params(const pmvs_flow_shape* s, const FlowPlan& p, char* ws, const float* depth_prev) {
+  FusedFetchParams f{};
+  f.src = (const float*)(ws + p.warp_src);
+  f.depth_prev = depth_prev; f.cam_blocks = (const float*)(ws + p.cam); f.feature = (float*)(ws + p.feature);
+  f.xyz = (float*)(ws + p.xyz);
+  f.B = s->B; f.V = s->V; f.h = s->flow_h; f.w = s->flow_w; f.hp = s->prev_h; f.wp = s->prev_w;
+  f.ratio = s->ratio; f.sub_begin = p.sub_begin; f.sub_count = p.S;
+  return f;
+}
+// the flow head's grid, weight, interval and outputs; h2, stats, gamma and beta are the caller's
+inline HeadArgs head_args(const pmvs_flow_shape* s, const FlowPlan& p, const pmvs_flow_weights* w,
+                          const float* depth_prev, const float* interval, float* depth_out, float* prob_out) {
+  HeadArgs h{};
+  h.w3 = w->mlp_w[3]; h.depth_prev = depth_prev; h.interval = interval; h.depth_out = depth_out;
+  h.prob_out = prob_out; h.eps = w->eps; h.interval_scale = s->interval_scale; h.B = s->B; h.S = p.S;
+  h.ratio = s->ratio; h.sub_begin = p.sub_begin; h.h = s->flow_h; h.w = s->flow_w; h.hp = s->prev_h; h.wp = s->prev_w;
+  return h;
+}
+// where EdgeConv layer l's central (layers 1, 2) or neighbour BatchNorm sums are in the stats region of plan p, for
+// the plan's EdgeConv family: a RunUpdate with only stats, off_sum, off_sq and gstride set
+inline RunUpdate ec_sums(const FlowPlan& p, const double* stats, int l, bool central) {
+  const int c = flow_ec_cout(l);
+  RunUpdate u{};
+  if (!p.tile) {
+    u.stats = stats + p.st_ec[l]; u.off_sum = central ? 0 : 2 * c; u.off_sq = central ? c : 3 * c; u.gstride = 4 * c;
+  } else if (central) {
+    u.stats = stats + p.st_ec[l]; u.off_sum = 0; u.off_sq = 2 * c; u.gstride = 4 * c;
+  } else {
+    u.stats = stats + p.st_ecn[l]; u.off_sum = 0; u.off_sq = c; u.gstride = 2 * c;
+  }
+  return u;
+}
 
 }  // namespace pmvs

@@ -318,7 +318,7 @@ __global__ void __launch_bounds__(256) mlp_bwd_eval_kernel(const MlpBn a, const 
 // s4 + l * 4 * 64, m / v the central half's (channels [0, C)), m' / v' the neighbour half's
 __global__ void __launch_bounds__(128) ec_run_sums_kernel(const float* __restrict__ run, double* __restrict__ s4,
                                                           double R) {
-  const int l = blockIdx.x, C = l == 2 ? 64 : 32, c = threadIdx.x;
+  const int l = blockIdx.x, C = flow_ec_cout(l), c = threadIdx.x;
   if (c >= C) return;
   const float* rm = run + flow_eval_run_offset(l);
   const int ctot = flow_eval_run_channels(l);
@@ -373,8 +373,9 @@ __global__ void __launch_bounds__(256) nearest_bwd_kernel(const float* __restric
 }
 
 struct BwdFlowPlan {
-  size_t R, npix, nrec;
-  int N, head_ctas, mlp_ctas;
+  FlowPlan fwd;  // the forward's workspace, which the backward reads
+  size_t npix, nrec;
+  int head_ctas, mlp_ctas;
   size_t idx32, idx64, inv, f0, xyz, le, dle, decat, dtmp, df0, dA, dh, act, st4, wt, layer, wpart, hpart, mpart, mcoef;
   size_t ddup, dfv, rec_idx, rec_w, rec_inv, dsrc, total;
 };
@@ -395,38 +396,33 @@ int bwd_flow_plan(const pmvs_flow_shape* s, BwdFlowPlan& p, bool eval) {
   PMVS_REQUIRE(s->ratio == 1 && s->sub_count == 0 && s->sub_begin == 0,
                "point_flow_backward: only one cloud per call (ratio 1, no sub_count); got ratio %d, sub_count %d",
                s->ratio, s->sub_count);
-  PMVS_REQUIRE((eval ? pmvs_point_flow_eval_keep_workspace_bytes(s) : pmvs_point_flow_workspace_bytes(s)) != 0, "%s",
-               pmvs_last_error());
-  p.N = PMVS_NUM_HYP * s->flow_h * s->flow_w;
-  p.R = (size_t)s->B * p.N;
+  PMVS_TRY(flow_plan(s, p.fwd, eval));
   p.npix = (size_t)s->B * s->flow_h * s->flow_w;
   p.nrec = p.npix * PMVS_NUM_HYP * s->V * 4;
-  PMVS_REQUIRE(p.R * PMVS_KNN < ((size_t)1 << 31) && p.nrec < ((size_t)1 << 31) &&
+  PMVS_REQUIRE(p.fwd.R * PMVS_KNN < ((size_t)1 << 31) && p.nrec < ((size_t)1 << 31) &&
                    (size_t)s->B * (p.nrec / 4 + 1) < ((size_t)1 << 31),
                "point_flow_backward: problem too large");
   p.head_ctas = cdiv((long long)p.npix, HEAD_THREADS);
-  p.mlp_ctas = cdiv((long long)p.R, FB_ROWS);
-  const long long R = (long long)p.R;
+  p.mlp_ctas = cdiv((long long)p.fwd.R, FB_ROWS);
+  const long long R = (long long)p.fwd.R;
   size_t lay = 0;
-  const int cin[3] = {136, 32, 64}, cout[3] = {32, 32, 64};
-  for (int l = 0; l < 3; ++l) lay = std::max(lay, edge_layer_bwd_scratch_bytes(R, cin[l], cout[l]));
-  size_t wp = weight_grad_scratch_bytes(R, 64, 224);
-  wp = std::max(wp, weight_grad_scratch_bytes(R, 64, 64));
-  wp = std::max(wp, weight_grad_scratch_bytes(R, 16, 64));
+  for (int l = 0; l < 3; ++l) lay = std::max(lay, edge_layer_bwd_scratch_bytes(R, flow_ec_cin(l), flow_ec_cout(l)));
+  size_t wp = 0;
+  for (int l = 0; l < 3; ++l) wp = std::max(wp, weight_grad_scratch_bytes(R, flow_mlp_cout(l), flow_mlp_cin(l)));
   size_t o = 0;
-  p.idx32 = o; o += up256(p.R * PMVS_KNN * 4);
-  p.idx64 = o; o += up256(p.R * PMVS_KNN * 8);
-  p.inv = o; o += up256(inv_lists_bytes(s->B, p.N, PMVS_KNN));
-  p.f0 = o; o += up256(p.R * PMVS_FEAT_CH * 4);
-  p.xyz = o; o += up256(p.R * 3 * 4);
-  p.le = o; o += up256(p.R * 128 * 4);
-  p.dle = o; o += up256(p.R * 128 * 4);
-  p.decat = o; o += up256(p.R * 224 * 4);
-  p.dtmp = o; o += up256(p.R * 64 * 4);
-  p.df0 = o; o += up256(p.R * PMVS_FEAT_CH * 4);
-  p.dA = o; o += up256(p.R * 64 * 4);
-  p.dh = o; o += up256(p.R * 64 * 4);
-  p.act = o; o += up256(p.R * 64 * 4);
+  p.idx32 = o; o += up256(p.fwd.R * PMVS_KNN * 4);
+  p.idx64 = o; o += up256(p.fwd.R * PMVS_KNN * 8);
+  p.inv = o; o += up256(inv_lists_bytes(s->B, p.fwd.N, PMVS_KNN));
+  p.f0 = o; o += up256(p.fwd.R * PMVS_FEAT_CH * 4);
+  p.xyz = o; o += up256(p.fwd.R * 3 * 4);
+  p.le = o; o += up256(p.fwd.R * 128 * 4);
+  p.dle = o; o += up256(p.fwd.R * 128 * 4);
+  p.decat = o; o += up256(p.fwd.R * 224 * 4);
+  p.dtmp = o; o += up256(p.fwd.R * 64 * 4);
+  p.df0 = o; o += up256(p.fwd.R * PMVS_FEAT_CH * 4);
+  p.dA = o; o += up256(p.fwd.R * 64 * 4);
+  p.dh = o; o += up256(p.fwd.R * 64 * 4);
+  p.act = o; o += up256(p.fwd.R * 64 * 4);
   p.st4 = o; o += up256(3 * 4 * 64 * 8);
   p.wt = o; o += up256(224 * 64 * 4);
   p.layer = o; o += up256(lay);
@@ -508,13 +504,12 @@ int point_flow_backward(const pmvs_flow_shape* shape, const pmvs_flow_weights* w
   PMVS_REQUIRE(((uintptr_t)fwd_workspace & 255) == 0, "point_flow_backward: fwd_workspace must be 256-byte aligned");
   PMVS_TRY(check_workspace("point_flow_backward", workspace, workspace_bytes, p.total));
   (void)cam_params; (void)mean; (void)stdv;  // the forward's camera blocks already hold them
-  FlowRegions fr;
-  PMVS_TRY(flow_regions(shape, fr, eval));
-  const bool gather = opt(OPT_EDGE) == 0;  // the EdgeConv family of the forward (the options must not change between)
+  const FlowPlan& fr = p.fwd;
+  const bool gather = !fr.tile;  // the EdgeConv family of the forward (the options must not change between)
   cudaStream_t st = (cudaStream_t)stream;
   const char* fw = (const char*)fwd_workspace;
   char* ws = (char*)workspace;
-  const int B = shape->B, N = p.N, R = (int)p.R, h = shape->flow_h, w = shape->flow_w;
+  const int B = shape->B, N = fr.N, R = (int)fr.R, h = shape->flow_h, w = shape->flow_w;
   const float eps = wts->eps;
   const float* ecat = (const float*)(fw + fr.ecat);
   const float* h0 = (const float*)(fw + fr.h0);
@@ -523,15 +518,9 @@ int point_flow_backward(const pmvs_flow_shape* shape, const pmvs_flow_weights* w
   const float* le2 = (const float*)(fw + fr.le);  // the LE scratch holds the last EdgeConv layer's
   const double* stats = (const double*)(fw + fr.stats);
   const float* fcoef = (const float*)(fw + fr.coef);
-  const float* warp_src = (const float*)(fw + fr.warp_src);
-  const float* cam_blocks = (const float*)(fw + fr.cam);
   // eval: the forward's flow_mlp table, raw outputs and running statistics
   const float* ecoef = eval ? (const float*)(fw + fr.mlp_coef) : nullptr;
   const float* run = eval ? (const float*)(fw + fr.run) : nullptr;
-  const int ec_cout[3] = {32, 32, 64}, ec_cin[3] = {136, 32, 64}, mlp_cout[3] = {64, 64, 16}, mlp_cin[3] = {224, 64, 64};
-  const size_t* st_ec = fr.st_ec;
-  const size_t* st_ecn = fr.st_ecn;
-  const size_t* st_mlp = fr.st_mlp;
 
   auto F = [&](size_t o) { return (float*)(ws + o); };
   double* part = (double*)(ws + p.mpart);
@@ -541,14 +530,13 @@ int point_flow_backward(const pmvs_flow_shape* shape, const pmvs_flow_weights* w
   const bool need_pyr = grads->dpyramids_cl[0] || grads->dpyramids_cl[1] || grads->dpyramids_cl[2];
 
   // ---- head
-  HeadArgs ha{};
-  ha.h2 = h2; ha.stats = stats + st_mlp[2]; ha.gamma = wts->mlp_gamma[2]; ha.beta = wts->mlp_beta[2];
-  ha.w3 = wts->mlp_w[3]; ha.interval = interval; ha.eps = eps; ha.interval_scale = shape->interval_scale;
-  ha.B = B; ha.S = 1; ha.ratio = 1; ha.h = h; ha.w = w;
+  HeadArgs ha = head_args(shape, fr, wts, depth_prev, interval, nullptr, nullptr);
+  ha.h2 = h2; ha.stats = stats + fr.st_mlp[2]; ha.gamma = wts->mlp_gamma[2]; ha.beta = wts->mlp_beta[2];
   if (eval) {
     prof_begin("head_bwd_eval", st);
     head_bwd_kernel<true><<<p.head_ctas, HEAD_THREADS, 0, st>>>(ha, grad_prob_out, grad_depth_out, F(p.dA),
-                                                                F(p.hpart), (const float*)(fw + fr.raw), ecoef + 256);
+                                                                F(p.hpart), (const float*)(fw + fr.raw),
+                                                                ecoef + flow_mlp_coef_offset(2));
   } else {
     prof_begin("head_bwd", st);
     head_bwd_kernel<false><<<p.head_ctas, HEAD_THREADS, 0, st>>>(ha, grad_prob_out, grad_depth_out, F(p.dA),
@@ -564,13 +552,12 @@ int point_flow_backward(const pmvs_flow_shape* shape, const pmvs_flow_weights* w
     const float* hs[3] = {h0, h1, h2};
     auto bn = [&](int l, int fma_form) {
       MlpBn a{};
-      a.h = hs[l]; a.stats = stats + st_mlp[l]; a.gamma = wts->mlp_gamma[l]; a.beta = wts->mlp_beta[l];
-      a.count = (double)R; a.eps = eps; a.fma_form = fma_form; a.R = R; a.C = mlp_cout[l];
+      a.h = hs[l]; a.stats = stats + fr.st_mlp[l]; a.gamma = wts->mlp_gamma[l]; a.beta = wts->mlp_beta[l];
+      a.count = (double)R; a.eps = eps; a.fma_form = fma_form; a.R = R; a.C = flow_mlp_cout(l);
       if (eval) {
-        const int coff[3] = {0, 128, 256};
-        a.ecoef = ecoef + coff[l];
+        a.ecoef = ecoef + flow_mlp_coef_offset(l);
         a.rmean = run + flow_eval_run_offset(3 + l);
-        a.rvar = a.rmean + mlp_cout[l];
+        a.rvar = a.rmean + flow_mlp_cout(l);
         a.fma_form = 1;
       }
       return a;
@@ -579,8 +566,9 @@ int point_flow_backward(const pmvs_flow_shape* shape, const pmvs_flow_weights* w
     auto consumer_fma = [&](int l) {
       if (l == 2 || eval) return 0;  // eval: the fused kernel's fma form (mlp_coef)
       GemmArgs g{};
-      g.x = hs[l]; g.ldx = mlp_cout[l]; g.w = wts->mlp_w[l + 1]; g.y = (float*)hs[l + 1]; g.ldy = mlp_cout[l + 1];
-      g.groups = 1; g.rows_per_group = R; g.cin = mlp_cin[l + 1]; g.cout = mlp_cout[l + 1];
+      g.x = hs[l]; g.ldx = flow_mlp_cout(l); g.w = wts->mlp_w[l + 1]; g.y = (float*)hs[l + 1];
+      g.ldy = flow_mlp_cout(l + 1); g.groups = 1; g.rows_per_group = R; g.cin = flow_mlp_cin(l + 1);
+      g.cout = flow_mlp_cout(l + 1);
       return gemm_in_bn_fma_form(g) ? 1 : 0;
     };
     float* dA = F(p.dA);
@@ -597,17 +585,16 @@ int point_flow_backward(const pmvs_flow_shape* shape, const pmvs_flow_weights* w
         PMVS_TRY(mlp_act(bn(l - 1, consumer_fma(l - 1)), F(p.act), st));
         x = F(p.act);
       }
-      PMVS_TRY(launch_weight_grad(dh, x, mlp_cin[l], mlp_cin[l], mlp_cout[l], R, F(p.wpart), grads->mlp_dw[l],
-                                  "mlp_bwd_wgrad_simt", st));
+      const int cin = flow_mlp_cin(l), cout = flow_mlp_cout(l);
+      PMVS_TRY(launch_weight_grad(dh, x, cin, cin, cout, R, F(p.wpart), grads->mlp_dw[l], "mlp_bwd_wgrad_simt", st));
       // dX: d act of layer l - 1 (into dA), or d ecat
-      PMVS_TRY(contract_dx(dh, mlp_cout[l], wts->mlp_w[l], mlp_cin[l], F(p.wt), l > 0 ? dA : F(p.decat), mlp_cin[l],
-                           R, eps, st));
+      PMVS_TRY(contract_dx(dh, cout, wts->mlp_w[l], cin, F(p.wt), l > 0 ? dA : F(p.decat), cin, R, eps, st));
     }
   }
 
   // ---- neighbour rows, inverse lists (once for the three layers), F0
   {
-    const long long total = (long long)p.R * PMVS_KNN;
+    const long long total = (long long)fr.R * PMVS_KNN;
     prof_begin("flow_bwd_idx", st);
     flow_idx_kernel<<<cdiv(total, 256), 256, 0, st>>>(gather ? nullptr : (const unsigned short*)(fw + fr.cand),
                                                      gather ? (const int32_t*)(fw + fr.idx) : nullptr,
@@ -619,15 +606,13 @@ int point_flow_backward(const pmvs_flow_shape* shape, const pmvs_flow_weights* w
   const int* inv_list = nullptr;
   PMVS_TRY(build_inv_lists((const int64_t*)(ws + p.idx64), B, N, PMVS_KNN, ws + p.inv, &inv_off, &inv_list,
                            "flow_bwd_lists", st));
-  FusedFetchParams ff{};
-  ff.src = warp_src; ff.depth_prev = depth_prev; ff.cam_blocks = cam_blocks; ff.feature = F(p.f0); ff.xyz = F(p.xyz);
-  ff.B = B; ff.V = shape->V; ff.h = h; ff.w = w; ff.hp = shape->prev_h; ff.wp = shape->prev_w; ff.ratio = 1;
-  ff.sub_begin = 0; ff.sub_count = 1;
+  // the forward's warp source and camera blocks; F0 and xyz go to this workspace
+  FusedFetchParams ff = fetch_params(shape, fr, (char*)fw, depth_prev);
+  ff.feature = F(p.f0); ff.xyz = F(p.xyz);
   PMVS_TRY(launch_fused_fetch(ff, st));
 
   // ---- flow_edge_conv, layer 2 -> 0
   {
-    const int in_off[3] = {0, 0, 32}, out_off[3] = {0, 32, 96};
     double* st4 = (double*)(ws + p.st4);
     if (eval) {  // the three layers' sums from the kept running statistics
       prof_begin("flow_bwd_run_sums", st);
@@ -635,32 +620,25 @@ int point_flow_backward(const pmvs_flow_shape* shape, const pmvs_flow_weights* w
       PMVS_TRY(check_launch("ec_run_sums_kernel", st));
     }
     for (int l = 2; l >= 0; --l) {
-      const int c = ec_cout[l];
+      const int c = flow_ec_cout(l), cin = flow_ec_cin(l);
       double* s4 = st4 + (size_t)l * 4 * 64;
-      if (eval) {
-        // s4 holds ec_run_sums_kernel's sums
-      } else if (gather) {
-        if (cudaMemcpyAsync(s4, stats + st_ec[l], 4 * c * sizeof(double), cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
-          set_error("point_flow_backward: copy failed");
-          return PMVS_ERR_CUDA;
-        }
-      } else {  // tile family: [sum(2c) | sumsq(2c)] of LE and [sum_n | sumsq_n] -> [sum_c | sumsq_c | sum_n | sumsq_n]
-        const double* cs = stats + st_ec[l];
-        const double* ns = stats + st_ecn[l];
-        const double* srcs[4] = {cs, cs + 2 * c, ns, ns + c};
+      if (!eval) {  // the forward's sums -> [sum_c | sumsq_c | sum_n | sumsq_n] (eval: ec_run_sums_kernel's are there)
+        const RunUpdate cen = ec_sums(fr, stats, l, true), nb = ec_sums(fr, stats, l, false);
+        const double* srcs[4] = {cen.stats + cen.off_sum, cen.stats + cen.off_sq, nb.stats + nb.off_sum,
+                                 nb.stats + nb.off_sq};
         for (int q = (l > 0 ? 0 : 2); q < 4; ++q)
           if (cudaMemcpyAsync(s4 + q * c, srcs[q], c * sizeof(double), cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
             set_error("point_flow_backward: copy failed");
             return PMVS_ERR_CUDA;
           }
       }
-      const float* x = l == 0 ? F(p.f0) : ecat + in_off[l];
+      const float* x = l == 0 ? F(p.f0) : ecat + flow_ec_in_off(l);
       const int ldx = l == 0 ? PMVS_FEAT_CH : 224;
       const float* le = le2;
       if (l < 2) {  // the forward's LE scratch holds layer 2's; recompute the others from the same inputs
         GemmArgs g{};
         g.x = x; g.ldx = ldx; g.w = wts->ec_w12[l]; g.y = F(p.le); g.ldy = 2 * c;
-        g.groups = 1; g.rows_per_group = R; g.cin = ec_cin[l]; g.cout = 2 * c; g.eps = eps;
+        g.groups = 1; g.rows_per_group = R; g.cin = cin; g.cout = 2 * c; g.eps = eps;
         PMVS_TRY(launch_gemm(g, st));
         le = F(p.le);
       }
@@ -668,14 +646,14 @@ int point_flow_backward(const pmvs_flow_shape* shape, const pmvs_flow_weights* w
       L.x = x; L.ldx = ldx; L.idx32 = (const int32_t*)(ws + p.idx32); L.inv_off = inv_off; L.inv_list = inv_list;
       L.w12 = wts->ec_w12[l]; L.gamma = wts->ec_gamma[l]; L.beta = wts->ec_beta[l]; L.eps = eps;
       L.concat_central = l > 0; L.bn_train = eval ? 0 : 1; L.le = le; L.stats = s4;
-      L.tile_coef = gather ? nullptr : fcoef + (size_t)l * 6 * 64;
-      L.dy = F(p.decat) + out_off[l]; L.lddy = 224;
+      L.tile_coef = gather ? nullptr : fcoef + flow_ec_coef_offset(l, 1, 0);
+      L.dy = F(p.decat) + flow_ec_out_off(l); L.lddy = 224;
       L.dx = l > 0 ? F(p.dtmp) : (need_fetch ? F(p.df0) : nullptr);
-      L.lddx = l > 0 ? ec_cin[l] : PMVS_FEAT_CH;
+      L.lddx = l > 0 ? cin : PMVS_FEAT_CH;
       L.dw12 = grads->ec_dw12[l]; L.dgamma = grads->ec_dgamma[l]; L.dbeta = grads->ec_dbeta[l];
-      L.dle = F(p.dle); L.scratch = ws + p.layer; L.B = B; L.N = N; L.K = PMVS_KNN; L.cin = ec_cin[l]; L.cout = c;
+      L.dle = F(p.dle); L.scratch = ws + p.layer; L.B = B; L.N = N; L.K = PMVS_KNN; L.cin = cin; L.cout = c;
       PMVS_TRY(edge_layer_backward(L, st));
-      if (l > 0) PMVS_TRY(add_cols(F(p.decat) + in_off[l], 224, F(p.dtmp), ec_cin[l], R, st));
+      if (l > 0) PMVS_TRY(add_cols(F(p.decat) + flow_ec_in_off(l), 224, F(p.dtmp), cin, R, st));
     }
   }
   if (!need_fetch) return PMVS_OK;

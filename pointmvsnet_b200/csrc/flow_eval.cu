@@ -301,11 +301,10 @@ __global__ void flow_eval_coef_kernel(const pmvs_flow_weights w, int S, float* _
   const int g = blockIdx.x;
   const float eps = w.eps;
   auto istd = [&](float rv) { return (float)(1.0 / sqrt((double)rv + (double)eps)); };
-  const int ec_cout[3] = {32, 32, 64};
   for (int l = 0; l < 3; ++l) {
-    const int C = ec_cout[l];
+    const int C = flow_ec_cout(l);
     const bool central = l > 0;  // EdgeConv: channels [0, C) central, [C, 2C) neighbour; EdgeConvNoC: neighbour only
-    float* cg = ec_coef + (size_t)l * S * 6 * 64 + (size_t)g * 6 * C;
+    float* cg = ec_coef + flow_ec_coef_offset(l, S, g);
     for (int c = threadIdx.x; c < C; c += blockDim.x) {
       // the same forms as the statistics kernel's table (edge_tile.cu)
       const int gn = central ? C + c : c;
@@ -321,17 +320,15 @@ __global__ void flow_eval_coef_kernel(const pmvs_flow_weights w, int S, float* _
     }
   }
   if (g == 0) {
-    const int mlp_cout[3] = {64, 64, 16};
-    float* t = mlp_coef;
     for (int l = 0; l < 3; ++l) {
-      const int C = mlp_cout[l];
+      const int C = flow_mlp_cout(l);
+      float* t = mlp_coef + flow_mlp_coef_offset(l);
       for (int c = threadIdx.x; c < C; c += blockDim.x) {
         // as gemm_tma_kernel's input BatchNorm table
         const float A = __fmul_rn(istd(w.mlp_run_var[l][c]), w.mlp_gamma[l][c]);
         t[c] = A;
         t[C + c] = fmaf(-w.mlp_run_mean[l][c], A, w.mlp_beta[l][c]);
       }
-      t += 2 * C;
     }
     if (run_copy != nullptr)
       for (int l = 0; l < 6; ++l) {
