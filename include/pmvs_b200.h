@@ -611,6 +611,18 @@ int pmvs_point_flow_eval_backward(const pmvs_flow_shape* shape, const pmvs_flow_
                                   const float* grad_prob_out, const pmvs_flow_grads* grads, void* workspace,
                                   size_t workspace_bytes, pmvs_stream_t stream);
 
+/* Debug/inspection view of the workspace after pmvs_point_flow_backward (eval = 0) or pmvs_point_flow_eval_backward
+ * (eval = 1), for a call that requested every input gradient (the fetch regions are only written when an input
+ * gradient is requested, dfv and the records only when a pyramid gradient is).  Byte offsets into that workspace, with
+ * R = 5 B flow_h flow_w points and P = B flow_h flow_w pixels:
+ * off[0]=df0 [R,136] (the gradient of the point features, rows in pmvs_point_flow_debug_offsets' feature order),
+ * off[1]=d depth_up [P] (the upsampled previous depth), off[2]=d f_v [P,5,V,112] (the fetched features, per pixel,
+ * hypothesis and view), off[3]=tap records [P,5,V,4] int64 (NW, NE, SW, SE texel of the view's [V*h*w] block of
+ * the batch element's warp source, -1 for a masked tap), off[4]=tap weights [P,5,V,4], off[5]=d warp source
+ * [B][V*h*w + 1][112] (the trailing texel of each batch element is not written), off[6]=total bytes.
+ * Refuses exactly the shapes the matching *_workspace_bytes function refuses. */
+int pmvs_point_flow_backward_debug_offsets(const pmvs_flow_shape* shape, int eval, size_t off[7]);
+
 /* ---- training loss and metrics (DESIGN 3.16; model.py:308-420, networks.py:170-181 MAELoss) ------------------- */
 /* The T predicted depth maps a step is scored on: T = 1 (coarse_depth_map, isFlow false) or T = 3 (coarse_depth_map,
  * flow1, flow2).  pred[t] is [B, 1, h[t], w[t]] fp32 device memory.  Where h[t - 1] == h[t], w[t - 1] must equal w[t]

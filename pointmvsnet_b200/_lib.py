@@ -148,6 +148,7 @@ _sig("pmvs_point_flow_eval_keep", I, [C.POINTER(FlowShape), C.POINTER(FlowWeight
 _sig("pmvs_point_flow_eval_backward_workspace_bytes", C.c_size_t, [C.POINTER(FlowShape)])
 _sig("pmvs_point_flow_eval_backward", I, [C.POINTER(FlowShape), C.POINTER(FlowWeights), C.POINTER(C.c_void_p * 3),
                                           P, P, P, P, P, P, P, P, C.POINTER(FlowGrads), P, C.c_size_t, P])
+_sig("pmvs_point_flow_backward_debug_offsets", I, [C.POINTER(FlowShape), I, C.POINTER(C.c_size_t * 7)])
 _sig("pmvs_depth_loss", I, [C.POINTER(DepthTerms), P, I, I, P, I, I, F, P, P, P, P])
 _sig("pmvs_depth_loss_backward", I, [C.POINTER(DepthTerms), P, I, I, P, I, I, P, P, C.POINTER(C.c_void_p * 3), P])
 _sig("pmvs_prepare_views_workspace_bytes", C.c_size_t, [I, I, I, I, C.c_double, I, I, I, I])
@@ -169,7 +170,7 @@ EXPORTED = [
     "pmvs_point_flow_debug_feature", "pmvs_point_flow_backward_workspace_bytes", "pmvs_point_flow_backward",
     "pmvs_depth_loss", "pmvs_depth_loss_backward", "pmvs_point_flow_eval_keep_workspace_bytes",
     "pmvs_point_flow_eval_keep", "pmvs_point_flow_eval_backward_workspace_bytes", "pmvs_point_flow_eval_backward",
-    "pmvs_prepare_views_workspace_bytes", "pmvs_prepare_views",
+    "pmvs_point_flow_backward_debug_offsets", "pmvs_prepare_views_workspace_bytes", "pmvs_prepare_views",
 ]
 
 

@@ -726,3 +726,12 @@ extern "C" int pmvs_point_flow_eval_backward(const pmvs_flow_shape* shape, const
   return point_flow_backward(shape, wts, pyramids_cl, depth_prev, cam_params, interval, mean, stdv, fwd_workspace,
                              grad_depth_out, grad_prob_out, grads, workspace, workspace_bytes, stream, true);
 }
+
+extern "C" int pmvs_point_flow_backward_debug_offsets(const pmvs_flow_shape* shape, int eval, size_t off[7]) {
+  BwdFlowPlan p;
+  PMVS_TRY(bwd_flow_plan(shape, p, eval != 0));
+  PMVS_REQUIRE(off != nullptr, "point_flow_backward_debug_offsets: NULL pointer");
+  off[0] = p.df0; off[1] = p.ddup; off[2] = p.dfv; off[3] = p.rec_idx; off[4] = p.rec_w; off[5] = p.dsrc;
+  off[6] = p.total;
+  return PMVS_OK;
+}

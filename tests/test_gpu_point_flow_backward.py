@@ -198,8 +198,9 @@ def test_edge_families_and_fetch_options(golden_weights, monkeypatch, edge):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("V,hw,prev_hw", [(2, (72, 100), (30, 40)), (3, (72, 100), (9, 12)), (6, (64, 96), (16, 24))],
-                         ids=["V2_ragged_downsample", "V3_ragged_upsample", "V6"])
+@pytest.mark.parametrize("V,hw,prev_hw", [(2, (72, 100), (30, 40)), (3, (72, 100), (9, 12)), (6, (64, 96), (16, 24)),
+                                          (12, (64, 80), (12, 15))],
+                         ids=["V2_ragged_downsample", "V3_ragged_upsample", "V6", "V12"])
 def test_shapes(golden_weights, monkeypatch, V, hw, prev_hw):
     """B = 2; flow grids 18 x 25 (not a multiple of the 8 x 4 tile) and 16 x 24; a previous depth map larger than the
     flow grid (nearest down-sample: some pixels get no gradient) and smaller (up-sample).  The synthetic pyramid maps
@@ -207,9 +208,18 @@ def test_shapes(golden_weights, monkeypatch, V, hw, prev_hw):
     texels are correlated.  Every parameter gradient within max(1e-2, 2 s) * max|ref| + 1e-6, s the relative spread
     between the oracle's own closure in fp32 and in float64 on the same input and kNN rows.  The pyramid and depth
     gradients get max(2e-2, 2 s): measured on an H100, pyramid1 1.3e-2 (V = 2; the fp32 oracle 2.6e-3) and
-    coarse_depth 1.2e-2 (V = 6; the fp32 oracle 3.7e-4).  The fp32 oracle forms BatchNorm variances in two passes, the
-    forward kernels from fp32 raw moments (E[x^2] - mean^2, DESIGN 4), which is the suspected, not yet isolated, source
-    of the excess on these 2 250- and 1 920-pixel clouds; on the golden pass every input gradient is within 2.2e-3."""
+    coarse_depth 1.2e-2 (V = 6; the fp32 oracle 3.7e-4); V = 12 at most 7.9e-3 (pyramid0).
+
+    The excess is the forward's fp32 state, which the backward only propagates; no backward stage adds to it.  From the
+    kernels' own fp32 point features and ReLU masks, dF0 is within 5.5e-5 of max|ref| of float64 in every EdgeConv
+    family and in eval mode (test_stage_isolated_parameter_gradients), and every stage after it matches a float64 or
+    exact fp32 reference built from the kernel's own previous stage in these geometries, B = 2, with the same seeded
+    inputs (test_gpu_point_flow_backward_inputs, on an H100): d depth_up within 0.08 of 24 u * sum |terms|
+    (u = 2^-24), the records the forward's taps, d f_v within its (V + 16) u rounding bound, the texel sums and the
+    nearest-resize transpose bit for bit, the resize transposes within 0.1 * 1e-6 max|ref|.  So the 1e-2 gap is where
+    the fp32 forward (point features avg(f^2) - avg(f)^2, fp32 coordinates, BatchNorm from fp32 raw moments, DESIGN 4)
+    and the float64 oracle's forward differ, and the ReLU masks and softmax amplify that difference; the backward
+    cannot remove it, and the 2e-2 floor stays.  On the golden pass every input gradient is within 2.2e-3."""
     from pointmvsnet_b200.synthetic import make_pointflow_inputs
     H, W = hw
     x = make_pointflow_inputs(H, W, views=V, batch=2, seed=5, device=DEV)
@@ -224,6 +234,63 @@ def test_shapes(golden_weights, monkeypatch, V, hw, prev_hw):
     _run_and_compare(_pf(golden_weights), pyr, depth0.contiguous(), x["cam_params_list"], x["mean"],
                      x["std"], x["depth_interval"], (H, W), ((0.25, 0.375),), monkeypatch, derive=True,
                      input_floor=2e-2)
+
+
+def _backward_regions(pf, pyr_cl, cams, interval, mean, std, gd, gp, bn_eval=False):
+    """The backward of pf's last forward run again through the C ABI (the forward's workspace is only read), every
+    input gradient requested, on a workspace of its own filled with NaN bytes.  -> ({df0, ddup, dfv, rec_idx, rec_w,
+    dsrc, dsrc_bytes}: views of that workspace, pmvs_point_flow_backward_debug_offsets' layouts), dpyramids (channels
+    last), ddepth_prev; every output is checked to be written (finite)."""
+    from pointmvsnet_b200._lib import lib, check, ptr, stream_ptr, f32c, FlowGrads
+    shape, fws, depth = pf._last
+    w, _ = pf._weights(fws.device)
+    if bn_eval:
+        size, bwd = lib.pmvs_point_flow_eval_backward_workspace_bytes, lib.pmvs_point_flow_eval_backward
+    else:
+        size, bwd = lib.pmvs_point_flow_backward_workspace_bytes, lib.pmvs_point_flow_backward
+    nbytes = size(C.byref(shape))
+    off = (C.c_size_t * 7)()
+    check(lib.pmvs_point_flow_backward_debug_offsets(C.byref(shape), int(bn_eval), C.byref(off)))
+    assert off[6] == nbytes
+    ws = torch.full((nbytes,), 255, dtype=torch.uint8, device=DEV)  # every float region NaN
+    nan = lambda *s: torch.full(s, float("nan"), device=DEV)  # noqa: E731
+    gr, outs = FlowGrads(), []
+    for l, ec in enumerate(pf.flow_edge_conv):
+        c, cin = ec.conv1.weight.shape[:2]
+        for name, t in (("ec_dw12", nan(2 * c, cin)), ("ec_dgamma", nan(ec.bn.num_features)),
+                        ("ec_dbeta", nan(ec.bn.num_features))):
+            getattr(gr, name)[l] = t.data_ptr()
+            outs.append(t)
+    for l, layer in enumerate(pf.flow_mlp[0]):
+        for name, t in (("mlp_dw", nan(*layer.conv.weight.shape[:2])), ("mlp_dgamma", nan(layer.bn.num_features)),
+                        ("mlp_dbeta", nan(layer.bn.num_features))):
+            getattr(gr, name)[l] = t.data_ptr()
+            outs.append(t)
+    outs.append(nan(16))
+    gr.mlp_dw[3] = outs[-1].data_ptr()
+    dpyr = [nan(*t.shape) for t in pyr_cl]
+    dprev = nan(*depth.shape)
+    for l in range(3):
+        gr.dpyramids_cl[l] = dpyr[l].data_ptr()
+    gr.ddepth_prev = dprev.data_ptr()
+    args = [f32c(t) for t in (cams, interval.reshape(-1), mean, std, gd, gp)]
+    pyr_ptrs = (C.c_void_p * 3)(*[t.data_ptr() for t in pyr_cl])
+    with torch.cuda.device(fws.device):
+        check(bwd(C.byref(shape), C.byref(w), C.byref(pyr_ptrs), ptr(depth), *[ptr(t) for t in args[:4]], ptr(fws),
+                  ptr(args[4]), ptr(args[5]), C.byref(gr), ptr(ws), nbytes, stream_ptr()))
+    torch.cuda.synchronize()
+    for t in outs + dpyr + [dprev]:
+        assert torch.isfinite(t).all(), "an output of the backward was not written"
+    B, V, h, w_ = shape.B, shape.V, shape.flow_h, shape.flow_w
+    P = B * h * w_
+    view = lambda o, n, dt=torch.float32: ws[o:o + n * dt.itemsize].view(dt)  # noqa: E731
+    ndsrc = B * (V * h * w_ + 1) * 112
+    reg = dict(df0=view(off[0], 5 * P * 136).view(5 * P, 136), ddup=view(off[1], P).view(B, h, w_),
+               dfv=view(off[2], P * 5 * V * 112).view(P, 5, V, 112),
+               rec_idx=view(off[3], P * 5 * V * 4, torch.int64).view(P, 5, V, 4),
+               rec_w=view(off[4], P * 5 * V * 4).view(P, 5, V, 4),
+               dsrc=view(off[5], ndsrc).view(B, V * h * w_ + 1, 112), dsrc_bytes=ws[off[5]:off[5] + 4 * ndsrc])
+    return reg, dpyr, dprev
 
 
 def _one_call(pf, gp, requires=True):
@@ -471,13 +538,14 @@ def _stage_masks(pf, st, mlp_fma):
 
 
 def _stage_reference(pf, st, masks, interval, gd, gp, hw):
-    """float64 chain from the fp32 feature with the fp32 masks; returns the 22 parameter gradients of
-    <gd, depth> + <gp, prob> (depth_up carries no parameter gradient)"""
+    """float64 chain from the fp32 feature (a leaf) with the fp32 masks; returns the 22 parameter gradients of
+    <gd, depth> + <gp, prob> (depth_up carries no parameter gradient) and the gradient of the feature [R, 136]"""
     B, N = st["B"], st["N"]
     leaf = lambda t: t.detach().double().clone().requires_grad_(True)  # noqa: E731
     params = [leaf(p) for p in pf._grad_params()]
     idx = st["idx"]
-    x = st["feature"].double().view(B, N, 136).permute(0, 2, 1)
+    feature = leaf(st["feature"])
+    x = feature.view(B, N, 136).permute(0, 2, 1)
     outs = []
     for l in range(3):
         w1, w2, g, b = params[4 * l:4 * l + 4]
@@ -497,7 +565,19 @@ def _stage_reference(pf, st, masks, interval, gd, gp, hw):
     hyp = torch.arange(-2, 3, device=DEV, dtype=torch.float64).view(1, 5, 1, 1)
     flow = (prob * hyp * interval.double().view(-1, 1, 1, 1)).sum(dim=1, keepdim=True)
     ((flow * gd.double()).sum() + (prob * gp.double()).sum()).backward()
-    return [p.grad for p in params]
+    return [p.grad for p in params], feature.grad
+
+
+def _df0_errors(df0, ref):
+    """|err| / max|ref| of the kernel's dF0 against the float64 feature gradient, the 112 variance columns and the 24
+    xyz columns apart (their scales differ), and whether each is within 2e-5 + 1e-4 max|ref|"""
+    out = {}
+    for name, cols in (("df0_var", slice(0, 112)), ("df0_xyz", slice(112, 136))):
+        r = ref[:, cols]
+        err = (df0[:, cols].double() - r).abs().max().item()
+        scale = r.abs().max().item()
+        out[name] = (err / max(scale, 1e-30), err <= 2e-5 + 1e-4 * scale, err, scale)
+    return out
 
 
 NAMES22 = ["ec%d_%s" % (l, k) for l in range(3) for k in ("w1", "w2", "gamma", "beta")] + \
@@ -539,6 +619,9 @@ def test_stage_isolated_parameter_gradients(golden_weights, edge, fetch, mode):
         gd = torch.randn(d.shape, generator=gen).to(DEV)
         gpb = torch.randn(p.shape, generator=gen).to(DEV)
         got = torch.autograd.grad((d, p), pf._grad_params(), (gd, gpb))
+        from pointmvsnet_b200.point_flow import PointFlow
+        reg, _, _ = _backward_regions(pf, PointFlow.pyramids_to_channels_last(pyr), cams, interval, mean, std, gd, gpb)
+        df0 = reg["df0"].clone()
         st = _stage_state(pf, edge)
         mlp_fma = _lib.get_option("gemm") != 0 and mode == 3
         masks = _stage_masks(pf, st, mlp_fma)
@@ -546,7 +629,7 @@ def test_stage_isolated_parameter_gradients(golden_weights, edge, fetch, mode):
         enable_backward(prev)
         _lib.set_gemm_mode(prev_mode)
         _set_options(prev_opts)
-    ref = _stage_reference(pf, st, masks, 0.375 * interval, gd, gpb, d.shape[2:])
+    ref, dfeat = _stage_reference(pf, st, masks, 0.375 * interval, gd, gpb, d.shape[2:])
     worst, bad = {}, []
     for name, g, r in zip(NAMES22, got, ref):
         err = (g.double() - r).abs().max().item()
@@ -554,6 +637,10 @@ def test_stage_isolated_parameter_gradients(golden_weights, edge, fetch, mode):
         tol = 1e-1 * scale if mode == 1 else 2e-5 + 1e-4 * scale
         worst[name] = err / max(scale, 1e-30)
         if err > tol:
+            bad.append((name, err, scale))
+    for name, (rel, ok, err, scale) in _df0_errors(df0, dfeat).items():
+        worst[name] = rel
+        if not (ok or (mode == 1 and err <= 1e-1 * scale)):
             bad.append((name, err, scale))
     print("stage-isolated |err|/max|ref|", {k: "%.1e" % v for k, v in worst.items()})
     assert not bad, bad

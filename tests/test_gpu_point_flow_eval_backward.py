@@ -127,13 +127,14 @@ def _eval_stage_masks(st):
 
 
 def _eval_stage_reference(pf, st, masks, interval, gd, gp, hw):
-    """float64 chain from the fp32 feature with the fp32 masks and running-statistics BatchNorm; returns the 22
-    parameter gradients of <gd, depth> + <gp, prob>"""
+    """float64 chain from the fp32 feature (a leaf) with the fp32 masks and running-statistics BatchNorm; returns the 22
+    parameter gradients of <gd, depth> + <gp, prob> and the gradient of the feature [R, 136]"""
     B, N = st["B"], st["N"]
     leaf = lambda t: t.detach().double().clone().requires_grad_(True)  # noqa: E731
     params = [leaf(p) for p in pf._grad_params()]
     bns = pf._bn_modules()
-    x = st["feature"].double().view(B, N, 136).permute(0, 2, 1)
+    feature = leaf(st["feature"])
+    x = feature.view(B, N, 136).permute(0, 2, 1)
     outs = []
     for l in range(3):
         w1, w2, g, b = params[4 * l:4 * l + 4]
@@ -154,7 +155,7 @@ def _eval_stage_reference(pf, st, masks, interval, gd, gp, hw):
     hyp = torch.arange(-2, 3, device=DEV, dtype=torch.float64).view(1, 5, 1, 1)
     flow = (prob * hyp * interval.double().view(-1, 1, 1, 1)).sum(dim=1, keepdim=True)
     ((flow * gd.double()).sum() + (prob * gp.double()).sum()).backward()
-    return [p.grad for p in params]
+    return [p.grad for p in params], feature.grad
 
 
 def test_stage_isolated_parameter_gradients(golden_weights, switches):
@@ -162,26 +163,41 @@ def test_stage_isolated_parameter_gradients(golden_weights, switches):
     From the kernels' own fp32 feature, neighbour rows and kept h0-h2, the float64 chain (EdgeConv x3, flow_mlp, head)
     with running-statistics BatchNorm and the ReLU masks the fp32 forward applied (from its own coefficient tables)
     gives the reference gradients of <gd, depth> + <gp, prob>; every element of all 22 within 2e-5 + 1e-4 max|ref|,
-    the batch-statistics path's bound (test_gpu_point_flow_backward.test_stage_isolated_parameter_gradients)."""
+    the batch-statistics path's bound (test_gpu_point_flow_backward.test_stage_isolated_parameter_gradients).  The
+    kernel's dF0 (the gradient of the point feature, from a re-run that requests every input gradient) is held to the
+    same bound, its variance and xyz columns apart, in both tile EdgeConv families."""
+    from pointmvsnet_b200.point_flow import PointFlow
     gp_ = load_golden("pass_small.npz")
     cams, mean, std, interval, depth0 = TB._inputs(gp_)
     img_hw = tuple(int(v) for v in gp_["img_hw"])
     pyr = {k: gp_[k].to(DEV) for k in ("conv1", "conv2", "conv3")}
-    pf = TB._pf(golden_weights).eval()
-    d, p = pf(depth0, interval, 0.25, interval_scale=0.375, feature_pyramids=pyr, cam_params_list=cams, mean=mean,
-              std=std, is_test=False, img_hw=img_hw)
-    gen = torch.Generator().manual_seed(11)
-    gd, gpb = torch.randn(d.shape, generator=gen).to(DEV), torch.randn(p.shape, generator=gen).to(DEV)
-    got = torch.autograd.grad((d, p), pf._grad_params(), (gd, gpb))
-    st = _eval_stage_state(pf)
-    ref = _eval_stage_reference(pf, st, _eval_stage_masks(st), 0.375 * interval, gd, gpb, d.shape[2:])
     worst, bad = {}, []
-    for name, g, r in zip(TB.NAMES22, got, ref):
-        err = (g.double() - r).abs().max().item()
-        scale = r.abs().max().item()
-        worst[name] = err / max(scale, 1e-30)
-        if err > 2e-5 + 1e-4 * scale:
-            bad.append((name, err, scale))
+    for edge in (1, 2):
+        prev_opts = TB._set_options({"edge": edge})
+        try:
+            pf = TB._pf(golden_weights).eval()
+            d, p = pf(depth0, interval, 0.25, interval_scale=0.375, feature_pyramids=pyr, cam_params_list=cams,
+                      mean=mean, std=std, is_test=False, img_hw=img_hw)
+            gen = torch.Generator().manual_seed(11)
+            gd, gpb = torch.randn(d.shape, generator=gen).to(DEV), torch.randn(p.shape, generator=gen).to(DEV)
+            got = torch.autograd.grad((d, p), pf._grad_params(), (gd, gpb))
+            reg, _, _ = TB._backward_regions(pf, PointFlow.pyramids_to_channels_last(list(pyr.values())), cams,
+                                             interval, mean, std, gd, gpb, bn_eval=True)
+            df0 = reg["df0"].clone()
+            st = _eval_stage_state(pf)
+        finally:
+            TB._set_options(prev_opts)
+        ref, dfeat = _eval_stage_reference(pf, st, _eval_stage_masks(st), 0.375 * interval, gd, gpb, d.shape[2:])
+        for name, g, r in zip(TB.NAMES22, got, ref):
+            err = (g.double() - r).abs().max().item()
+            scale = r.abs().max().item()
+            worst["edge%d %s" % (edge, name)] = err / max(scale, 1e-30)
+            if err > 2e-5 + 1e-4 * scale:
+                bad.append((edge, name, err, scale))
+        for name, (rel, ok, err, scale) in TB._df0_errors(df0, dfeat).items():
+            worst["edge%d %s" % (edge, name)] = rel
+            if not ok:
+                bad.append((edge, name, err, scale))
     print("stage-isolated |err|/max|ref|", {k: "%.1e" % v for k, v in worst.items()})
     assert not bad, bad
 
