@@ -5,7 +5,8 @@ The batch-statistics oracle (oracle/pointflow_oracle.py) is reused for everythin
 features and hypothesis points (build_point_features), the kNN, the gather and the contractions.  What is restated here
 is the part whose BatchNorm changes: EdgeConv / EdgeConvNoC (networks.py:18-81), flow_mlp (model.py:40-43), the
 sub-cloud flow (model.py:207-229) and the iteration with its strided sub-clouds (model.py:150-295).  BatchNorm is
-y = (x - running_mean) / sqrt(running_var + eps) * gamma + beta, evaluated in float64.
+y = (x - running_mean) / sqrt(running_var + eps) * gamma + beta, evaluated in float64; every function takes the
+BatchNorm ``eps`` (default O.BN_EPS, the reference's), since PointFlow passes its modules' eps to the kernels.
 
 ``params`` is pointflow_oracle.params_from_state_dict's dict plus the running statistics (``eval_params``)."""
 import torch
@@ -36,7 +37,7 @@ def batch_norm_eval(x, rm, rv, gamma, beta, eps=O.BN_EPS):
     return y.to(x.dtype)
 
 
-def edge_conv(feature, knn_inds, w1, w2, gamma, beta, rm, rv, concat_central):
+def edge_conv(feature, knn_inds, w1, w2, gamma, beta, rm, rv, concat_central, eps=O.BN_EPS):
     """pointflow_oracle.edge_conv with running-statistics BatchNorm"""
     K = knn_inds.shape[2]
     local = O.conv1x1(feature, w1)
@@ -44,19 +45,19 @@ def edge_conv(feature, knn_inds, w1, w2, gamma, beta, rm, rv, concat_central):
     neighbour = O.gather_knn(edge, knn_inds)
     central = local.unsqueeze(-1).expand(-1, -1, -1, K)
     e = torch.cat([central, neighbour - central], dim=1) if concat_central else neighbour - central
-    return F.relu(batch_norm_eval(e, rm, rv, gamma, beta)).mean(dim=3)
+    return F.relu(batch_norm_eval(e, rm, rv, gamma, beta, eps)).mean(dim=3)
 
 
-def flow_mlp(x, params):
+def flow_mlp(x, params, eps=O.BN_EPS):
     """pointflow_oracle.flow_mlp with running-statistics BatchNorm: [B,224,N] -> [B,1,N]"""
     for i in range(3):
         x = O.conv1x1(x, params["mlp%d_w" % i])
         x = F.relu(batch_norm_eval(x, params["mlp%d_rm" % i], params["mlp%d_rv" % i], params["mlp%d_gamma" % i],
-                                   params["mlp%d_beta" % i]))
+                                   params["mlp%d_beta" % i], eps))
     return O.conv1x1(x, params["mlp3_w"])
 
 
-def cal_sub_flow(xyz, feature, interval, params, knn=16, return_stages=False, nn_idx=None):
+def cal_sub_flow(xyz, feature, interval, params, knn=16, return_stages=False, nn_idx=None, eps=O.BN_EPS):
     """model.py:207-229: xyz [B,3,5,h,w], feature [B,136,5,h,w] -> flow [B,1,h,w], prob [B,5,h,w].  nn_idx [B,N,16]
     replaces the canonical-order kNN (to replay another implementation's order among equal distances)."""
     B, _, M, h, w = xyz.shape
@@ -66,9 +67,10 @@ def cal_sub_flow(xyz, feature, interval, params, knn=16, return_stages=False, nn
     outs = []
     for l in range(3):
         x = edge_conv(x, nn_idx, params["ec%d_w1" % l], params["ec%d_w2" % l], params["ec%d_gamma" % l],
-                      params["ec%d_beta" % l], params["ec%d_rm" % l], params["ec%d_rv" % l], concat_central=l > 0)
+                      params["ec%d_beta" % l], params["ec%d_rm" % l], params["ec%d_rv" % l], concat_central=l > 0,
+                      eps=eps)
         outs.append(x)
-    raw = flow_mlp(torch.cat(outs, dim=1), params).reshape(B, M, h, w)
+    raw = flow_mlp(torch.cat(outs, dim=1), params, eps).reshape(B, M, h, w)
     prob = F.softmax(-raw, dim=1)
     length = torch.tensor(O.HYPOTHESES).float().view(1, -1, 1, 1) * interval.view(-1, 1, 1, 1)
     flow = torch.sum(prob * length, dim=1, keepdim=True)
@@ -78,7 +80,7 @@ def cal_sub_flow(xyz, feature, interval, params, knn=16, return_stages=False, nn
 
 
 def point_flow(depth, interval, image_scale, pyramids, cam_params, mean, std, img_hw, params, is_test=True,
-               return_stages=False, knn_idx=None):
+               return_stages=False, knn_idx=None, eps=O.BN_EPS):
     """pointflow_oracle.point_flow in eval mode: (flow_result [B,1,h,w], flow_prob [B,5,h,w]).  return_stages adds
     {"edge": [S] of the concatenated EdgeConv outputs [B,224,N] and "nn_idx": [S] of [B,N,16]}, S in the reference's
     sub-cloud order (i, j).  knn_idx: [S] of [B,N,16], the neighbours to use in each sub-cloud (cal_sub_flow)."""
@@ -90,7 +92,7 @@ def point_flow(depth, interval, image_scale, pyramids, cam_params, mean, std, im
 
     def sub_flow(x, f):
         idx = None if knn_idx is None else knn_idx[len(stages["edge"])]
-        fl, pr, st = cal_sub_flow(x, f, interval, params, return_stages=True, nn_idx=idx)
+        fl, pr, st = cal_sub_flow(x, f, interval, params, return_stages=True, nn_idx=idx, eps=eps)
         stages["edge"].append(torch.cat(st["edge"], dim=1))
         stages["nn_idx"].append(st["nn_idx"])
         return fl, pr
@@ -114,7 +116,7 @@ def point_flow(depth, interval, image_scale, pyramids, cam_params, mean, std, im
     return depth_up + flow, prob
 
 
-def mlp_head_from_edge(edge, depth_prev, interval, params, ratio, h, w):
+def mlp_head_from_edge(edge, depth_prev, interval, params, ratio, h, w, eps=O.BN_EPS):
     """flow_mlp and the flow head (model.py:220-227, 244-266) in float64 on whatever device the tensors live on, from the
     concatenated EdgeConv output of an iteration: edge [S, B, N, 224] (PointFlow.debug_stages()["edge"], all S = ratio^2
     sub-clouds in (i, j) order), depth_prev [B,1,hp,wp], interval [B] -> (depth [B,1,h,w], prob [B,5,h,w]) float64.
@@ -126,7 +128,7 @@ def mlp_head_from_edge(edge, depth_prev, interval, params, ratio, h, w):
         def v(k):
             return params[k % i].to(x.device).double()
         x = x @ v("mlp%d_w")[:, :, 0].t()
-        x = torch.relu((x - v("mlp%d_rm")) / torch.sqrt(v("mlp%d_rv") + O.BN_EPS) * v("mlp%d_gamma") + v("mlp%d_beta"))
+        x = torch.relu((x - v("mlp%d_rm")) / torch.sqrt(v("mlp%d_rv") + eps) * v("mlp%d_gamma") + v("mlp%d_beta"))
     raw = (x @ params["mlp3_w"].to(x.device).double()[:, :, 0].t()).view(S, B, len(O.HYPOTHESES), hs, ws)
     prob = torch.softmax(-raw, dim=2)
     length = torch.tensor(O.HYPOTHESES, dtype=torch.float64, device=x.device).view(1, 1, -1, 1, 1) * \
