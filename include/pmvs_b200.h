@@ -672,6 +672,31 @@ int pmvs_prepare_views(const unsigned char* src, int N, int V, int H0, int W0, d
                        int H, int W, float* img_out, unsigned char* ref_out, void* workspace, size_t workspace_bytes,
                        pmvs_stream_t stream);
 
+/* ---- probability filter: zero the depths of low flow / coarse confidence (DESIGN 3.20) ---------------------------- */
+/* Interpolation modes, with OpenCV's values: 0 NEAREST, 1 LINEAR, 2 CUBIC, 4 LANCZOS4 (K = 1, 2, 4, 8 taps). */
+#define PMVS_INTER_NEAREST 0
+#define PMVS_INTER_LINEAR 1
+#define PMVS_INTER_CUBIC 2
+#define PMVS_INTER_LANCZOS4 4
+/* bytes of device workspace pmvs_probability_filter needs (the tables plus one [V, Hs, Wd] horizontal-pass buffer per
+ * map that is resized); 0 (with pmvs_last_error) for arguments it rejects. */
+size_t pmvs_probability_filter_workspace_bytes(int V, int Hd, int Wd, int Hf, int Wf, int Hc, int Wc, int mode);
+/* depth [V,Hd,Wd], flow_conf [V,Hf,Wf], init_conf [V,Hc,Wc] fp32 device memory -> out [V,Hd,Wd]: out = depth, or 0
+ * where the flow confidence resized to Hd x Wd is < flow_thr or the coarse one is < init_thr (a NaN confidence keeps
+ * the depth).  A map already at Hd x Wd is read as is.  The resize is cv2.resize's float32 rule for `mode`, computed
+ * from host tables (`tables`, int32 words, copied to the workspace inside): for each resized map in the order flow,
+ * coarse, [Wd*K] source columns, [Wd*K] float column coefficients, [Hd*K] source rows, [Hd*K] float row coefficients
+ * (utils/depthfusion.py:resize_tables builds them); table_words must be 2 K (Wd + Hd) per resized map.  Horizontal
+ * taps are summed first to last; vertical taps last to first where x < (Wd & ~3) and first to last elsewhere, as
+ * cv2's 4-lane SIMD loop and its scalar tail do; every product and sum is one fp32 rounding.  Rejected
+ * (PMVS_ERR_ARG, before any launch): an unknown mode, a NaN or negative threshold, V or a size < 1, V*H*W >= 2^31 for
+ * any map or horizontal-pass buffer, a NULL pointer, a table of the wrong length or with an index outside its map,
+ * and LINEAR at an exact 2x downsample in both axes (cv2's area path).  Two launches on `stream`, no atomics. */
+int pmvs_probability_filter(const float* depth, const float* flow_conf, const float* init_conf, int V, int Hd, int Wd,
+                            int Hf, int Wf, int Hc, int Wc, float flow_thr, float init_thr, int mode,
+                            const int* tables, size_t table_words, float* out, void* workspace,
+                            size_t workspace_bytes, pmvs_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -153,6 +153,8 @@ _sig("pmvs_depth_loss", I, [C.POINTER(DepthTerms), P, I, I, P, I, I, F, P, P, P,
 _sig("pmvs_depth_loss_backward", I, [C.POINTER(DepthTerms), P, I, I, P, I, I, P, P, C.POINTER(C.c_void_p * 3), P])
 _sig("pmvs_prepare_views_workspace_bytes", C.c_size_t, [I, I, I, I, C.c_double, I, I, I, I])
 _sig("pmvs_prepare_views", I, [P, I, I, I, I, C.c_double, I, I, I, I, P, P, P, C.c_size_t, P])
+_sig("pmvs_probability_filter_workspace_bytes", C.c_size_t, [I, I, I, I, I, I, I, I])
+_sig("pmvs_probability_filter", I, [P, P, P, I, I, I, I, I, I, I, F, F, I, P, C.c_size_t, P, P, C.c_size_t, P])
 
 EXPORTED = [
     "pmvs_version", "pmvs_last_error", "pmvs_launch_count", "pmvs_set_option", "pmvs_get_option", "pmvs_profile_enable", "pmvs_profile_collect", "pmvs_set_gemm_mode", "pmvs_get_gemm_mode", "pmvs_gather_knn_forward",
@@ -171,6 +173,7 @@ EXPORTED = [
     "pmvs_depth_loss", "pmvs_depth_loss_backward", "pmvs_point_flow_eval_keep_workspace_bytes",
     "pmvs_point_flow_eval_keep", "pmvs_point_flow_eval_backward_workspace_bytes", "pmvs_point_flow_eval_backward",
     "pmvs_point_flow_backward_debug_offsets", "pmvs_prepare_views_workspace_bytes", "pmvs_prepare_views",
+    "pmvs_probability_filter_workspace_bytes", "pmvs_probability_filter",
 ]
 
 

@@ -11,13 +11,15 @@ The step the reference hands to the external `fusibile` binary (`depthfusion.py:
 library's own consistency rule (DESIGN.md section 3.10).  It is not bit-compatible with fusibile; the
 Gipuma export above is unchanged for anyone who still runs fusibile.
 """
+import functools
+import math
 import os
 
 import numpy as np
 
 from .io import load_cam_dtu, load_pfm, mkdir, read_gipuma_dmb, write_gipuma_dmb, write_pfm
 
-__all__ = ["probability_filter", "mvsnet_to_gipuma", "mvsnet_to_gipuma_cam", "mvsnet_to_gipuma_dmb",
+__all__ = ["probability_filter", "filter_depth_maps", "resize_tables", "INTER_MODES", "mvsnet_to_gipuma", "mvsnet_to_gipuma_cam", "mvsnet_to_gipuma_dmb",
            "fake_colmap_normal", "fusion_camera_block", "fuse_depth_maps", "write_ply", "fuse_scene"]
 
 
@@ -40,6 +42,136 @@ def probability_filter(scene_folder, init_prob_threshold, flow_prob_threshold, n
         out = depth.copy()
         out[(flow_prob < flow_prob_threshold) | (init_prob < init_prob_threshold)] = 0
         write_pfm(stem + name + "_prob_filtered.pfm", out)
+
+
+# ----------------------------------------------------------------------------------------
+# probability filter on the GPU (DESIGN.md section 3.20)
+# ----------------------------------------------------------------------------------------
+# the reference's --inter_mode names -> OpenCV's interpolation constants (tools/depthfusion.py:220-229)
+INTER_MODES = {"NEAREST": 0, "BILINEAR": 1, "CUBIC": 2, "LANCZOS4": 4}
+_TAPS = {0: 1, 1: 2, 2: 4, 4: 8}
+_S45 = 0.70710678118654752440084436210485
+_LANCZOS_CS = ((1.0, 0.0), (-_S45, -_S45), (0.0, 1.0), (_S45, -_S45), (-1.0, 0.0), (_S45, _S45), (0.0, -1.0),
+               (-_S45, _S45))
+
+
+def _inter_mode(mode):
+    if isinstance(mode, str) and mode in INTER_MODES:
+        return INTER_MODES[mode]
+    if not isinstance(mode, str) and int(mode) in _TAPS and int(mode) == mode:
+        return int(mode)
+    raise ValueError("unknown interpolation mode %r (NEAREST, BILINEAR, CUBIC, LANCZOS4 or cv2's 0, 1, 2, 4)" % (mode,))
+
+
+def _cubic_coefs(x):
+    """cv2 interpolateCubic (A = -0.75) in float32, x a float32 [n] array -> [n,4]."""
+    f = np.float32
+    A = f(-0.75)
+    x1 = x + f(1)
+    c0 = ((A * x1 - f(5) * A) * x1 + f(8) * A) * x1 - f(4) * A
+    c1 = ((A + f(2)) * x - (A + f(3))) * x * x + f(1)
+    y = f(1) - x
+    c2 = ((A + f(2)) * y - (A + f(3))) * y * y + f(1)
+    c3 = f(1) - c0 - c1 - c2
+    return np.stack([c0, c1, c2, c3], axis=1).astype(np.float32)
+
+
+def _lanczos4_coefs(x):
+    """cv2 interpolateLanczos4: sin/cos in double, each coefficient rounded to float, summed in float, scaled by the
+    float 1/sum.  math.sin / math.cos are the C library's, as in cv2, not numpy's vectorised ones."""
+    f = np.float32
+    out = np.empty((len(x), 8), np.float32)
+    for n, xv in enumerate(x):
+        x3 = f(xv + f(3))
+        y0 = -float(x3) * math.pi * 0.25
+        s0, c0 = math.sin(y0), math.cos(y0)
+        total = f(0)
+        for i in range(8):
+            yi = f(x3 - f(i))
+            if abs(yi) >= f(1e-6):
+                y = -float(yi) * math.pi * 0.25
+                out[n, i] = f((_LANCZOS_CS[i][0] * s0 + _LANCZOS_CS[i][1] * c0) / (y * y))
+            else:
+                out[n, i] = f(1e30)
+            total = f(total + out[n, i])
+        out[n] *= f(f(1) / total)
+    return out
+
+
+@functools.lru_cache(maxsize=64)
+def _axis_table(src, dst, mode, is_x):
+    """cv2.resize's source indices [dst,K] int32 and coefficients [dst,K] float32 along one axis of size src -> dst."""
+    scale = 1.0 / (float(dst) / float(src))  # cv2: scale_x = 1. / inv_scale_x, inv_scale_x = dst / src
+    d = np.arange(dst, dtype=np.float64)
+    if mode == 0:
+        idx = np.minimum(np.floor(d * scale).astype(np.int64), src - 1)
+        return idx.reshape(dst, 1).astype(np.int32), np.ones((dst, 1), np.float32)
+    K = _TAPS[mode]
+    fx = ((d + 0.5) * scale - 0.5).astype(np.float32)
+    sx = np.floor(fx).astype(np.int64)
+    fx = (fx - sx.astype(np.float32)).astype(np.float32)
+    if mode == 1:
+        if is_x:  # only the column table moves its border taps; rows are clamped when they are read
+            lo, hi = sx < 0, sx >= src - 1
+            fx[lo | hi] = 0
+            sx[lo], sx[hi] = 0, src - 1
+        coef = np.stack([np.float32(1) - fx, fx], axis=1).astype(np.float32)
+    elif mode == 2:
+        coef = _cubic_coefs(fx)
+    else:
+        coef = _lanczos4_coefs(fx)
+    idx = np.clip(sx[:, None] - (K // 2 - 1) + np.arange(K)[None, :], 0, src - 1)
+    return idx.astype(np.int32), coef
+
+
+def resize_tables(src_hw, dst_hw, mode):
+    """cv2.resize(map [src_hw], (dst_hw[1], dst_hw[0]), interpolation=mode) as tables, in float64 / float32 on the
+    host: (xofs [Wd,K] int32, xcoef [Wd,K] float32, yofs [Hd,K] int32, ycoef [Hd,K] float32)."""
+    mode = _inter_mode(mode)
+    xo, xc = _axis_table(int(src_hw[1]), int(dst_hw[1]), mode, True)
+    yo, yc = _axis_table(int(src_hw[0]), int(dst_hw[0]), mode, False)
+    return xo, xc, yo, yc
+
+
+def filter_depth_maps(depth, flow_conf, init_conf, init_prob_threshold=0.2, flow_prob_threshold=0.1,
+                      mode="LANCZOS4"):
+    """`probability_filter` for every view of a scan in one library call (pmvs_probability_filter, DESIGN.md 3.20).
+
+    depth [V,Hd,Wd], flow_conf [V,Hf,Wf], init_conf [V,Hc,Wc]: CUDA fp32 tensors on one device.  Each confidence map
+    not at Hd x Wd is resized with cv2.resize's float32 rule for `mode` (the reference's name or cv2's constant), and
+    the depth is set to 0 where flow_conf < flow_prob_threshold or init_conf < init_prob_threshold.
+    -> the filtered depth [V,Hd,Wd]; the inputs are not modified."""
+    import torch
+    from .. import _lib
+    m = _inter_mode(mode)
+    for name, t in (("depth", depth), ("flow_conf", flow_conf), ("init_conf", init_conf)):
+        if not isinstance(t, torch.Tensor) or not t.is_cuda:
+            raise RuntimeError("filter_depth_maps: %s must be a CUDA tensor (sm_90a); there is no CPU fallback" % name)
+        if t.dtype != torch.float32 or t.dim() != 3 or t.device != depth.device:
+            raise RuntimeError("filter_depth_maps: %s must be fp32 [V,H,W] on %s, got %s %s on %s"
+                               % (name, depth.device, t.dtype, tuple(t.shape), t.device))
+    V, Hd, Wd = depth.shape
+    if flow_conf.shape[0] != V or init_conf.shape[0] != V:
+        raise RuntimeError("filter_depth_maps: %d depth maps but %d / %d confidence maps"
+                           % (V, flow_conf.shape[0], init_conf.shape[0]))
+    (_, Hf, Wf), (_, Hc, Wc) = flow_conf.shape, init_conf.shape
+    parts = []
+    for (h, w) in ((Hf, Wf), (Hc, Wc)):
+        if (h, w) != (Hd, Wd) and min(V, Hd, Wd, h, w) >= 1:
+            xo, xc, yo, yc = resize_tables((h, w), (Hd, Wd), m)
+            parts += [xo.ravel(), xc.ravel().view(np.int32), yo.ravel(), yc.ravel().view(np.int32)]
+    tables = np.ascontiguousarray(np.concatenate(parts) if parts else np.zeros(0, np.int32), dtype=np.int32)
+    dev = depth.device
+    with torch.cuda.device(dev):
+        depth, flow_conf, init_conf = depth.contiguous(), flow_conf.contiguous(), init_conf.contiguous()
+        nbytes = int(_lib.lib.pmvs_probability_filter_workspace_bytes(V, Hd, Wd, Hf, Wf, Hc, Wc, m))
+        ws = _lib.workspace(nbytes, dev)
+        out = torch.empty_like(depth)
+        _lib.check(_lib.lib.pmvs_probability_filter(
+            depth.data_ptr(), flow_conf.data_ptr(), init_conf.data_ptr(), V, Hd, Wd, Hf, Wf, Hc, Wc,
+            float(flow_prob_threshold), float(init_prob_threshold), m, tables.ctypes.data, len(tables),
+            out.data_ptr(), ws.data_ptr(), nbytes, _lib.stream_ptr()))
+    return out
 
 
 def mvsnet_to_gipuma_dmb(in_path, out_path):
