@@ -194,6 +194,27 @@ int pmvs_fuse_depth_maps(const float* depth, const float* cam_block, int V, int 
                          float depth_thresh, float reproj_thresh, int* count_out, float* xyz_out,
                          unsigned char* used_out, void* workspace, size_t workspace_bytes, pmvs_stream_t stream);
 
+/* ---- geometric-consistency fusion: the MVSNet-family per-view filter, with this library's own rule (DESIGN 3.21) -- */
+/* depth [V,H,W] and cam_block [V,40] as for pmvs_fuse_depth_maps (device memory).  src [V,S] int32 device memory: the
+ * source views of each reference view r, in the order they are checked; -1 pads a list.  Every other entry must be a
+ * view index != r in [0, V): the library cannot read the list on the host without a synchronisation, so it is the
+ * caller's to check (utils/depthfusion.py:consistency_filter refuses other lists before any launch); the kernel skips
+ * such an entry as it skips -1 and never reads out of bounds.  A duplicate entry is checked, and counts, twice.
+ * For each valid pixel (0 < d <= FLT_MAX) of every view r: X = backproject(r, pixel centre, d); for each source s:
+ * (u, w, z) = project(s, X) with z > 0; ds = depth[s] sampled bilinearly at index coordinates (u - 0.5, w - 0.5)
+ * (a tap off the map or invalid reads 0; a coordinate that is non-finite or beyond +-2^24 fails) and valid;
+ * (u', w', z') = project(r, backproject(s, u, w, ds)); s is consistent iff z' > 0, the round trip lands within
+ * reproj_thresh pixels of the centre and |z' - d| <= depth_thresh * d.  count_out [V,H,W] = the number of consistent
+ * sources (-1 for an invalid pixel); depth_avg_out [V,H,W] = (d + sum z') / (count + 1), summed in list order, where
+ * count >= num_consistent, else 0; xyz_out [V,H,W,3] (may be NULL) = backproject(r, pixel centre, depth_avg) there,
+ * else 0.  Every operation is one fp32 rounding (no FMA contraction); no result depends on another view's, so the
+ * outputs do not depend on thread or view order.  Limits as pmvs_fuse_depth_maps: V, H, W >= 1, V*H*W < 2^31,
+ * S >= 0, num_consistent >= 1, thresholds finite and >= 0, NULL pointers refused (src may be NULL when S = 0), all
+ * PMVS_ERR_ARG before any launch.  One launch, no allocation, no synchronisation (CUDA-graph capturable). */
+int pmvs_consistency_filter(const float* depth, const float* cam_block, const int* src, int V, int S, int H, int W,
+                            int num_consistent, float depth_thresh, float reproj_thresh, int* count_out,
+                            float* depth_avg_out, float* xyz_out, pmvs_stream_t stream);
+
 /* ---- point-cloud evaluation (DESIGN 3.11): accuracy / completeness of a fused cloud against a reference scan ---- */
 /* The library's own DTU-style rule, not claimed to reproduce the DTU MATLAB evaluation's numbers.  xyz arrays are
  * [n,3] fp32 device memory; a point with a non-finite coordinate is never kept by thinning and is nobody's neighbour.

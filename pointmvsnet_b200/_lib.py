@@ -105,6 +105,7 @@ _sig("pmvs_cost_volume_backward_workspace_bytes", C.c_size_t, [I, I, I, I, I, I]
 _sig("pmvs_cost_volume_backward", I, [P, P, P, P, P, C.c_size_t, I, I, I, I, I, I, I, P])
 _sig("pmvs_fuse_depth_maps_workspace_bytes", C.c_size_t, [I, I, I])
 _sig("pmvs_fuse_depth_maps", I, [P, P, I, I, I, I, F, F, P, P, P, P, C.c_size_t, P])
+_sig("pmvs_consistency_filter", I, [P, P, P, I, I, I, I, I, F, F, P, P, P, P])
 _sig("pmvs_thin_cloud_workspace_bytes", C.c_size_t, [I])
 _sig("pmvs_thin_cloud", I, [P, P, I, F, F, I, I, P, P, P, C.c_size_t, P])
 _sig("pmvs_nearest_distances_workspace_bytes", C.c_size_t, [I])
@@ -173,7 +174,7 @@ EXPORTED = [
     "pmvs_depth_loss", "pmvs_depth_loss_backward", "pmvs_point_flow_eval_keep_workspace_bytes",
     "pmvs_point_flow_eval_keep", "pmvs_point_flow_eval_backward_workspace_bytes", "pmvs_point_flow_eval_backward",
     "pmvs_point_flow_backward_debug_offsets", "pmvs_prepare_views_workspace_bytes", "pmvs_prepare_views",
-    "pmvs_probability_filter_workspace_bytes", "pmvs_probability_filter",
+    "pmvs_probability_filter_workspace_bytes", "pmvs_probability_filter", "pmvs_consistency_filter",
 ]
 
 

@@ -4,50 +4,19 @@
 //   X = backproject(r, pixel centre, d); (u, w, z) = project(j, X); dj = depth[j] at floor(u, w);
 //   Y = backproject(j, that pixel's centre, dj); (u', w', z') = project(r, Y);
 //   consistent iff z, z' > 0, (u' - px)^2 + (w' - py)^2 <= reproj^2 and |z - dj| <= depth_thresh dj.
-// Every operation is one fp32 rounding (__fmul_rn / __fadd_rn / __fsub_rn / __fdiv_rn are never contracted into FFMA),
-// so the results equal the numpy float32 restatement the tests compare against, bit for bit.
+// Every operation is one fp32 rounding (fusion_geometry.cuh: no FMA contraction), so the results equal the numpy
+// float32 restatement the tests compare against, bit for bit.
 // Within a pass threads read only used[r] and write only used[j != r], and every write stores 1: no atomics, no races,
 // and the outputs do not depend on thread order.
-#include <float.h>
-
 #include "common.cuh"
+#include "fusion_geometry.cuh"
 
 namespace pmvs {
 
 namespace {
 
-// per-view camera block (floats), built on the host by utils/depthfusion.py:fusion_camera_block
-constexpr int FB_KINV = 0, FB_RINV = 9, FB_T = 18, FB_R = 21, FB_K = 30, FB_STRIDE = 40;
-
 // consistency bits are kept per chunk of 32 source views, one word per pixel and chunk
 constexpr int FUSE_CHUNK = 32;
-
-// (a0 b0 + a1 b1) + a2 b2, every product and sum rounded on its own; c points at a uniform camera row
-__device__ __forceinline__ float dot3_rn(const float* __restrict__ c, float b0, float b1, float b2) {
-  return __fadd_rn(__fadd_rn(__fmul_rn(__ldg(c), b0), __fmul_rn(__ldg(c + 1), b1)), __fmul_rn(__ldg(c + 2), b2));
-}
-
-__device__ __forceinline__ void backproject(const float* __restrict__ cb, float px, float py, float d, float& X0,
-                                            float& X1, float& X2) {
-  const float c0 = __fsub_rn(__fmul_rn(dot3_rn(cb + FB_KINV + 0, px, py, 1.f), d), __ldg(cb + FB_T + 0));
-  const float c1 = __fsub_rn(__fmul_rn(dot3_rn(cb + FB_KINV + 3, px, py, 1.f), d), __ldg(cb + FB_T + 1));
-  const float c2 = __fsub_rn(__fmul_rn(dot3_rn(cb + FB_KINV + 6, px, py, 1.f), d), __ldg(cb + FB_T + 2));
-  X0 = dot3_rn(cb + FB_RINV + 0, c0, c1, c2);
-  X1 = dot3_rn(cb + FB_RINV + 3, c0, c1, c2);
-  X2 = dot3_rn(cb + FB_RINV + 6, c0, c1, c2);
-}
-
-__device__ __forceinline__ void project(const float* __restrict__ cb, float X0, float X1, float X2, float& u,
-                                        float& w, float& z) {
-  const float c0 = __fadd_rn(dot3_rn(cb + FB_R + 0, X0, X1, X2), __ldg(cb + FB_T + 0));
-  const float c1 = __fadd_rn(dot3_rn(cb + FB_R + 3, X0, X1, X2), __ldg(cb + FB_T + 1));
-  z = __fadd_rn(dot3_rn(cb + FB_R + 6, X0, X1, X2), __ldg(cb + FB_T + 2));
-  const float nx = __fdiv_rn(c0, z), ny = __fdiv_rn(c1, z);
-  u = dot3_rn(cb + FB_K + 0, nx, ny, 1.f);
-  w = dot3_rn(cb + FB_K + 3, nx, ny, 1.f);
-}
-
-__device__ __forceinline__ bool valid_depth(float d) { return d > 0.f && d <= FLT_MAX; }  // false for NaN
 
 // Step 1 of the check: the pixel of view j that X lands on, or false when it is behind j or off its image.
 __device__ __forceinline__ bool land(const float* __restrict__ cbj, float X0, float X1, float X2, int H, int W,

@@ -2,13 +2,15 @@
 
 The test pipeline of the reference (`test.py` -> `eval_file_logger` per view -> `tools/depthfusion.py`:
 `probability_filter` -> fusion) as one call: the model's outputs that fusion needs stay on the GPU, every view of a
-scene is probability-filtered in one `filter_depth_maps` call and fused with `fuse_depth_maps`.  No per-view files
-are written.  Scoring stays with `utils.cloud_eval.evaluate_cloud`, which takes the returned points.
+scene is probability-filtered in one `filter_depth_maps` call and fused with `fuse_depth_maps` (or, with
+fusion="consistency", `fuse_consistent_views`, DESIGN.md section 3.21).  No per-view files are written.  Scoring
+stays with `utils.cloud_eval.evaluate_cloud`, which takes the returned points.
 """
 import numpy as np
 import torch
 
-from .utils.depthfusion import _axis_table, filter_depth_maps, fuse_depth_maps, write_ply
+from .utils.depthfusion import (_axis_table, _check_fusion, filter_depth_maps, fuse_consistent_views, fuse_depth_maps,
+                               write_ply)
 from .utils.eval_file_logger import _scaled_cam, flow_confidence
 
 __all__ = ["reconstruct_scan"]
@@ -39,7 +41,7 @@ def _text_round_trip(cam):
 
 def reconstruct_scan(net, loader, img_scales, inter_scales, name="flow3", init_prob_threshold=0.2,
                      flow_prob_threshold=0.1, inter_mode="LANCZOS4", num_consistent=3, depth_thresh=0.01,
-                     reproj_thresh=1.0, ply_path=None):
+                     reproj_thresh=1.0, ply_path=None, fusion="fusibile", src_views=None):
     """Run `net` over a test DeviceLoader and fuse each scene's depth maps into a point cloud.
 
     net          a PointMVSNet; its train / eval mode is left as the caller set it
@@ -49,8 +51,12 @@ def reconstruct_scan(net, loader, img_scales, inter_scales, name="flow3", init_p
     name         the flow stage whose depth (preds[name]) and confidence (preds[name + "_prob"]) are fused
     inter_mode   the confidence resize: NEAREST, BILINEAR, CUBIC, LANCZOS4 or cv2's constant
     ply_path     optional PLY path; "{scene}" in it is replaced by the scene's name
+    fusion       "fusibile" (fuse_depth_maps, DESIGN 3.10) or "consistency" (fuse_consistent_views, DESIGN 3.21)
+    src_views    with fusion="consistency": each view's source views (utils.depthfusion.source_list), rows and
+                 entries being positions in the scene's views in ascending view index; default every other view
     -> {scene: {"points": [N,3] fp32, "colors": [N,3] uint8 RGB, "index": [N] int64}} on the device, in the order
        the scenes came.  index = r*H*W + y*W + x over the scene's views in ascending view index."""
+    _check_fusion("reconstruct_scan", fusion, src_views)
     out = {}
     pending = {}  # view index -> (depth, flow confidence, coarse confidence, rgb, camera) of the open scene
     scene = None
@@ -60,9 +66,14 @@ def reconstruct_scan(net, loader, img_scales, inter_scales, name="flow3", init_p
         depth, conf, init, rgb, cams = ([pending[v][i] for v in views] for i in range(5))
         filtered = filter_depth_maps(torch.stack(depth), torch.stack(conf), torch.stack(init), init_prob_threshold,
                                      flow_prob_threshold, inter_mode)
-        points, colors, index = fuse_depth_maps(filtered, np.stack(cams), torch.stack(rgb),
-                                                num_consistent=num_consistent, depth_thresh=depth_thresh,
-                                                reproj_thresh=reproj_thresh)
+        if fusion == "consistency":
+            points, colors, index = fuse_consistent_views(filtered, np.stack(cams), torch.stack(rgb),
+                                                          src_views=src_views, num_consistent=num_consistent,
+                                                          depth_thresh=depth_thresh, reproj_thresh=reproj_thresh)
+        else:
+            points, colors, index = fuse_depth_maps(filtered, np.stack(cams), torch.stack(rgb),
+                                                    num_consistent=num_consistent, depth_thresh=depth_thresh,
+                                                    reproj_thresh=reproj_thresh)
         out[scene] = {"points": points, "colors": colors, "index": index}
         if ply_path is not None:
             write_ply(ply_path.replace("{scene}", scene), points.cpu().numpy(), colors.cpu().numpy())

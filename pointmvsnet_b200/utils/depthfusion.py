@@ -20,7 +20,8 @@ import numpy as np
 from .io import load_cam_dtu, load_pfm, mkdir, read_gipuma_dmb, write_gipuma_dmb, write_pfm
 
 __all__ = ["probability_filter", "filter_depth_maps", "resize_tables", "INTER_MODES", "mvsnet_to_gipuma", "mvsnet_to_gipuma_cam", "mvsnet_to_gipuma_dmb",
-           "fake_colmap_normal", "fusion_camera_block", "fuse_depth_maps", "write_ply", "fuse_scene"]
+           "fake_colmap_normal", "fusion_camera_block", "fuse_depth_maps", "write_ply", "fuse_scene",
+           "source_list", "consistency_filter", "fuse_consistent_views", "FUSION_RULES"]
 
 
 def _resized_to(prob, shape, mode):
@@ -286,18 +287,135 @@ def fuse_depth_maps(depth, cams, images=None, num_consistent=3, depth_thresh=0.0
     -> points [N,3] fp32, colors [N,3] uint8 (None without images), index [N] int64 = r*H*W + y*W + x of each point's
     reference pixel, in ascending index order.  A point is a pixel with at least `num_consistent` consistent views
     (depth_thresh relative, reproj_thresh in pixels); its position is the mean of its own and the views' 3-D points."""
-    import torch
     count, xyz, _ = _fusion_maps(depth, fusion_camera_block(cams), num_consistent, depth_thresh, reproj_thresh)
+    return _compact("fuse_depth_maps", depth, count, xyz, images, num_consistent)
+
+
+def _compact(what, depth, count, xyz, images, num_consistent):
+    """the accepted pixels (count >= num_consistent) of [V,H,W] maps -> points, colours and ascending flat indices"""
+    import torch
     if images is not None:
         if not isinstance(images, torch.Tensor) or images.device != depth.device:
-            raise RuntimeError("fuse_depth_maps: images must be a tensor on %s" % depth.device)
+            raise RuntimeError("%s: images must be a tensor on %s" % (what, depth.device))
         if images.dtype != torch.uint8 or tuple(images.shape) != tuple(depth.shape) + (3,):
-            raise RuntimeError("fuse_depth_maps: images must be uint8 [V,H,W,3] = %s, got %s %s"
-                               % (tuple(depth.shape) + (3,), images.dtype, tuple(images.shape)))
+            raise RuntimeError("%s: images must be uint8 [V,H,W,3] = %s, got %s %s"
+                               % (what, tuple(depth.shape) + (3,), images.dtype, tuple(images.shape)))
     index = torch.nonzero((count >= int(num_consistent)).reshape(-1)).reshape(-1)
     points = xyz.reshape(-1, 3)[index]
     colors = None if images is None else images.reshape(-1, 3)[index]
     return points, colors, index
+
+
+# ----------------------------------------------------------------------------------------
+# geometric-consistency fusion (DESIGN.md section 3.21)
+# ----------------------------------------------------------------------------------------
+def source_list(src_views, V, what="consistency_filter"):
+    """The source views of each of V reference views -> int32 [V,S], checked on the host.
+
+    src_views  None (every other view in ascending order, S = V - 1), an integer array or tensor [V,S], or a sequence
+               of V sequences of view indices (shorter rows are padded with -1).  An entry is -1 (skipped) or a view
+               index != its row in [0, V); a duplicate is checked, and counts, twice."""
+    import torch
+    if src_views is None:
+        return np.array([[s for s in range(V) if s != r] for r in range(V)], dtype=np.int32).reshape(V, V - 1)
+    if isinstance(src_views, torch.Tensor):
+        src_views = src_views.detach().cpu().numpy()
+    if isinstance(src_views, (list, tuple)):
+        rows = [np.asarray(row).reshape(-1) for row in src_views]
+        arr = np.full((len(rows), max((len(row) for row in rows), default=0)), -1, dtype=np.int64)
+        for r, row in enumerate(rows):
+            if len(row) and row.dtype.kind not in "iu":
+                raise RuntimeError("%s: source list row %d is not integer (%s)" % (what, r, row.dtype))
+            arr[r, :len(row)] = row
+    else:
+        arr = np.asarray(src_views)
+        if arr.dtype.kind not in "iu":
+            raise RuntimeError("%s: the source list must be integer, got %s" % (what, arr.dtype))
+    if arr.ndim != 2 or arr.shape[0] != V:
+        raise RuntimeError("%s: the source list must be [V=%d, S], got shape %s" % (what, V, arr.shape))
+    own = np.arange(V)[:, None]
+    bad = (arr != -1) & ((arr < 0) | (arr >= V) | (arr == own))
+    if bad.any():
+        r, k = np.argwhere(bad)[0]
+        raise RuntimeError("%s: source list entry [%d, %d] = %d (must be -1 or a view index != %d in [0, %d))"
+                           % (what, r, k, arr[r, k], r, V))
+    return np.ascontiguousarray(arr, dtype=np.int32)
+
+
+def _consistency_maps(what, depth, cams, src_views, num_consistent, depth_thresh, reproj_thresh, with_xyz):
+    """pmvs_consistency_filter on a CUDA fp32 depth [V,H,W] -> (count [V,H,W] int32, depth_avg [V,H,W] fp32,
+    xyz [V,H,W,3] fp32 or None), all on depth's device.  Everything is checked before any launch."""
+    import torch
+    from .. import _lib
+    if not isinstance(depth, torch.Tensor):
+        raise RuntimeError("%s: depth must be a CUDA tensor (sm_90a); there is no CPU fallback" % what)
+    if depth.dtype != torch.float32 or depth.dim() != 3:
+        raise RuntimeError("%s: depth must be fp32 [V,H,W], got %s %s" % (what, depth.dtype, tuple(depth.shape)))
+    V, H, W = depth.shape
+    block = fusion_camera_block(cams)
+    if block.shape[0] != V:
+        raise RuntimeError("%s: %d depth maps but a camera block of shape %s" % (what, V, block.shape))
+    src = source_list(src_views, V, what)
+    if not depth.is_cuda:
+        raise RuntimeError("%s: depth must be a CUDA tensor (sm_90a); there is no CPU fallback" % what)
+    dev = depth.device
+    with torch.cuda.device(dev):
+        depth = depth.contiguous()
+        block = torch.from_numpy(block).to(dev)
+        src_d = torch.from_numpy(src).to(dev)
+        count = torch.empty(V, H, W, device=dev, dtype=torch.int32)
+        depth_avg = torch.empty(V, H, W, device=dev, dtype=torch.float32)
+        xyz = torch.empty(V, H, W, 3, device=dev, dtype=torch.float32) if with_xyz else None
+        _lib.check(_lib.lib.pmvs_consistency_filter(
+            depth.data_ptr(), block.data_ptr(), src_d.data_ptr() if src.size else None, V, src.shape[1], H, W,
+            int(num_consistent), float(depth_thresh), float(reproj_thresh), count.data_ptr(), depth_avg.data_ptr(),
+            _lib.ptr(xyz), _lib.stream_ptr()))
+    return count, depth_avg, xyz
+
+
+def consistency_filter(depth, cams, src_views=None, num_consistent=3, depth_thresh=0.01, reproj_thresh=1.0):
+    """The MVSNet-family geometric-consistency filter with this library's own rule, every view in one launch
+    (pmvs_consistency_filter, DESIGN.md section 3.21).
+
+    depth      CUDA fp32 [V,H,W]; 0, NaN, inf and negatives are invalid
+    cams       [V,2,4,4] cameras, K at the depth maps' resolution
+    src_views  the source views of each reference view (see `source_list`); default every other view
+    -> count [V,H,W] int32 (consistent sources, -1 for an invalid pixel) and depth_avg [V,H,W] fp32: the mean of the
+    pixel's depth and its consistent sources' reprojected depths where count >= num_consistent, else 0.  A source is
+    consistent when the round trip through its bilinearly sampled depth lands within reproj_thresh pixels and its
+    depth within depth_thresh (relative) of the pixel's."""
+    count, depth_avg, _ = _consistency_maps("consistency_filter", depth, cams, src_views, num_consistent,
+                                            depth_thresh, reproj_thresh, False)
+    return count, depth_avg
+
+
+def fuse_consistent_views(depth, cams, images=None, src_views=None, num_consistent=3, depth_thresh=0.01,
+                          reproj_thresh=1.0):
+    """Fuse a scene's depth maps with the geometric-consistency rule (DESIGN.md section 3.21): every accepted pixel
+    of every view is a point, back-projected at its averaged depth; nothing is suppressed.  Arguments as
+    `consistency_filter`, `images` as `fuse_depth_maps`.
+    -> points [N,3] fp32, colors [N,3] uint8 (None without images), index [N] int64 = r*H*W + y*W + x, ascending."""
+    count, _, xyz = _consistency_maps("fuse_consistent_views", depth, cams, src_views, num_consistent, depth_thresh,
+                                      reproj_thresh, True)
+    return _compact("fuse_consistent_views", depth, count, xyz, images, num_consistent)
+
+
+FUSION_RULES = ("fusibile", "consistency")
+
+
+def _check_fusion(what, fusion, src_views):
+    if fusion not in FUSION_RULES:
+        raise ValueError("%s: unknown fusion rule %r (one of %s)" % (what, fusion, ", ".join(FUSION_RULES)))
+    if fusion != "consistency" and src_views is not None:
+        raise ValueError("%s: src_views applies to fusion='consistency' only" % what)
+
+
+def _fuse(fusion, depth, cams, images=None, src_views=None, num_consistent=3, depth_thresh=0.01, reproj_thresh=1.0):
+    """fuse_depth_maps (fusion="fusibile") or fuse_consistent_views (fusion="consistency")"""
+    _check_fusion("fuse", fusion, src_views)
+    if fusion == "consistency":
+        return fuse_consistent_views(depth, cams, images, src_views, num_consistent, depth_thresh, reproj_thresh)
+    return fuse_depth_maps(depth, cams, images, num_consistent, depth_thresh, reproj_thresh)
 
 
 def write_ply(path, points, colors=None):
@@ -323,13 +441,15 @@ def write_ply(path, points, colors=None):
 
 
 def fuse_scene(scene_folder, name, view_num, ply_path, device="cuda", num_consistent=3, depth_thresh=0.01,
-               reproj_thresh=1.0):
+               reproj_thresh=1.0, fusion="fusibile", src_views=None):
     """The on-disk fusion step of a scene folder (what the reference's mvsnet_to_gipuma + fusibile do,
     depthfusion.py:119-150,173-192): reads %08d_<name>_prob_filtered.pfm (probability_filter's output),
     cam_%08d_<name>.txt and %08d.jpg for the first `view_num` views, resizes each image to its depth map with
-    nearest-neighbour interpolation, fuses on `device` and writes a coloured binary PLY.  Returns the point count."""
+    nearest-neighbour interpolation, fuses on `device` and writes a coloured binary PLY.  Returns the point count.
+    fusion="consistency" fuses with fuse_consistent_views and the source lists `src_views` instead."""
     import cv2
     import torch
+    _check_fusion("fuse_scene", fusion, src_views)
     depths, cams, images = [], [], []
     for v in range(view_num):
         depth = load_pfm(os.path.join(scene_folder, "{:08d}_{}_prob_filtered.pfm".format(v, name)))[0]
@@ -344,7 +464,7 @@ def fuse_scene(scene_folder, name, view_num, ply_path, device="cuda", num_consis
         images.append(cv2.cvtColor(image, cv2.COLOR_BGR2RGB))
     depth = torch.from_numpy(np.stack(depths)).to(device)
     rgb = torch.from_numpy(np.stack(images)).to(device)
-    points, colors, _ = fuse_depth_maps(depth, np.stack(cams), rgb, num_consistent=num_consistent,
-                                        depth_thresh=depth_thresh, reproj_thresh=reproj_thresh)
+    points, colors, _ = _fuse(fusion, depth, np.stack(cams), rgb, src_views=src_views,
+                              num_consistent=num_consistent, depth_thresh=depth_thresh, reproj_thresh=reproj_thresh)
     write_ply(ply_path, points.cpu().numpy(), colors.cpu().numpy())
     return int(points.shape[0])
