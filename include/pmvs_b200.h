@@ -564,6 +564,38 @@ int pmvs_point_flow_debug_offsets(const pmvs_flow_shape* shape, size_t off[10]);
 int pmvs_point_flow_debug_feature(const pmvs_flow_shape* shape, const float* depth_prev, void* workspace,
                                   pmvs_stream_t stream);
 
+/* ---- foveated depth inference: one iteration over a region of the flow grid (DESIGN 3.22) ------------ */
+/* The region [y0, y0 + h) x [x0, x0 + w) of the iteration's flow grid (flow_h x flow_w), in flow-grid pixels.  All four
+ * are multiples of the shape's ratio, h / ratio and w / ratio are at least 2, and the rectangle lies inside the grid.
+ * depth_prev [B,1,prev_h,prev_w] covers rows [prev_y0, prev_y0 + prev_h) and columns [prev_x0, prev_x0 + prev_w) of the
+ * previous iteration's grid of prev_frame_h x prev_frame_w: a whole map has prev_y0 = prev_x0 = 0 and prev_frame_h/w =
+ * prev_h/w; the output of an earlier region call has that call's origin and grid.  Every region pixel's nearest source
+ * pixel (the whole-frame rule) must lie inside the given map. */
+typedef struct pmvs_flow_roi {
+  int y0, x0, h, w;
+  int prev_y0, prev_x0;
+  int prev_frame_h, prev_frame_w;
+} pmvs_flow_roi;
+
+/* bytes of device workspace pmvs_point_flow_iter_roi needs; 0 if the shape or the region is refused */
+size_t pmvs_point_flow_roi_workspace_bytes(const pmvs_flow_shape* shape, const pmvs_flow_roi* roi);
+
+/* pmvs_point_flow_iter restricted to a region (inference, test branch): only the region's pixels become points, split
+ * into ratio^2 strided sub-clouds of 5 * (h / ratio) * (w / ratio) points; the pyramid levels are still resized to the
+ * whole flow grid.  depth_out [B,1,roi.h,roi.w], prob_out [B,5,roi.h,roi.w] (may be NULL).  BatchNorm as
+ * pmvs_point_flow_iter (bn_eval 0: batch statistics of each region sub-cloud, running statistics updated when given).
+ * PMVS_ERR_ARG before any launch for a refused region, is_test = 0 or sub_count > 0.  No allocation and no
+ * synchronisation, so the call can be captured in a CUDA graph.  roi = (0, 0, flow_h, flow_w) with a whole map
+ * computes what pmvs_point_flow_iter computes, bit for bit. */
+int pmvs_point_flow_iter_roi(const pmvs_flow_shape* shape, const pmvs_flow_roi* roi, const pmvs_flow_weights* weights,
+                             const float* const pyramids_cl[3], const float* depth_prev, const float* cam_params,
+                             const float* interval, const float* mean, const float* std, float* depth_out,
+                             float* prob_out, void* workspace, size_t workspace_bytes, pmvs_stream_t stream);
+
+/* pmvs_point_flow_debug_offsets for a region call (the offsets of the workspace pmvs_point_flow_iter_roi used; the
+ * sub-grid is roi.h/ratio x roi.w/ratio) */
+int pmvs_point_flow_roi_debug_offsets(const pmvs_flow_shape* shape, const pmvs_flow_roi* roi, size_t off[10]);
+
 /* ---- backward of one PointFlow iteration (train branch, model.py:150-204, 271-293) ------------ */
 /* Output pointers of pmvs_point_flow_backward.  Every output is overwritten, not accumulated.  The parameter
  * gradients are required; the input gradients may be NULL ("not needed").  ec_dw12[l] is [conv1.weight ; conv2.weight]

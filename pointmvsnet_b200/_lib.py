@@ -43,6 +43,13 @@ class FlowShape(C.Structure):
     ]
 
 
+class FlowRoi(C.Structure):
+    _fields_ = [
+        ("y0", C.c_int), ("x0", C.c_int), ("h", C.c_int), ("w", C.c_int), ("prev_y0", C.c_int), ("prev_x0", C.c_int),
+        ("prev_frame_h", C.c_int), ("prev_frame_w", C.c_int),
+    ]
+
+
 class FlowGrads(C.Structure):
     _fields_ = [
         ("ec_dw12", C.c_void_p * 3), ("ec_dgamma", C.c_void_p * 3), ("ec_dbeta", C.c_void_p * 3),
@@ -137,6 +144,10 @@ _sig("pmvs_linear_pm", I, [P, I, P, P, I, I, I, I, I, P, P, P, C.c_double, F, P,
 _sig("pmvs_point_flow_workspace_bytes", C.c_size_t, [C.POINTER(FlowShape)])
 _sig("pmvs_point_flow_iter", I, [C.POINTER(FlowShape), C.POINTER(FlowWeights), C.POINTER(C.c_void_p * 3),
                                  P, P, P, P, P, P, P, P, C.c_size_t, P])
+_sig("pmvs_point_flow_roi_workspace_bytes", C.c_size_t, [C.POINTER(FlowShape), C.POINTER(FlowRoi)])
+_sig("pmvs_point_flow_iter_roi", I, [C.POINTER(FlowShape), C.POINTER(FlowRoi), C.POINTER(FlowWeights),
+                                     C.POINTER(C.c_void_p * 3), P, P, P, P, P, P, P, P, C.c_size_t, P])
+_sig("pmvs_point_flow_roi_debug_offsets", I, [C.POINTER(FlowShape), C.POINTER(FlowRoi), C.POINTER(C.c_size_t * 10)])
 _sig("pmvs_pyramid_to_channels_last", I, [P, P, I, I, I, I, P])
 _sig("pmvs_point_flow_debug_offsets", I, [C.POINTER(FlowShape), C.POINTER(C.c_size_t * 10)])
 _sig("pmvs_point_flow_debug_feature", I, [C.POINTER(FlowShape), P, P, P])
@@ -175,6 +186,7 @@ EXPORTED = [
     "pmvs_point_flow_eval_keep", "pmvs_point_flow_eval_backward_workspace_bytes", "pmvs_point_flow_eval_backward",
     "pmvs_point_flow_backward_debug_offsets", "pmvs_prepare_views_workspace_bytes", "pmvs_prepare_views",
     "pmvs_probability_filter_workspace_bytes", "pmvs_probability_filter", "pmvs_consistency_filter",
+    "pmvs_point_flow_roi_workspace_bytes", "pmvs_point_flow_iter_roi", "pmvs_point_flow_roi_debug_offsets",
 ]
 
 

@@ -132,7 +132,39 @@ __global__ void __launch_bounds__(256)
 // ---------------------------------------------------------------------------------------
 // PointFlow iteration: workspace plan
 // ---------------------------------------------------------------------------------------
-int flow_plan(const pmvs_flow_shape* s, FlowPlan& p, bool keep) {
+// The region limits of pmvs_point_flow_iter_roi (DESIGN 3.22), checked against an accepted shape.  The nearest source
+// row of a region row Y is min(floor(Y * (prev_frame_h / flow_h)), prev_frame_h - 1) in fp32 as the kernels compute it
+// (fetch_describe, flow_head_store); it is monotone in Y, so the region's first and last rows bound it.
+static int check_roi(const pmvs_flow_shape* s, const pmvs_flow_roi& r) {
+  const int q = s->ratio;
+  PMVS_REQUIRE(s->is_test == 1, "point_flow_roi: a region is served on the test branch only (is_test = 1)");
+  PMVS_REQUIRE(s->sub_count == 0 && s->sub_begin == 0, "point_flow_roi: sub-cloud sharding cannot be combined with a region");
+  PMVS_REQUIRE(r.y0 >= 0 && r.x0 >= 0 && r.h > 0 && r.w > 0 && r.y0 % q == 0 && r.x0 % q == 0 && r.h % q == 0 &&
+                   r.w % q == 0,
+               "point_flow_roi: region (%d, %d, %d, %d) is not aligned to the sub-grid stride %d", r.y0, r.x0, r.h, r.w, q);
+  PMVS_REQUIRE(r.h / q >= 2 && r.w / q >= 2, "point_flow_roi: region %dx%d smaller than 2x2 sub-grid cells of %d", r.h,
+               r.w, q);
+  PMVS_REQUIRE((long long)r.y0 + r.h <= s->flow_h && (long long)r.x0 + r.w <= s->flow_w,
+               "point_flow_roi: region (%d, %d, %d, %d) outside the %dx%d flow grid", r.y0, r.x0, r.h, r.w, s->flow_h,
+               s->flow_w);
+  PMVS_REQUIRE(r.prev_frame_h > 0 && r.prev_frame_w > 0 && r.prev_y0 >= 0 && r.prev_x0 >= 0 &&
+                   (long long)r.prev_y0 + s->prev_h <= r.prev_frame_h && (long long)r.prev_x0 + s->prev_w <= r.prev_frame_w,
+               "point_flow_roi: previous map %dx%d at (%d, %d) outside its %dx%d frame", s->prev_h, s->prev_w, r.prev_y0,
+               r.prev_x0, r.prev_frame_h, r.prev_frame_w);
+  auto src = [](int Y, int n, int pn) {
+    const int v = (int)floorf((float)Y * ((float)pn / (float)n));
+    return v < pn - 1 ? v : pn - 1;
+  };
+  const int ylo = src(r.y0, s->flow_h, r.prev_frame_h), yhi = src(r.y0 + r.h - 1, s->flow_h, r.prev_frame_h);
+  const int xlo = src(r.x0, s->flow_w, r.prev_frame_w), xhi = src(r.x0 + r.w - 1, s->flow_w, r.prev_frame_w);
+  PMVS_REQUIRE(ylo >= r.prev_y0 && yhi < r.prev_y0 + s->prev_h && xlo >= r.prev_x0 && xhi < r.prev_x0 + s->prev_w,
+               "point_flow_roi: the region reads previous rows [%d, %d] and columns [%d, %d], the previous map covers "
+               "rows [%d, %d) and columns [%d, %d)",
+               ylo, yhi, xlo, xhi, r.prev_y0, r.prev_y0 + s->prev_h, r.prev_x0, r.prev_x0 + s->prev_w);
+  return PMVS_OK;
+}
+
+int flow_plan(const pmvs_flow_shape* s, FlowPlan& p, bool keep, const pmvs_flow_roi* roi) {
   PMVS_REQUIRE(s != nullptr, "point_flow: NULL shape");
   const int edge = opt(OPT_EDGE);
   p.tile = edge != 0;
@@ -153,8 +185,14 @@ int flow_plan(const pmvs_flow_shape* s, FlowPlan& p, bool keep) {
                s->sub_begin + s->sub_count, s_all);
   p.S = s->sub_count > 0 ? s->sub_count : s_all;
   p.sub_begin = s->sub_begin;
-  p.hs = s->flow_h / s->ratio;
-  p.ws = s->flow_w / s->ratio;
+  if (roi) {
+    PMVS_TRY(check_roi(s, *roi));
+    p.roi = *roi;
+  } else {
+    p.roi = pmvs_flow_roi{0, 0, s->flow_h, s->flow_w, 0, 0, s->prev_h, s->prev_w};
+  }
+  p.hs = p.roi.h / s->ratio;
+  p.ws = p.roi.w / s->ratio;
   p.N = PMVS_NUM_HYP * p.hs * p.ws;
   p.R = (size_t)p.S * s->B * p.N;
   PMVS_REQUIRE(p.R * 224 < (size_t)1 << 40, "point_flow: problem too large");
@@ -341,14 +379,24 @@ extern "C" size_t pmvs_point_flow_workspace_bytes(const pmvs_flow_shape* shape) 
   return p.total;
 }
 
-extern "C" int pmvs_point_flow_debug_offsets(const pmvs_flow_shape* shape, size_t off[10]) {
+static int debug_offsets(const pmvs_flow_shape* shape, const pmvs_flow_roi* roi, size_t off[10]) {
   FlowPlan p;
-  PMVS_TRY(flow_plan(shape, p, false));
+  PMVS_TRY(flow_plan(shape, p, false, roi));
   off[0] = p.feature; off[1] = p.xyz; off[2] = p.idx; off[3] = p.ecat; off[4] = p.h2;  // h2, stats: 0 under bn_eval
   off[5] = p.le; off[6] = p.stats; off[7] = p.total;
   off[8] = p.cand;
   off[9] = p.write_idx32 ? 1 : 0;  // 1: idx32 is materialised, 0: only cand
   return PMVS_OK;
+}
+
+extern "C" int pmvs_point_flow_debug_offsets(const pmvs_flow_shape* shape, size_t off[10]) {
+  return debug_offsets(shape, nullptr, off);
+}
+
+extern "C" int pmvs_point_flow_roi_debug_offsets(const pmvs_flow_shape* shape, const pmvs_flow_roi* roi,
+                                                 size_t off[10]) {
+  PMVS_REQUIRE(roi != nullptr, "point_flow_roi: NULL region");
+  return debug_offsets(shape, roi, off);
 }
 
 extern "C" int pmvs_point_flow_debug_feature(const pmvs_flow_shape* shape, const float* depth_prev, void* workspace,
@@ -359,13 +407,14 @@ extern "C" int pmvs_point_flow_debug_feature(const pmvs_flow_shape* shape, const
   return launch_fused_fetch(fetch_params(shape, p, (char*)workspace, depth_prev), (cudaStream_t)stream);
 }
 
-// pmvs_point_flow_iter, and with keep pmvs_point_flow_eval_keep
+// pmvs_point_flow_iter, with keep pmvs_point_flow_eval_keep, and with roi pmvs_point_flow_iter_roi
 static int point_flow_iter(const pmvs_flow_shape* shape, const pmvs_flow_weights* wts,
                            const float* const pyramids_cl[3], const float* depth_prev, const float* cam_params,
                            const float* interval, const float* mean, const float* stdv, float* depth_out,
-                           float* prob_out, void* workspace, size_t workspace_bytes, pmvs_stream_t stream, bool keep) {
+                           float* prob_out, void* workspace, size_t workspace_bytes, pmvs_stream_t stream, bool keep,
+                           const pmvs_flow_roi* roi = nullptr) {
   FlowPlan p;
-  PMVS_TRY(flow_plan(shape, p, keep));
+  PMVS_TRY(flow_plan(shape, p, keep, roi));
   PMVS_REQUIRE(wts && pyramids_cl && depth_prev && cam_params && interval && mean && stdv && depth_out && workspace,
                "point_flow: NULL pointer");
   PMVS_TRY(check_workspace("point_flow", workspace, workspace_bytes, p.total));
@@ -550,4 +599,24 @@ extern "C" int pmvs_point_flow_eval_keep(const pmvs_flow_shape* shape, const pmv
                                          size_t workspace_bytes, pmvs_stream_t stream) {
   return point_flow_iter(shape, wts, pyramids_cl, depth_prev, cam_params, interval, mean, stdv, depth_out, prob_out,
                          workspace, workspace_bytes, stream, true);
+}
+
+extern "C" size_t pmvs_point_flow_roi_workspace_bytes(const pmvs_flow_shape* shape, const pmvs_flow_roi* roi) {
+  FlowPlan p;
+  if (roi == nullptr) {
+    set_error("point_flow_roi: NULL region");
+    return 0;
+  }
+  if (flow_plan(shape, p, false, roi) != PMVS_OK) return 0;
+  return p.total;
+}
+
+extern "C" int pmvs_point_flow_iter_roi(const pmvs_flow_shape* shape, const pmvs_flow_roi* roi,
+                                        const pmvs_flow_weights* wts, const float* const pyramids_cl[3],
+                                        const float* depth_prev, const float* cam_params, const float* interval,
+                                        const float* mean, const float* stdv, float* depth_out, float* prob_out,
+                                        void* workspace, size_t workspace_bytes, pmvs_stream_t stream) {
+  PMVS_REQUIRE(roi != nullptr, "point_flow_roi: NULL region");
+  return point_flow_iter(shape, wts, pyramids_cl, depth_prev, cam_params, interval, mean, stdv, depth_out, prob_out,
+                         workspace, workspace_bytes, stream, false, roi);
 }

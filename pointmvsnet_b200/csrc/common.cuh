@@ -281,8 +281,12 @@ struct FusedFetchParams {
   const float* cam_blocks;  // [B, cam_block_floats(V)]
   float* feature;           // [S,B,N,136]
   float* xyz;               // [S,B,3,N]
-  int B, V, h, w, hp, wp, ratio;
+  int B, V, h, w, hp, wp, ratio;  // h, w: the frame (size of the resized source map); hp, wp: depth_prev's size
   int sub_begin, sub_count; // sub-clouds [sub_begin, sub_begin + sub_count) of the ratio^2 are produced
+  // the processed rectangle [y0, y0 + rh) x [x0, x0 + rw) of the frame (all multiples of ratio); depth_prev covers
+  // rows [py0, py0 + hp) and columns [px0, px0 + wp) of a previous frame of pfh x pfw.  A whole-frame call has
+  // (0, 0, h, w), (0, 0) and pfh, pfw = hp, wp.
+  int y0, x0, rh, rw, py0, px0, pfh, pfw;
   int ppw, hs, ws, rlog2;   // set by the launcher: pixels per warp, sub-grid size, log2(ratio) or -1
 };
 // model.py:184 for the three levels at once: channels-last pyramids [B*V,hl,wl,16<<l] -> [B*V,h,w,112]
@@ -326,13 +330,16 @@ struct HeadArgs {
   float* depth_out;         // [B,1,h,w]
   float* prob_out;          // [B,5,h,w] or NULL
   float eps, interval_scale;
-  int B, S, ratio, h, w, hp, wp;
+  int B, S, ratio, h, w, hp, wp;  // h, w: the processed grid (the region); hp, wp: depth_prev's size
   int sub_begin;            // group s of this launch is sub-cloud sub_begin + s of the iteration
+  // the region's origin (y0, x0) in a frame of fh x fw, and depth_prev's origin (py0, px0) in a previous frame of
+  // pfh x pfw: the nearest lookup is that of the whole frames (FusedFetchParams)
+  int y0, x0, fh, fw, py0, px0, pfh, pfw;
 };
 int launch_flow_head(const HeadArgs& a, cudaStream_t st);
 // The end of the flow head for pixel pp of cloud b in group s, given its five raw flow_mlp outputs: softmax(-raw) over
 // the hypotheses (model.py:222), the expected offset (:224-227), depth_up (nearest, :153-158) + flow, scattered to the
-// full grid at the pixel of sub-cloud s + sub_begin (:244-266).  Used by flow_head_kernel and the eval-mode
+// processed grid at the pixel of sub-cloud s + sub_begin (:244-266).  Used by flow_head_kernel and the eval-mode
 // flow_mlp_head_eval_kernel (flow_eval.cu).
 __device__ __forceinline__ void flow_head_store(const HeadArgs& a, const float (&raw)[PMVS_NUM_HYP], int s, int b,
                                                 int pp) {
@@ -360,10 +367,10 @@ __device__ __forceinline__ void flow_head_store(const HeadArgs& a, const float (
     flow = __fadd_rn(flow, __fmul_rn(pr, __fmul_rn((float)(m - 2), itv)));  // model.py:224-227
     if (a.prob_out) a.prob_out[((size_t)b * PMVS_NUM_HYP + m) * plane + pix] = pr;
   }
-  const float nsy = (float)a.hp / (float)a.h, nsx = (float)a.wp / (float)a.w;
-  int ys = (int)floorf((float)Y * nsy), xs = (int)floorf((float)X * nsx);
-  ys = ys < a.hp - 1 ? ys : a.hp - 1;
-  xs = xs < a.wp - 1 ? xs : a.wp - 1;
+  const float nsy = (float)a.pfh / (float)a.fh, nsx = (float)a.pfw / (float)a.fw;
+  int ys = (int)floorf((float)(Y + a.y0) * nsy), xs = (int)floorf((float)(X + a.x0) * nsx);
+  ys = (ys < a.pfh - 1 ? ys : a.pfh - 1) - a.py0;
+  xs = (xs < a.pfw - 1 ? xs : a.pfw - 1) - a.px0;
   const float dprev = __ldg(a.depth_prev + ((size_t)b * a.hp + ys) * a.wp + xs);
   a.depth_out[(size_t)b * plane + pix] = __fadd_rn(dprev, flow);
 }
@@ -449,8 +456,9 @@ int launch_bn_running_update(const RunUpdateBatch& rb, cudaStream_t st);
 // The workspace of pmvs_point_flow_iter (byte offsets of its regions) and the EdgeConv family that serves the call,
 // for the forward and for the backward that reads it.
 struct FlowPlan {
-  int S, hs, ws, N;  // S = sub-clouds PROCESSED by this call (all ratio^2 unless sharded)
+  int S, hs, ws, N;  // S = sub-clouds PROCESSED by this call (all ratio^2 unless sharded); hs, ws: of the region
   int sub_begin;
+  pmvs_flow_roi roi;  // the processed region and the previous map's origin (the whole frame unless a region call)
   size_t R;  // rows = S * B * N
   size_t cam, feature, xyz, idx, le, ecat, h0, h1, h2, stats, total;
   size_t warp_src;     // the pyramid levels resized to the flow grid, [B,V,h,w,112]
@@ -472,7 +480,8 @@ struct FlowPlan {
   bool tile, write_idx32;
   int tile_w;
 };
-int flow_plan(const pmvs_flow_shape* s, FlowPlan& p, bool keep);
+// roi NULL: the whole frame.  A region is checked against the shape (alignment, size, the previous map's coverage).
+int flow_plan(const pmvs_flow_shape* s, FlowPlan& p, bool keep, const pmvs_flow_roi* roi = nullptr);
 // the fetch of an iteration (rows a2-a9) over the workspace ws of plan p
 inline FusedFetchParams fetch_params(const pmvs_flow_shape* s, const FlowPlan& p, char* ws, const float* depth_prev) {
   FusedFetchParams f{};
@@ -481,6 +490,8 @@ inline FusedFetchParams fetch_params(const pmvs_flow_shape* s, const FlowPlan& p
   f.xyz = (float*)(ws + p.xyz);
   f.B = s->B; f.V = s->V; f.h = s->flow_h; f.w = s->flow_w; f.hp = s->prev_h; f.wp = s->prev_w;
   f.ratio = s->ratio; f.sub_begin = p.sub_begin; f.sub_count = p.S;
+  f.y0 = p.roi.y0; f.x0 = p.roi.x0; f.rh = p.roi.h; f.rw = p.roi.w;
+  f.py0 = p.roi.prev_y0; f.px0 = p.roi.prev_x0; f.pfh = p.roi.prev_frame_h; f.pfw = p.roi.prev_frame_w;
   return f;
 }
 // the flow head's grid, weight, interval and outputs; h2, stats, gamma and beta are the caller's
@@ -489,7 +500,9 @@ inline HeadArgs head_args(const pmvs_flow_shape* s, const FlowPlan& p, const pmv
   HeadArgs h{};
   h.w3 = w->mlp_w[3]; h.depth_prev = depth_prev; h.interval = interval; h.depth_out = depth_out;
   h.prob_out = prob_out; h.eps = w->eps; h.interval_scale = s->interval_scale; h.B = s->B; h.S = p.S;
-  h.ratio = s->ratio; h.sub_begin = p.sub_begin; h.h = s->flow_h; h.w = s->flow_w; h.hp = s->prev_h; h.wp = s->prev_w;
+  h.ratio = s->ratio; h.sub_begin = p.sub_begin; h.h = p.roi.h; h.w = p.roi.w; h.hp = s->prev_h; h.wp = s->prev_w;
+  h.y0 = p.roi.y0; h.x0 = p.roi.x0; h.fh = s->flow_h; h.fw = s->flow_w;
+  h.py0 = p.roi.prev_y0; h.px0 = p.roi.prev_x0; h.pfh = p.roi.prev_frame_h; h.pfw = p.roi.prev_frame_w;
   return h;
 }
 // where EdgeConv layer l's central (layers 1, 2) or neighbour BatchNorm sums are in the stats region of plan p, for

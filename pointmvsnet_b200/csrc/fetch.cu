@@ -234,23 +234,24 @@ __host__ __device__ constexpr size_t fetch_smem_total(int V) {  // + 16 floats o
 // un-projects the hypothesis, projects it into the view and writes the 4-tap descriptor desc[t]; lanes 0..4 write the
 // normalised xyz of the 5 hypothesis points to xyzs[3 m ..].  SHARE: returns the ballot `eqmask`, bit m*V+v set <=>
 // hypothesis m hits the same texel quad as hypothesis m-1 in view v (npair <= 30: all 32 lanes vote).  `cam` is the
-// batch element's camera block.
+// batch element's camera block; (X, Y) is a frame pixel, whose nearest previous pixel is taken in the previous frame
+// and then read from depth_prev at (ys - py0, xs - px0).
 template <bool SHARE>
 __device__ __forceinline__ unsigned fetch_describe(const FusedFetchParams& p, const float* cam, Desc* desc,
                                                    float* xyzs, int lane, int b, int X, int Y) {
   const int V = p.V, h = p.h, w = p.w;
   const int npair = PMVS_NUM_HYP * V;
   const float interval = cam[CB_INTERVAL];
-  const float nsy = (float)p.hp / (float)h, nsx = (float)p.wp / (float)w;
+  const float nsy = (float)p.pfh / (float)h, nsx = (float)p.pfw / (float)w;
   const unsigned zero_tex = (unsigned)(V * h * w) * (unsigned)FETCH_C4;  // the batch element's all-zero texel
   // (hypothesis, view) pairs this lane describes: t = lane and, for V > 6, lane + 32
   const int m_a = lane / V, v_a = lane - m_a * V;
   const int m_b = (lane + 32) / V, v_b = lane + 32 - m_b * V;
   int ys = (int)floorf((float)Y * nsy);  // nearest upsample row (model.py:153-158; ATen nearest rule)
-  ys = ys < p.hp - 1 ? ys : p.hp - 1;
+  ys = (ys < p.pfh - 1 ? ys : p.pfh - 1) - p.py0;
   const float py = (float)Y + 0.5f;
   int xs = (int)floorf((float)X * nsx);
-  xs = xs < p.wp - 1 ? xs : p.wp - 1;
+  xs = (xs < p.pfw - 1 ? xs : p.pfw - 1) - p.px0;
   const float dprev = __ldg(p.depth_prev + ((size_t)b * p.hp + ys) * p.wp + xs);
 
   // uv = K_ref^-1 * (x + .5, y + .5, 1)   (functions.py:128-138, model.py:165-170)
@@ -374,7 +375,8 @@ __device__ __forceinline__ void fetch_variance_share(const float4* src, const De
   }
 }
 
-// rows a2-a9; a CTA covers (4 * p.ppw) x 2 pixels, one pixel per warp at a time: phase 1 (fetch_describe), then
+// rows a2-a9 over the region; a CTA covers (4 * p.ppw) x 2 region pixels, one pixel per warp at a time: phase 1
+// (fetch_describe), then
 // phase 2: lanes 0..27 each own one float4 of the 112 channels; for every hypothesis the views are walked in order and
 // the lane keeps the sum / sum of squares of its channels (model.py:188-189), so there is no cross-lane reduction; one
 // tap = one 128-bit ld.global.nc + 4 FFMA per lane, 448 contiguous bytes per warp.
@@ -433,15 +435,16 @@ __global__ void __launch_bounds__(FETCH_WARPS * 32, MINB) fused_fetch_kernel(con
 
   // At step k the 8 warps of the CTA cover a 4 x 2 block of ADJACENT pixels, so the taps they have
   // in flight overlap in L1 (neighbouring pixels project about one texel apart).
+  // region coordinates; y0 and x0 are multiples of ratio, so the sub-cloud of a pixel is that of its frame pixel
   const int Y = blockIdx.y * 2 + (warp >> 2);
-  if (Y >= h) return;  // warp-uniform; no CTA-wide barrier below
+  if (Y >= p.rh) return;  // warp-uniform; no CTA-wide barrier below
   const int yy = p.rlog2 >= 0 ? Y >> p.rlog2 : Y / p.ratio;
   const int ii = Y - yy * p.ratio;
   const int X0 = blockIdx.x * p.ppw * 4 + (warp & 3);
 
   for (int k = 0; k < p.ppw; ++k) {
     const int X = X0 + k * 4;
-    if (X >= w) break;  // warp-uniform
+    if (X >= p.rw) break;  // warp-uniform
     {
       // sub-cloud sharding (model.py:236-267 units spread over GPUs): only pixels of the sub-clouds
       // [sub_begin, sub_begin + sub_count) are produced; rows are numbered from sub_begin
@@ -451,7 +454,7 @@ __global__ void __launch_bounds__(FETCH_WARPS * 32, MINB) fused_fetch_kernel(con
     }
 
     // ---- phase 1: one lane per (hypothesis, view) builds its sampling descriptor --------------
-    const unsigned eqmask = fetch_describe<SHARE>(p, cam, desc, xyzs, lane, b, X, Y);
+    const unsigned eqmask = fetch_describe<SHARE>(p, cam, desc, xyzs, lane, b, X + p.x0, Y + p.y0);
     __syncwarp();
 
     // ---- phase 2: fetch + variance over views ---------------------------------------------------
@@ -566,8 +569,8 @@ __global__ void __launch_bounds__(fg::THREADS, 1)
   long long* rows = reinterpret_cast<long long*>(smem + SM_ROWS);
   auto bar_full = [&](int s) { return sbase + SM_BAR + 8u * (uint32_t)s; };
   auto bar_empty = [&](int s) { return sbase + SM_BAR + 8u * (uint32_t)(NST + s); };
-  const int V = p.V, h = p.h, w = p.w, hw = h * w;
-  const long long npix = (long long)p.B * hw;
+  const int V = p.V, hw = p.h * p.w, rw = p.rw, rhw = p.rh * rw;
+  const long long npix = (long long)p.B * rhw;  // region pixels
   // contiguous, balanced range of tiles
   const long long tiles = (npix + PIX - 1) / PIX;
   const long long t0 = blockIdx.x * tiles / gridDim.x;
@@ -606,10 +609,10 @@ __global__ void __launch_bounds__(fg::THREADS, 1)
       bool ok = pix < npix;
       int b = 0, X = 0, Y = 0, cloud = 0, n0 = 0;
       if (ok) {
-        b = (int)(pix / hw);
-        const int rem = (int)(pix - (long long)b * hw);
-        Y = rem / w;
-        X = rem - Y * w;
+        b = (int)(pix / rhw);
+        const int rem = (int)(pix - (long long)b * rhw);
+        Y = rem / rw;
+        X = rem - Y * rw;
         const int yy = p.rlog2 >= 0 ? Y >> p.rlog2 : Y / p.ratio, xx = p.rlog2 >= 0 ? X >> p.rlog2 : X / p.ratio;
         const int sc = (Y - yy * p.ratio) * p.ratio + (X - xx * p.ratio) - p.sub_begin;
         ok = sc >= 0 && sc < p.sub_count;  // sub-cloud sharding, as in fused_fetch_kernel
@@ -618,7 +621,8 @@ __global__ void __launch_bounds__(fg::THREADS, 1)
       }
       if (ok) {  // warp-uniform
         const unsigned eqmask =
-            fetch_describe<true>(p, p.cam_blocks + (size_t)b * cam_block_floats(V), desc, xyzs, lane, b, X, Y);
+            fetch_describe<true>(p, p.cam_blocks + (size_t)b * cam_block_floats(V), desc, xyzs, lane, b, X + p.x0,
+                                 Y + p.y0);
         __syncwarp();
         const uint32_t tile = sbase + SM_RING + s * STAGE;
         const int r0 = slot * PMVS_NUM_HYP;
@@ -778,7 +782,7 @@ static int fetch_setup(const FusedFetchParams& p0, FusedFetchParams& p) {
   // tap offsets are 32-bit float4 offsets inside one batch element's [V, h, w, 112] map
   PMVS_REQUIRE((npix * p.V + 1) * FETCH_C4 < (1ll << 32), "fused_fetch: V=%d x %dx%d too large", p.V, p.h, p.w);
   PMVS_REQUIRE(p.h <= 65535 && p.B <= 65535, "fused_fetch: h or B too large");
-  p.hs = p.h / p.ratio; p.ws = p.w / p.ratio;
+  p.hs = p.rh / p.ratio; p.ws = p.rw / p.ratio;
   p.rlog2 = -1;
   for (int q = 0; q < 16; ++q) if ((1 << q) == p.ratio) p.rlog2 = q;
   return PMVS_OK;
@@ -787,11 +791,11 @@ static int fetch_setup(const FusedFetchParams& p0, FusedFetchParams& p) {
 int launch_fused_fetch(const FusedFetchParams& p0, cudaStream_t st) {
   FusedFetchParams p;
   PMVS_TRY(fetch_setup(p0, p));
-  const long long npix = (long long)p.h * p.w;
+  const long long npix = (long long)p.rh * p.rw;
   // several consecutive pixels of a row per warp once there are enough pixels to fill the machine
   const long long per = npix / ((long long)sm_count() * FETCH_WARPS * 8);
   p.ppw = per >= 4 ? 4 : (per >= 2 ? 2 : 1);
-  dim3 grid(cdiv(p.w, 4 * p.ppw), cdiv(p.h, 2), p.B);  // CTA = (4 * ppw) x 2 pixels
+  dim3 grid(cdiv(p.rw, 4 * p.ppw), cdiv(p.rh, 2), p.B);  // CTA = (4 * ppw) x 2 region pixels
   const size_t smem = fetch_smem_total(p.V);
   prof_begin("fused_fetch", st);
   // option 3 (fetch_gemm_kernel) runs this kernel where it does not apply
@@ -814,7 +818,7 @@ int launch_fetch_gemm(const FusedFetchParams& p0, const float* w12, float* le, c
     return -1;
   static unsigned long long smem_done = 0;
   if (ensure_dyn_smem(fetch_gemm_kernel, fg::SMEM, smem_done, "fetch_gemm") != PMVS_OK) return -1;
-  const long long tiles = ((long long)p.B * p.h * p.w + fg::PIX - 1) / fg::PIX;
+  const long long tiles = ((long long)p.B * p.rh * p.rw + fg::PIX - 1) / fg::PIX;
   const int grid = (int)std::min<long long>(tiles, sm_count());
   // profiled as the fetch it replaces: the contraction runs inside it
   prof_begin("fused_fetch", st);

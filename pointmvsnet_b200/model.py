@@ -74,11 +74,17 @@ class PointMVSNet(nn.Module):
                                       nn.Conv1d(flow_channels[-2], flow_channels[-1], 1, bias=False))
         object.__setattr__(self, "_point_flow", PointFlow(flow_edge_conv=self.flow_edge_conv, flow_mlp=self.flow_mlp))
 
-    def forward(self, data_batch, img_scales, inter_scales, isFlow, isTest=False):
+    def forward(self, data_batch, img_scales, inter_scales, isFlow, isTest=False, fovea=None):
         """model.py:45-305: data_batch holds img_list [B,V,3,H,W], cam_params_list [B,V,2,4,4] and (with isFlow)
         mean, std [B,3], all CUDA.  Returns the reference's OrderedDict: world_points [B,3,D*h*w], coarse_depth_map
         and coarse_prob_map [B,1,h,w] (h, w = H/8, W/8), then per iteration i flow{i}_prob [B,5,..] and flow{i}
-        [B,1,..], in the reference's insertion order."""
+        [B,1,..], in the reference's insertion order.
+
+        fovea (foveated depth inference, DESIGN 3.22; needs isFlow and isTest): a dict with ``box`` = (y0, x0, h, w) in
+        input-image pixels, all multiples of 8, ``img_scales`` and ``inter_scales``.  After the whole-image iterations
+        one region iteration per scale s refines the box's rectangle (y0 s, x0 s, h s, w s) of the grid
+        int(H s) x int(W s); the first reads the last flow{i}, each later one the previous region.  Adds fovea{j}
+        [B,1,h s,w s], fovea{j}_prob [B,5,h s,w s] and fovea{j}_origin = (y0 s, x0 s, int(H s), int(W s)), j = 1, 2, .."""
         img_list = data_batch["img_list"]
         cams = data_batch["cam_params_list"]
         require_cuda(img_list, cams)
@@ -97,6 +103,8 @@ class PointMVSNet(nn.Module):
             raise RuntimeError("PointMVSNet: img_list must be [B,V,3,H,W] and cam_params_list [B,V,2,4,4], got %s "
                                "and %s" % (tuple(img_list.shape), tuple(cams.shape)))
         B, V, _, H, W = img_list.shape
+        if fovea is not None:
+            fovea = _fovea_plan(fovea, H, W, isFlow, isTest)
         h, w = networks._level_sizes(H, W)[3]
         D = int(cams[0, 0, 1, 3, 2].item())  # model.py:65 (the reference reads it on the host too)
         if D < 8 or h < 8 or w < 8 or D % 8 or h % 8 or w % 8:
@@ -129,7 +137,45 @@ class PointMVSNet(nn.Module):
             preds["flow{}_prob".format(i + 1)] = flow_prob
             preds["flow{}".format(i + 1)] = flow
             depth = flow
+        origin = None
+        for j, (img_scale, inter_scale, roi, frame) in enumerate(fovea or ()):
+            with torch.no_grad():
+                flow, flow_prob = pf(depth.detach(), depth_interval, img_scale, interval_scale=inter_scale,
+                                     feature_pyramids=None, pyramids_channels_last=pyr_cl, cam_params_list=cams,
+                                     mean=data_batch["mean"], std=data_batch["std"], is_test=True, img_hw=(H, W),
+                                     roi=roi, prev_origin=origin)
+            origin = (roi[0], roi[1]) + frame
+            preds["fovea{}".format(j + 1)] = flow
+            preds["fovea{}_prob".format(j + 1)] = flow_prob
+            preds["fovea{}_origin".format(j + 1)] = origin
+            depth = flow
         return preds
+
+
+def _fovea_plan(fovea, H, W, isFlow, isTest):
+    """[(img_scale, inter_scale, roi, (frame_h, frame_w))] of PointMVSNet.forward's fovea argument, checked on the
+    host.  A box aligned to 8 input pixels is aligned to the sub-grid stride 8 s of every scale s."""
+    if not (isFlow and isTest):
+        raise ValueError("PointMVSNet: fovea needs isFlow and isTest (foveated inference runs after the test branch's "
+                         "whole-image iterations)")
+    try:
+        box = tuple(int(v) for v in fovea["box"])
+        scales = tuple(float(s) for s in fovea["img_scales"])
+        inters = tuple(float(s) for s in fovea["inter_scales"])
+    except (KeyError, TypeError):
+        raise ValueError("PointMVSNet: fovea must be a dict with box=(y0, x0, h, w), img_scales and inter_scales")
+    if len(box) != 4 or any(v % 8 for v in box) or box[2] <= 0 or box[3] <= 0:
+        raise ValueError("PointMVSNet: fovea box %r must be (y0, x0, h, w) in image pixels, multiples of 8" % (box,))
+    if box[0] < 0 or box[1] < 0 or box[0] + box[2] > H or box[1] + box[3] > W:
+        raise ValueError("PointMVSNet: fovea box %r outside the %dx%d image" % (box, H, W))
+    if not scales or len(scales) != len(inters):
+        raise ValueError("PointMVSNet: fovea needs one inter_scale per img_scale, got %r and %r" % (scales, inters))
+    plan = []
+    for s, isc in zip(scales, inters):
+        if s not in (0.125, 0.25, 0.5, 1.0):
+            raise ValueError("PointMVSNet: fovea img_scale %r (0.125, 0.25, 0.5 or 1.0)" % (s,))
+        plan.append((s, isc, tuple(int(v * s) for v in box), (int(H * s), int(W * s))))
+    return plan
 
 
 def _world_points(cams, D, h, w, is_test):

@@ -25,7 +25,7 @@ from torch.autograd.function import once_differentiable
 
 from . import _lib
 from . import networks
-from ._lib import lib, check, stream_ptr, ptr, require_cuda, FlowShape, FlowWeights, FlowGrads
+from ._lib import lib, check, stream_ptr, ptr, require_cuda, FlowShape, FlowWeights, FlowGrads, FlowRoi
 from .networks import EdgeConv, EdgeConvNoC
 from .nn.mlp import SharedMLP
 
@@ -42,6 +42,31 @@ def _ratio_for(image_scale, is_test):
     if image_scale in (0.25, 0.5, 1.0):
         return int(image_scale * 8)
     raise NotImplementedError("point_flow: image_scale %r (reference supports 0.125, 0.25, 0.5, 1.0)" % (image_scale,))
+
+
+def region_struct(shape, roi, prev_origin=None):
+    """The pmvs_flow_roi of a region iteration over ``shape`` (a FlowShape whose prev_h / prev_w are the previous map's
+    size).  ``roi = (y0, x0, h, w)`` in flow-grid pixels; ``prev_origin = (y0, x0, frame_h, frame_w)`` places a previous
+    map that is itself a region output in its frame (None: the previous map is the whole previous frame).  Every limit
+    (DESIGN 3.22) is checked here, by the library's own check, so a refused region raises ValueError before any launch."""
+    try:
+        vals = [int(v) for v in roi]
+    except TypeError:
+        raise ValueError("PointFlow: roi must be (y0, x0, h, w), got %r" % (roi,))
+    if len(vals) != 4:
+        raise ValueError("PointFlow: roi must be (y0, x0, h, w), got %r" % (roi,))
+    r = FlowRoi()
+    r.y0, r.x0, r.h, r.w = vals
+    if prev_origin is None:
+        r.prev_y0, r.prev_x0, r.prev_frame_h, r.prev_frame_w = 0, 0, shape.prev_h, shape.prev_w
+    else:
+        po = [int(v) for v in prev_origin]
+        if len(po) != 4:
+            raise ValueError("PointFlow: prev_origin must be (y0, x0, frame_h, frame_w), got %r" % (prev_origin,))
+        r.prev_y0, r.prev_x0, r.prev_frame_h, r.prev_frame_w = po
+    if lib.pmvs_point_flow_roi_workspace_bytes(C.byref(shape), C.byref(r)) == 0:
+        raise ValueError("PointFlow: " + lib.pmvs_last_error().decode("utf-8", "replace"))
+    return r
 
 
 class PointFlow(nn.Module):
@@ -212,8 +237,9 @@ class PointFlow(nn.Module):
         s.bn_eval = 1 if bn_eval else 0
         return s
 
-    def _workspace(self, shape, device):
-        need = lib.pmvs_point_flow_workspace_bytes(C.byref(shape))
+    def _workspace(self, shape, device, roi=None):
+        need = (lib.pmvs_point_flow_workspace_bytes(C.byref(shape)) if roi is None else
+                lib.pmvs_point_flow_roi_workspace_bytes(C.byref(shape), C.byref(roi)))
         if need == 0 or self._ws is None or self._ws.numel() < need or self._ws.device != device:
             self._ws = _lib.workspace(need, device)
         return self._ws, need
@@ -221,7 +247,7 @@ class PointFlow(nn.Module):
     # ------------------------------------------------------------------ forward
     def forward(self, estimated_depth_map, interval, image_scale, it=0, *, feature_pyramids, cam_params_list,
                 mean, std, is_test=True, img_hw=None, pyramids_channels_last=None, out=None, interval_scale=1.0,
-                sub_range=None):
+                sub_range=None, roi=None, prev_origin=None):
         """One refinement iteration (model.py:150-295).
 
         estimated_depth_map [B,1,hp,wp]; interval [B] (= inter_scale * depth_interval,
@@ -239,7 +265,17 @@ class PointFlow(nn.Module):
         are then only read.  A grad-needing eval-mode call (fine-tuning with frozen BatchNorm) needs both
         ``networks.enable_backward()`` and ``networks.enable_flow_eval_backward()``, and raises NotImplementedError
         without them; its backward fills the same gradients as in train mode, BatchNorm differentiated as the affine
-        map of the running statistics, which it leaves untouched.  A mix of modes raises RuntimeError."""
+        map of the running statistics, which it leaves untouched.  A mix of modes raises RuntimeError.
+
+        ``roi=(y0, x0, h, w)`` (foveated inference, DESIGN 3.22) runs the iteration over that rectangle of the flow grid
+        only and returns (depth [B,1,h,w], prob [B,5,h,w]); its origin in the frame is (y0, x0) of a frame of
+        int(H * image_scale) x int(W * image_scale).  ``prev_origin=(y0, x0, frame_h, frame_w)`` says that
+        ``estimated_depth_map`` is itself a region output (None: a whole map).  Inference only: a grad-enabled call, the
+        train branch (is_test=False) and ``sub_range`` raise before any launch."""
+        if roi is not None or prev_origin is not None:
+            return self._forward_roi(estimated_depth_map, interval, image_scale, feature_pyramids, cam_params_list,
+                                     mean, std, is_test, img_hw, pyramids_channels_last, out, interval_scale, sub_range,
+                                     roi, prev_origin)
         require_cuda(estimated_depth_map, interval, cam_params_list, mean, std)
         given = pyramids_channels_last if pyramids_channels_last is not None else (
             [feature_pyramids[k] for k in PYR_KEYS] if isinstance(feature_pyramids, dict) else list(feature_pyramids))
@@ -290,6 +326,34 @@ class PointFlow(nn.Module):
         return self._run(estimated_depth_map, interval, image_scale, cam_params_list, mean, std, is_test, img_hw,
                          pyr, out, interval_scale, sub_range, None, bn_eval)
 
+    def _forward_roi(self, depth, interval, image_scale, feature_pyramids, cam_params_list, mean, std, is_test,
+                     img_hw, pyramids_channels_last, out, interval_scale, sub_range, roi, prev_origin):
+        if roi is None:
+            raise ValueError("PointFlow: prev_origin is given without a roi")
+        if not is_test:
+            raise NotImplementedError("PointFlow: a region iteration runs the test branch only (is_test=True)")
+        if sub_range is not None:
+            raise NotImplementedError("PointFlow: sub_range cannot be combined with a roi")
+        given = pyramids_channels_last if pyramids_channels_last is not None else (
+            [feature_pyramids[k] for k in PYR_KEYS] if isinstance(feature_pyramids, dict) else list(feature_pyramids))
+        if torch.is_grad_enabled() and (depth.requires_grad or any(t.requires_grad for t in given) or
+                                        any(p.requires_grad for p in self.parameters())):
+            raise NotImplementedError("PointFlow: a region iteration is inference only; wrap the call in "
+                                      "torch.no_grad()")
+        require_cuda(depth, interval, cam_params_list, mean, std)
+        bn_eval = self._bn_eval(False)
+        # the region is refused before the pyramid transposes launch
+        pyr_hw = [tuple(int(v) for v in (t.shape[2:4] if pyramids_channels_last is not None else t.shape[3:5]))
+                  for t in given]
+        hw = img_hw if img_hw is not None else (pyr_hw[0][0] * 2, pyr_hw[0][1] * 2)
+        region_struct(self.make_shape(int(cam_params_list.shape[0]), int(cam_params_list.shape[1]), pyr_hw,
+                                      tuple(depth.shape[2:]), hw, image_scale, True, interval_scale, None, bn_eval),
+                      roi, prev_origin)
+        if pyramids_channels_last is None:
+            pyramids_channels_last = self.pyramids_to_channels_last(feature_pyramids)
+        return self._run(depth, interval, image_scale, cam_params_list, mean, std, True, img_hw,
+                         list(pyramids_channels_last), out, interval_scale, None, None, bn_eval, (roi, prev_origin))
+
     def _grad_params(self):
         """The 22 parameters the backward fills, in pmvs_flow_grads order."""
         ps = []
@@ -301,11 +365,11 @@ class PointFlow(nn.Module):
         return ps + [self.flow_mlp[1].weight]
 
     def _run(self, estimated_depth_map, interval, image_scale, cam_params_list, mean, std, is_test, img_hw, pyr, out,
-             interval_scale, sub_range, ctx, bn_eval=False):
+             interval_scale, sub_range, ctx, bn_eval=False, region=None):
         """The forward launches.  ctx None: the module's shared workspace; else (an autograd context) a workspace of
         the call's own, kept with what the backward reads (with bn_eval, pmvs_point_flow_eval_keep's, which also
         holds flow_mlp's activations and a copy of the running statistics).  bn_eval: BatchNorm from the running
-        statistics."""
+        statistics.  region: (roi, prev_origin) of a region iteration (pmvs_point_flow_iter_roi)."""
         dev = estimated_depth_map.device
         B, V = cam_params_list.shape[:2]
         pyr_hw = [(int(t.shape[2]), int(t.shape[3])) for t in pyr]
@@ -316,8 +380,9 @@ class PointFlow(nn.Module):
         self._validate(dev, B, V, pyr, depth, interval, mean, std, cam_params_list, bn_eval)
         shape = self.make_shape(B, V, pyr_hw, tuple(depth.shape[2:]), img_hw, image_scale, is_test, interval_scale,
                                 sub_range, bn_eval)
+        roi = None if region is None else region_struct(shape, *region)
         if ctx is None:
-            ws, need = self._workspace(shape, dev)
+            ws, need = self._workspace(shape, dev, roi)
         else:
             size = lib.pmvs_point_flow_eval_keep_workspace_bytes if bn_eval else lib.pmvs_point_flow_workspace_bytes
             need = size(C.byref(shape))
@@ -333,7 +398,7 @@ class PointFlow(nn.Module):
             w.mlp_run_var[l] = ptr(bns[3 + l].running_var) if stats else None
             w.ec_nbt[l] = ptr(bns[l].num_batches_tracked) if track else None
             w.mlp_nbt[l] = ptr(bns[3 + l].num_batches_tracked) if track else None
-        h, wd = shape.flow_h, shape.flow_w
+        h, wd = (shape.flow_h, shape.flow_w) if roi is None else (roi.h, roi.w)
         if out is None:
             depth_out = torch.empty(B, 1, h, wd, device=dev, dtype=torch.float32)
             prob_out = torch.empty(B, 5, h, wd, device=dev, dtype=torch.float32)
@@ -346,11 +411,16 @@ class PointFlow(nn.Module):
         itv = _lib.f32c(interval.detach().reshape(-1))
         mean_c, std_c = _lib.f32c(mean.detach()), _lib.f32c(std.detach())
         pyr_ptrs = (C.c_void_p * 3)(*[t.data_ptr() for t in pyr])
-        run = lib.pmvs_point_flow_eval_keep if ctx is not None and bn_eval else lib.pmvs_point_flow_iter
+        args = (C.byref(w), C.byref(pyr_ptrs), ptr(depth), ptr(cams), ptr(itv), ptr(mean_c), ptr(std_c),
+                ptr(depth_out), ptr(prob_out), ptr(ws), need, stream_ptr())
         with torch.cuda.device(dev):
-            check(run(C.byref(shape), C.byref(w), C.byref(pyr_ptrs), ptr(depth), ptr(cams), ptr(itv), ptr(mean_c),
-                      ptr(std_c), ptr(depth_out), ptr(prob_out), ptr(ws), need, stream_ptr()))
+            if roi is not None:
+                check(lib.pmvs_point_flow_iter_roi(C.byref(shape), C.byref(roi), *args))
+            else:
+                run = lib.pmvs_point_flow_eval_keep if ctx is not None and bn_eval else lib.pmvs_point_flow_iter
+                check(run(C.byref(shape), *args))
         self._last = (shape, ws, depth)  # debug_stages() recomputes the point features from `depth`
+        self._last_roi = roi
         if ctx is not None:
             ctx.fwd_tensors = (depth, pyr[0], pyr[1], pyr[2], cams, itv, mean_c, std_c, ws)
             # the weight struct points into `keep` (fp32 copies of the parameters), which must outlive the backward
@@ -399,14 +469,20 @@ class PointFlow(nn.Module):
         indexed [S, B, ...].  The fused fetch of PMVS_OPT_FETCH 3 does not write `feature`: it is recomputed here
         by the unfused fetch kernel from the workspace and the last call's previous depth map, which must not have
         been modified since.  After an eval-mode call (running statistics) there is no "h2": flow_mlp and the head run
-        in one kernel and its activations never reach memory."""
+        in one kernel and its activations never reach memory.  After a region call the sub-grid is the region's, and
+        "feature" is not recomputed: it holds what the call's fetch wrote (nothing under PMVS_OPT_FETCH 3)."""
         shape, ws, depth = self._last
+        roi = getattr(self, "_last_roi", None)
         off = (C.c_size_t * 10)()
-        check(lib.pmvs_point_flow_debug_offsets(C.byref(shape), C.byref(off)))
-        with torch.cuda.device(ws.device):
-            check(lib.pmvs_point_flow_debug_feature(C.byref(shape), ptr(depth), ptr(ws), stream_ptr()))
+        if roi is None:
+            check(lib.pmvs_point_flow_debug_offsets(C.byref(shape), C.byref(off)))
+            with torch.cuda.device(ws.device):
+                check(lib.pmvs_point_flow_debug_feature(C.byref(shape), ptr(depth), ptr(ws), stream_ptr()))
+        else:
+            check(lib.pmvs_point_flow_roi_debug_offsets(C.byref(shape), C.byref(roi), C.byref(off)))
         S = shape.sub_count if shape.sub_count > 0 else shape.ratio * shape.ratio
-        hs, wsub = shape.flow_h // shape.ratio, shape.flow_w // shape.ratio
+        gh, gw = (shape.flow_h, shape.flow_w) if roi is None else (roi.h, roi.w)
+        hs, wsub = gh // shape.ratio, gw // shape.ratio
         N = 5 * hs * wsub
         R = S * shape.B * N
 
