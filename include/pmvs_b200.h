@@ -215,6 +215,62 @@ int pmvs_consistency_filter(const float* depth, const float* cam_block, const in
                             int num_consistent, float depth_thresh, float reproj_thresh, int* count_out,
                             float* depth_avg_out, float* xyz_out, pmvs_stream_t stream);
 
+/* ---- surface reconstruction: TSDF integration, marching-cubes extraction and mesh sampling (DESIGN 3.23) ---- */
+/* The grid is dense, nx x ny x nz points; grid point (i, j, k) has linear index (i*ny + j)*nz + k and sits at
+ * X = (ox + fl(voxel*i), oy + fl(voxel*j), oz + fl(voxel*k)), each sum one fp32 rounding.  Limits of every grid:
+ * nx, ny, nz >= 2 and 3*nx*ny*nz < 2^31 (edge ids are int32).
+ *
+ * Integration: depth [V,H,W] fp32 and cam_block [V,40] as for pmvs_fuse_depth_maps; rgb [V,H,W,3] uint8 or NULL (all
+ * device memory).  For each grid point the views are taken in ascending order: (u, w, z) = project(v, X); the view
+ * counts when z > 0, 0 <= u < W, 0 <= w < H, d = depth[v, floor w, floor u] is valid (0 < d <= FLT_MAX) and
+ * sdf = fl(d - z) >= -trunc; then F = fl(F + fl(min(sdf, trunc) / trunc)), n += 1, and the pixel's RGB is added to
+ * integer sums.  tsdf_out [N] fp32 = fl(F / n), or +1 where n = 0; weight_out [N] uint16 = n; color_out [N,3] uint8
+ * = (sum + n/2) / n per channel in integers, 0 where n = 0 (NULL exactly when rgb is NULL).  Every operation is one
+ * fp32 rounding (no FMA contraction); each grid point is written once by one thread, so the volume does not depend on
+ * thread order.  Limits: 1 <= V <= 65535, H, W >= 1, V*H*W < 2^31, voxel and trunc finite and > 0, origin finite,
+ * NULL pointers refused, all PMVS_ERR_ARG before any launch.  One launch, no allocation, no synchronisation
+ * (CUDA-graph capturable). */
+int pmvs_tsdf_integrate(const float* depth, const float* cam_block, const unsigned char* rgb, int V, int H, int W,
+                        int nx, int ny, int nz, float ox, float oy, float oz, float voxel, float trunc,
+                        float* tsdf_out, unsigned short* weight_out, unsigned char* color_out, pmvs_stream_t stream);
+/* Marching cubes over a volume (tsdf, weight, color as pmvs_tsdf_integrate writes them; color may be NULL, and then
+ * colors_out must be NULL too; with color, colors_out may be NULL only when nv = 0).  A grid
+ * point is observed when weight >= min_weight (1 <= min_weight <= 65535); cube (i, j, k) with i < nx-1, j < ny-1,
+ * k < nz-1 is active when its 8 corners are observed; a corner is inside when tsdf < 0.  The triangles of each case
+ * come from the generated table csrc/mc_table.cuh (utils/mc_table.py): counter-clockwise seen from outside (tsdf > 0),
+ * at most 5 per cube, and two cubes sharing a face draw the same segments on it.  Edge id 3g + a is the edge from grid
+ * point g along axis a; it carries a vertex when an active cube cuts it, at t = fl(f0 / fl(f0 - f1)) (f0 the tsdf at g,
+ * f1 at the other end): the axis coordinate is fl(o_a + fl(voxel * fl(i_a + t))), the other two are g's, and the
+ * colour is rintf(fl(c0 + fl(t * fl(c1 - c0)))) per channel.  Vertices come in ascending edge id; faces [NF,3] int32
+ * vertex indices in ascending cube index and, within a cube, in table order.
+ * Protocol: pmvs_tsdf_mesh_count writes counts_out[0] = NV and counts_out[1] = NF (int64, device memory) and leaves
+ * its state in the workspace; the caller reads the counts, sizes the outputs and calls pmvs_tsdf_mesh_emit with the
+ * same volume, min_weight and workspace, and nv, nf the counts (writes beyond them are skipped).  workspace:
+ * pmvs_tsdf_mesh_workspace_bytes(nx, ny, nz) bytes (about 12 per grid point), 256-byte aligned, device memory.
+ * count: four operations (memset + three launches); emit: two launches; no allocation, no synchronisation.  Argument
+ * errors (the grid limits, NULL pointers, min_weight, voxel and origin finite, the workspace) are PMVS_ERR_ARG or
+ * PMVS_ERR_WORKSPACE before any launch. */
+size_t pmvs_tsdf_mesh_workspace_bytes(int nx, int ny, int nz); /* 0 + pmvs_last_error on a bad shape */
+int pmvs_tsdf_mesh_count(const float* tsdf, const unsigned short* weight, int nx, int ny, int nz, int min_weight,
+                         long long* counts_out, void* workspace, size_t workspace_bytes, pmvs_stream_t stream);
+int pmvs_tsdf_mesh_emit(const float* tsdf, const unsigned short* weight, const unsigned char* color, int nx, int ny,
+                        int nz, float ox, float oy, float oz, float voxel, int min_weight, long long nv, long long nf,
+                        float* vertices_out, unsigned char* colors_out, int* faces_out, void* workspace,
+                        size_t workspace_bytes, pmvs_stream_t stream);
+/* Dense sampling of a triangle mesh: vertices [nv,3] fp32, faces [nf,3] int32 (device memory).  For each face ABC in
+ * order: n = max(1, ceil(fl(sqrt(L2) / dst))) with L2 the largest squared side ((dx*dx + dy*dy) + dz*dz, each side
+ * fl(B - A) per coordinate), at most 1024 (1 when the quotient is NaN); the points A + fl(i/n) (B - A) + fl(j/n) (C - A)
+ * for i, j >= 0, i + j <= n, in ascending (i, j), each operation one fp32 rounding, summed left to right.  A face
+ * with an index outside [0, nv) yields no points (the library cannot read faces on the host; utils/surface.py refuses
+ * such faces).  count writes the total (int64, device memory); emit writes points_out [n,3] (writes beyond n are
+ * skipped).  dst finite > 0, nv, nf >= 0.  workspace: pmvs_mesh_sample_workspace_bytes(nf) bytes, 256-byte aligned,
+ * device memory, the same for both calls. */
+size_t pmvs_mesh_sample_workspace_bytes(int nf); /* 0 + pmvs_last_error on a bad shape */
+int pmvs_mesh_sample_count(const float* vertices, int nv, const int* faces, int nf, float dst, long long* count_out,
+                           void* workspace, size_t workspace_bytes, pmvs_stream_t stream);
+int pmvs_mesh_sample_emit(const float* vertices, int nv, const int* faces, int nf, float dst, long long n,
+                          float* points_out, void* workspace, size_t workspace_bytes, pmvs_stream_t stream);
+
 /* ---- point-cloud evaluation (DESIGN 3.11): accuracy / completeness of a fused cloud against a reference scan ---- */
 /* The library's own DTU-style rule, not claimed to reproduce the DTU MATLAB evaluation's numbers.  xyz arrays are
  * [n,3] fp32 device memory; a point with a non-finite coordinate is never kept by thinning and is nobody's neighbour.

@@ -166,6 +166,13 @@ _sig("pmvs_depth_loss_backward", I, [C.POINTER(DepthTerms), P, I, I, P, I, I, P,
 _sig("pmvs_prepare_views_workspace_bytes", C.c_size_t, [I, I, I, I, C.c_double, I, I, I, I])
 _sig("pmvs_prepare_views", I, [P, I, I, I, I, C.c_double, I, I, I, I, P, P, P, C.c_size_t, P])
 _sig("pmvs_probability_filter_workspace_bytes", C.c_size_t, [I, I, I, I, I, I, I, I])
+_sig("pmvs_tsdf_integrate", I, [P, P, P, I, I, I, I, I, I, F, F, F, F, F, P, P, P, P])
+_sig("pmvs_tsdf_mesh_workspace_bytes", C.c_size_t, [I, I, I])
+_sig("pmvs_tsdf_mesh_count", I, [P, P, I, I, I, I, P, P, C.c_size_t, P])
+_sig("pmvs_tsdf_mesh_emit", I, [P, P, P, I, I, I, F, F, F, F, I, LL, LL, P, P, P, P, C.c_size_t, P])
+_sig("pmvs_mesh_sample_workspace_bytes", C.c_size_t, [I])
+_sig("pmvs_mesh_sample_count", I, [P, I, P, I, F, P, P, C.c_size_t, P])
+_sig("pmvs_mesh_sample_emit", I, [P, I, P, I, F, LL, P, P, C.c_size_t, P])
 _sig("pmvs_probability_filter", I, [P, P, P, I, I, I, I, I, I, I, F, F, I, P, C.c_size_t, P, P, C.c_size_t, P])
 
 EXPORTED = [
@@ -187,6 +194,8 @@ EXPORTED = [
     "pmvs_point_flow_backward_debug_offsets", "pmvs_prepare_views_workspace_bytes", "pmvs_prepare_views",
     "pmvs_probability_filter_workspace_bytes", "pmvs_probability_filter", "pmvs_consistency_filter",
     "pmvs_point_flow_roi_workspace_bytes", "pmvs_point_flow_iter_roi", "pmvs_point_flow_roi_debug_offsets",
+    "pmvs_tsdf_integrate", "pmvs_tsdf_mesh_workspace_bytes", "pmvs_tsdf_mesh_count", "pmvs_tsdf_mesh_emit",
+    "pmvs_mesh_sample_workspace_bytes", "pmvs_mesh_sample_count", "pmvs_mesh_sample_emit",
 ]
 
 

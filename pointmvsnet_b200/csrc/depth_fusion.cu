@@ -18,17 +18,6 @@ namespace {
 // consistency bits are kept per chunk of 32 source views, one word per pixel and chunk
 constexpr int FUSE_CHUNK = 32;
 
-// Step 1 of the check: the pixel of view j that X lands on, or false when it is behind j or off its image.
-__device__ __forceinline__ bool land(const float* __restrict__ cbj, float X0, float X1, float X2, int H, int W,
-                                     float& z, int& xq, int& yq) {
-  float u, w;
-  project(cbj, X0, X1, X2, u, w, z);
-  if (!(z > 0.f && u >= 0.f && u < (float)W && w >= 0.f && w < (float)H)) return false;
-  xq = min((int)floorf(u), W - 1);  // u < fl(W) already implies floor(u) <= W - 1; the min only guards the gather
-  yq = min((int)floorf(w), H - 1);
-  return true;
-}
-
 __global__ void __launch_bounds__(256)
     fuse_view_kernel(const float* __restrict__ depth, const float* __restrict__ cams, int r, int V, int H, int W,
                      int num_consistent, float depth_thresh, float reproj_thresh, int* __restrict__ count_out,
